@@ -28,11 +28,20 @@ def nvcc():
     return 'nvcc'
 
 
-def _run(cmd, verbose):
+def _run(cmd, verbose, res=None):
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('nvcc failed: %s\n%s' % (' '.join(cmd), r.stderr[-6000:]))
+    if res:   # the assembler's resource report of a step instance (registers, stack frame, spill bytes per function), kept beside its object
+        with open(res, 'w') as f:
+            f.write(r.stderr)
     return r.stderr if verbose else ''
+
+
+def res_path(obj):
+    """the resource report written beside a step instance's object file, or None for the other objects."""
+    name = os.path.basename(obj)
+    return obj[:-2] + '.res' if name.startswith('step_') and name.endswith('.o') else None
 
 
 def build(force=False, verbose=False, out=None):
@@ -42,13 +51,13 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES:
-        jobs.append([nvcc()] + ARCH + ptx + ['-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
+    for tag, real, dr, feat in INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+        jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])
     jobs.append([nvcc()] + ARCH + ['-c', os.path.join(CSRC, 'mjcf.cpp'), '-o', os.path.join(OBJ, 'mjcf.o')])
     with ThreadPoolExecutor(max_workers=max(2, min(len(jobs), (os.cpu_count() or 4)))) as ex:
-        logs = list(ex.map(lambda c: _run(c, verbose), jobs))
+        logs = list(ex.map(lambda c: _run(c, verbose, res_path(c[-1])), jobs))
     if verbose:
         sys.stderr.write(''.join(logs))
     objs = [j[-1] for j in jobs]

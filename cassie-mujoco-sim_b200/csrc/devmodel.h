@@ -167,7 +167,7 @@ constexpr int S_QLD = S_CDOF + 192;             // [320] (qM itself lives in a g
 constexpr int S_DINV = S_QLD + NM_MAX;          // [32]
 constexpr int S_DSQI = S_DINV + 32;             // [32]
 constexpr int S_QPOS = S_DSQI + 32;             // [44]
-constexpr int S_VEC = S_QPOS + 44;              // [6][32] general vectors ([96..127]: IMU stash; [128..159]: exchange buffer; [160..183]: extra-body qvel / qacc_smooth / qacc_ws / qacc)
+constexpr int S_VEC = S_QPOS + 44;              // [6][32] general vectors ([96..127]: IMU stash; [128..159]: exchange buffer; [160..183]: extra-body qvel / qacc_smooth / qacc_ws / qacc; [184..186]: centre of mass)
 constexpr int S_CON = S_VEC + 192;              // [MAXCON][16]
 constexpr int S_EFC = S_CON + MAXCON * 16;               // [NEFC][4]: row-build scalars {.., pos, src, ineq} then solver constants {b, 1/A, A, +-R}
 constexpr int S_Y = S_EFC + 4 * NEFC;           // [NEFC][ystride] constraint matrix; before the constraint stage it holds the temporaries below
@@ -181,7 +181,10 @@ constexpr int T_CVEL = 640;                     // [32][6]
 constexpr int T_CFRC = 832;                     // [32][6]
 constexpr int T_CDOFD = 1024;                   // [32][6]
 constexpr int T_GEOM = 1216;                    // [16][12] geom world poses (position + rotation by columns), live from the collision stage until the contact list is written
+constexpr int T_CBUF = 0;                       // [4 x 7][32] collision: the contacts of each lane's candidate pair, [pos3 normal3 dist] each, lane index fastest
+constexpr int T_CSORT = 0;                      // [MAXCON][16] after the collision passes: the unsorted contact list while it is put back into MuJoCo's order
 static_assert(T_GEOM + 192 <= NEFC * YSTRIDE_MAIN, "temporaries must fit in the constraint-matrix region");
+static_assert(T_CBUF + 28 * 32 <= T_GEOM && T_CSORT + 16 * MAXCON <= T_GEOM, "the collision buffers must not overlap the geom poses");
 static_assert(NEFC >= 48 && 16 * YSTRIDE_MAX <= S_QLD - S_XPOS, "the dense solver path keeps A in rows 32..47 of Y and in the kinematics buffers");
 // slots of a row's 4 scalars while the rows are being built (overwritten by the solver constants afterwards)
 constexpr int E_POS = 0, E_SRC = 1, E_INEQ = 2, E_SIDE = 3;   // E_SIDE: 0 / 1 the row touches the base and at most the first leg, 2 ... the second leg, 3 both legs
