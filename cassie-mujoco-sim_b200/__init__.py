@@ -201,6 +201,14 @@ def lib():
             f.restype = ci
     L.cassie_batch_set_const.argtypes = [vp, C.c_void_p, ci]
     L.cassie_batch_set_const.restype = ci
+    L.cassie_batch_set_geom_pose.argtypes = [vp, C.c_char_p, cd, cd, cd]
+    L.cassie_batch_set_geom_pose.restype = ci
+    L.cassie_batch_set_env_geom_pose.argtypes = [vp, C.c_char_p, cd, cd, cd, C.c_void_p]
+    L.cassie_batch_set_env_geom_pose.restype = ci
+    L.cassie_batch_get_env_geom_pose.argtypes = [vp, C.c_char_p, cd, cd, cd]
+    L.cassie_batch_get_env_geom_pose.restype = ci
+    L.cassie_batch_clear_env_geom_poses.argtypes = [vp]
+    L.cassie_batch_clear_env_geom_poses.restype = ci
     L.cassie_sim_params.argtypes = [vp, C.POINTER(ci)]
     for n in ('cassie_sim_dof_damping', 'cassie_sim_body_mass', 'cassie_sim_body_ipos', 'cassie_sim_geom_friction'):
         getattr(L, n).argtypes = [vp]
@@ -414,6 +422,35 @@ class CassieBatch:
         """mj_setConst on the device for the masked environments (all if None); reset_state=True adds cassie_sim_set_const's state reset."""
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
         if self.L.cassie_batch_set_const(self.h, None if m is None else m.ctypes.data_as(C.c_void_p), 1 if reset_state else 0) != 0:
+            raise RuntimeError(_last_error())
+
+    # ---- placement of static geoms (stairs, floor tilt; reference: src/cassiemujoco.c:1466-1541, example/test_terrain.c:118-157)
+    def set_geom_pose(self, name, pos=None, quat=None, size=None):
+        """one placement shared by every environment: pos [3] / quat [4] in the geom's body frame, size [3]; None leaves that part alone.  As in
+        MuJoCo a new size leaves the bounding radius alone.  Per-environment rows, if any, take this placement for the geom."""
+        a = [None if v is None else np.ascontiguousarray(v, dtype=np.float64).reshape(w) for v, w in ((pos, 3), (quat, 4), (size, 3))]
+        if self.L.cassie_batch_set_geom_pose(self.h, name.encode(), *[None if v is None else self._dp(v) for v in a]) != 0:
+            raise RuntimeError(_last_error())
+
+    def set_env_geom_pose(self, name, pos=None, quat=None, size=None, mask=None):
+        """per-environment placement of a static plane / box: pos [3] or [n, 3], quat [4] or [n, 4], size [3] or [n, 3] (broadcast over the
+        environments; None leaves that part alone); mask [n]: only the selected environments change.  A box's bounding radius follows |size|."""
+        a = [None if v is None else np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n, w))) for v, w in ((pos, 3), (quat, 4), (size, 3))]
+        m = None if mask is None else np.ascontiguousarray(np.broadcast_to(np.asarray(mask, dtype=np.uint8), (self.n,)))
+        if self.L.cassie_batch_set_env_geom_pose(self.h, name.encode(), *[None if v is None else self._dp(v) for v in a],
+                                                 None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_geom_pose(self, name):
+        """(pos [n, 3], quat [n, 4], size [n, 3]): the placement of a static plane / box each environment sees"""
+        pos, quat, size = np.zeros((self.n, 3)), np.zeros((self.n, 4)), np.zeros((self.n, 3))
+        if self.L.cassie_batch_get_env_geom_pose(self.h, name.encode(), self._dp(pos), self._dp(quat), self._dp(size)) != 0:
+            raise RuntimeError(_last_error())
+        return pos, quat, size
+
+    def clear_env_geom_poses(self):
+        """drop the per-environment placements: every environment follows the shared placement again"""
+        if self.L.cassie_batch_clear_env_geom_poses(self.h) != 0:
             raise RuntimeError(_last_error())
 
     def query(self):

@@ -18,6 +18,10 @@ DEPS = [os.path.join(CSRC, f) for f in ('cassie_b200.cu', 'mjcf.cpp', 'step_inst
 INSTANCES = [('f00', 'float', 0, 0), ('f10', 'float', 1, 0), ('f02', 'float', 0, 2), ('f12', 'float', 1, 2), ('f04', 'float', 0, 4), ('f14', 'float', 1, 4), ('f05', 'float', 0, 5), ('f15', 'float', 1, 5),
              ('f07', 'float', 0, 7), ('f17', 'float', 1, 7), ('d07', 'double', 0, 7), ('d17', 'double', 1, 7),
              ('f20', 'float', 2, 0), ('f22', 'float', 2, 2), ('f24', 'float', 2, 4), ('f25', 'float', 2, 5), ('f27', 'float', 2, 7), ('d27', 'double', 2, 7)]
+# the same kernel with the static geoms' placement read from per-environment rows (feature 8 = F_EG; cassie_batch_set_env_geom_pose): boxes (also for
+# models without boxes, floor tilt only) or every feature, in each instance kind; the tag's last digit is the feature set in hex
+ENV_GEOM_INSTANCES = [('f0c', 'float', 0, 12), ('f1c', 'float', 1, 12), ('f2c', 'float', 2, 12), ('f0f', 'float', 0, 15), ('f1f', 'float', 1, 15), ('f2f', 'float', 2, 15),
+                      ('d0f', 'double', 0, 15), ('d1f', 'double', 1, 15), ('d2f', 'double', 2, 15)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -51,7 +55,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

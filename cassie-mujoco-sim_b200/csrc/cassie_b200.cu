@@ -25,12 +25,21 @@
 CASSIE_STEP_ENTRY(f00) CASSIE_STEP_ENTRY(f10) CASSIE_STEP_ENTRY(f02) CASSIE_STEP_ENTRY(f12) CASSIE_STEP_ENTRY(f04) CASSIE_STEP_ENTRY(f14) CASSIE_STEP_ENTRY(f05) CASSIE_STEP_ENTRY(f15) CASSIE_STEP_ENTRY(f07) CASSIE_STEP_ENTRY(f17)
 CASSIE_STEP_ENTRY(d07) CASSIE_STEP_ENTRY(d17)
 CASSIE_STEP_ENTRY(f20) CASSIE_STEP_ENTRY(f22) CASSIE_STEP_ENTRY(f24) CASSIE_STEP_ENTRY(f25) CASSIE_STEP_ENTRY(f27) CASSIE_STEP_ENTRY(d27)
+CASSIE_STEP_ENTRY(f0c) CASSIE_STEP_ENTRY(f1c) CASSIE_STEP_ENTRY(f2c) CASSIE_STEP_ENTRY(f0f) CASSIE_STEP_ENTRY(f1f) CASSIE_STEP_ENTRY(f2f)
+CASSIE_STEP_ENTRY(d0f) CASSIE_STEP_ENTRY(d1f) CASSIE_STEP_ENTRY(d2f)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_EG) {   // per-environment static-geom rows: F_BOX | F_EG covers models with at most boxes (a floor without boxes too), F_ALL | F_EG the rest
+    const bool box = !std::is_same<real, double>::value && (feat & ~(F_BOX | F_EG)) == 0;
+    if (compiled_feat) *compiled_feat = box ? (F_BOX | F_EG) : (F_ALL | F_EG);
+    if (std::is_same<real, double>::value) return inst == 1 ? cassie_step_entry_d1f() : (inst == 2 ? cassie_step_entry_d2f() : cassie_step_entry_d0f());
+    if (box) return inst == 1 ? cassie_step_entry_f1c() : (inst == 2 ? cassie_step_entry_f2c() : cassie_step_entry_f0c());
+    return inst == 1 ? cassie_step_entry_f1f() : (inst == 2 ? cassie_step_entry_f2f() : cassie_step_entry_f0f());
+  }
   int f = F_ALL;
   if (!std::is_same<real, double>::value) { if (feat == 0) f = 0; else if (feat == F_HFIELD) f = F_HFIELD; else if (feat == F_BOX) f = F_BOX; else if ((feat & ~(F_XB | F_BOX)) == 0) f = F_XB | F_BOX; }
   if (compiled_feat) *compiled_feat = f;
@@ -223,6 +232,11 @@ struct BatchBase {
   virtual bool snap_set(const Snap *snap, const unsigned char *mask) = 0;
   virtual bool copy_model_from(BatchBase *src) = 0;     // per-environment constants, height fields, timestep (mj_copyModel in cassie_sim_copy, :1083-1091)
   virtual bool rebuild_model() = 0;                     // after hm was edited (timestep, hold / release): rebuild and upload the constant block
+  // per-environment placement of static planes / boxes (GEOM_ENV_W rows): pos / quat / size [n][3] / [n][4] / [n][3] or null (that part unchanged)
+  virtual bool set_env_geom(int g, const double *pos, const double *quat, const double *size, const unsigned char *mask) = 0;
+  virtual bool get_env_geom(int g, double *pos, double *quat, double *size) = 0;
+  virtual bool clear_env_geoms() = 0;
+  virtual bool shared_geom_changed(int g) = 0;          // after the shared placement of geom g was rebuilt: its slot in every row follows it
   int nsub_override = 0;                                // > 0: physics sub-steps per control tick of the next launches (cassie_sim_step_pd_no2khz)
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
 };
@@ -239,8 +253,11 @@ template <typename real> struct Batch : BatchBase {
   cudaStream_t aos_stream[AOS_MAXC] = {};                              // their streams
   bool task_from_aos = false;   // the task-PD rows were created by the AoS entry point's forwarding (not by cassie_batch_set_task_pd)
   float *d_hfield = nullptr; unsigned char *d_mask = nullptr; DevModel<real> h_model_copy{}; int geom_dev[256]; void *d_row = nullptr;
+  real *d_genv = nullptr;                  // A.genv: [n][GEOM_ENV_W] per-environment static-geom placement, allocated by the first per-environment placement
+  std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   ~Batch() override {
     cudaSetDevice(device);
+    cudaFree(d_genv);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -302,6 +319,7 @@ template <typename real> struct Batch : BatchBase {
       int per_sm = 0;
       { const void *entry = step_entry<real>(ext, feat);
         CUDA_OK(cudaFuncSetAttribute(entry, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+        CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, feat | F_EG), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // same scratch, same shape
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -631,12 +649,83 @@ template <typename real> struct Batch : BatchBase {
     if (!rebuild_model()) return false;
     if (src->A.cenv) { if (!ensure_cenv()) return false; CUDA_OK(cudaMemcpyAsync(A.cenv, src->A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToDevice, stream)); }
     else if (A.cenv) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; }
+    if (src->d_genv) { if (!ensure_genv()) return false; CUDA_OK(cudaMemcpyAsync(d_genv, src->d_genv, sizeof(real) * n * GEOM_ENV_W, cudaMemcpyDeviceToDevice, stream)); }
+    else if (!clear_env_geoms()) return false;
+    for (int k = 0; k < MGS; k++) ge_host[k] = src->ge_host[k];
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
       std::vector<float> tmp(cells); CUDA_OK(cudaMemcpy(tmp.data(), src->d_hfield, sizeof(float) * cells, cudaMemcpyDeviceToHost));
       if (!set_hfield(tmp.data(), src->A.n_terrain)) return false;
     }
     return sync();
+  }
+  // ---- per-environment placement of the static planes / boxes (stairs and slopes that differ between environments)
+  bool ensure_genv() {
+    if (d_genv) return true;
+    CUDA_OK(cudaSetDevice(device));
+    std::vector<real> row(GEOM_ENV_W), all((size_t)n * GEOM_ENV_W); init_genv_row(h_model_copy, row.data());
+    for (int e = 0; e < n; e++) memcpy(&all[(size_t)e * GEOM_ENV_W], row.data(), sizeof(real) * GEOM_ENV_W);
+    CUDA_OK(cudaMalloc(&d_genv, sizeof(real) * n * GEOM_ENV_W));
+    CUDA_OK(cudaMemcpyAsync(d_genv, all.data(), sizeof(real) * n * GEOM_ENV_W, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    A.genv = d_genv;
+    return true;
+  }
+  // slot k of every row <- slots[n][GE_SLOT]: one strided copy, the rest of the rows is not moved
+  bool put_genv_slot(int k, const std::vector<real> &slots) {
+    CUDA_OK(cudaMemcpy2DAsync(d_genv + GE_SLOT * k, sizeof(real) * GEOM_ENV_W, slots.data(), sizeof(real) * GE_SLOT, sizeof(real) * GE_SLOT, n, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  std::vector<double> &ge_mirror(int g, int k) {   // the body-frame placement every environment sees; starts as the shared one
+    std::vector<double> &h = ge_host[k];
+    if (h.empty()) { h.resize((size_t)n * 10);
+      for (int e = 0; e < n; e++) { double *r = &h[(size_t)e * 10]; for (int c = 0; c < 3; c++) { r[c] = hm.geom_pos[3 * g + c]; r[7 + c] = hm.geom_size[3 * g + c]; } for (int c = 0; c < 4; c++) r[3 + c] = hm.geom_quat[4 * g + c]; } }
+    return h;
+  }
+  bool set_env_geom(int g, const double *pos, const double *quat, const double *size, const unsigned char *mask) override {
+    std::string err; const int k = env_geom_check(hm, geom_dev, g, err);
+    if (k < 0) { set_err("cassie_batch_set_env_geom_pose: " + err); return false; }
+    if (!ensure_genv()) return false;
+    // the selected environments' slots from their new placement; the others keep the slot they have (read back: 64 B per environment)
+    std::vector<real> slots((size_t)n * GE_SLOT);
+    CUDA_OK(cudaMemcpy2DAsync(slots.data(), sizeof(real) * GE_SLOT, d_genv + GE_SLOT * k, sizeof(real) * GEOM_ENV_W, sizeof(real) * GE_SLOT, n, cudaMemcpyDeviceToHost, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    std::vector<double> &h = ge_mirror(g, k);
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      double *r = &h[(size_t)e * 10];
+      if (pos) for (int c = 0; c < 3; c++) r[c] = pos[(size_t)e * 3 + c];
+      if (quat) for (int c = 0; c < 4; c++) r[3 + c] = quat[(size_t)e * 4 + c];
+      if (size) for (int c = 0; c < 3; c++) r[7 + c] = size[(size_t)e * 3 + c];
+      env_geom_slot(hm, g, r, r + 3, r + 7, &slots[(size_t)e * GE_SLOT]);
+    }
+    return put_genv_slot(k, slots);
+  }
+  bool get_env_geom(int g, double *pos, double *quat, double *size) override {
+    std::string err; const int k = env_geom_check(hm, geom_dev, g, err);
+    if (k < 0) { set_err("cassie_batch_get_env_geom_pose: " + err); return false; }
+    for (int e = 0; e < n; e++) {
+      const double *r = ge_host[k].empty() ? nullptr : &ge_host[k][(size_t)e * 10];
+      for (int c = 0; c < 3; c++) { if (pos) pos[(size_t)e * 3 + c] = r ? r[c] : hm.geom_pos[3 * g + c]; if (size) size[(size_t)e * 3 + c] = r ? r[7 + c] : hm.geom_size[3 * g + c]; }
+      if (quat) for (int c = 0; c < 4; c++) quat[(size_t)e * 4 + c] = r ? r[3 + c] : hm.geom_quat[4 * g + c];
+    }
+    return true;
+  }
+  bool clear_env_geoms() override {
+    for (int k = 0; k < MGS; k++) ge_host[k].clear();
+    if (!d_genv) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_genv)); d_genv = nullptr; A.genv = nullptr;
+    return true;
+  }
+  bool shared_geom_changed(int g) override {
+    const int k = g >= 0 && g < hm.ngeom ? geom_dev[g] - MG : -1;
+    if (k < 0 || k >= MGS) return true;
+    ge_host[k].clear();
+    if (!d_genv) return true;
+    std::vector<real> row(GEOM_ENV_W), slots((size_t)n * GE_SLOT); init_genv_row(h_model_copy, row.data());
+    for (int e = 0; e < n; e++) memcpy(&slots[(size_t)e * GE_SLOT], &row[GE_SLOT * k], sizeof(real) * GE_SLOT);
+    return put_genv_slot(k, slots);
   }
   // open-loop sinusoidal gait on the motor-PD targets (BASELINE config 5 "random PD gaits"): evaluated in the kernel every control tick, so
   // multi-tick launches follow it without a host round trip; installing it restarts the tick clock
@@ -663,7 +752,7 @@ template <typename real> struct Batch : BatchBase {
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
-      CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, feat), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
+      CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, A.genv ? feat | F_EG : feat), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
     CUDA_OK(cudaGetLastError());
     return true;
@@ -994,8 +1083,16 @@ int cassie_batch_set_geom_pose(cassie_batch_t *b, const char *name, const double
   if (pos) for (int k = 0; k < 3; k++) hm.geom_pos[3 * g + k] = pos[k];
   if (quat) for (int k = 0; k < 4; k++) hm.geom_quat[4 * g + k] = quat[k];
   if (size) for (int k = 0; k < 3; k++) hm.geom_size[3 * g + k] = size[k];
-  return b->impl->rebuild_model() ? 0 : -1;
+  return b->impl->rebuild_model() && b->impl->shared_geom_changed(g) ? 0 : -1;   // per-environment rows, if any, take the shared placement of this geom
 }
+// per-environment placement of a static plane / box (extends src/cassiemujoco.c:1466-1541 to one placement per environment); see include/cassie_b200.h
+int cassie_batch_set_env_geom_pose(cassie_batch_t *b, const char *name, const double *pos, const double *quat, const double *size, const unsigned char *mask) {
+  return b->impl->set_env_geom(b->impl->hm.geom_id(name ? name : ""), pos, quat, size, mask) ? 0 : -1;
+}
+int cassie_batch_get_env_geom_pose(cassie_batch_t *b, const char *name, double *pos, double *quat, double *size) {
+  return b->impl->get_env_geom(b->impl->hm.geom_id(name ? name : ""), pos, quat, size) ? 0 : -1;
+}
+int cassie_batch_clear_env_geom_poses(cassie_batch_t *b) { return b->impl->clear_env_geoms() ? 0 : -1; }
 
 // ---- legacy verbs RL wrappers call around cassie_sim_step_pd (src/cassiemujoco.c:1072-1093, 1137-1145, 1159-1181, 1196-1225, 1974-2000, 2086-2092, 3380-3452)
 // the dynamic subset of cassie_out_t from an observation row, the rest as cassie_out_init leaves it (:672-734)

@@ -21,6 +21,49 @@ inline void q2m_d(double *m, const double *q) {
 }
 }  // namespace detail
 
+// world pose of geom g on a static body (the world or a body welded to it) with its frame in the body given by pos / quat (MuJoCo's geom_pos /
+// geom_quat), in the layout the collision stage reads: position, then the z, x and y axes of the geom frame.  The chain of static bodies is constant.
+inline void static_geom_wpose(const HostModel &m, int g, const double *pos, const double *quat, double *w) {
+  double R[9]; detail::q2m_d(R, quat);
+  double bp[3] = {0, 0, 0}, bq[4] = {1, 0, 0, 0};
+  { std::vector<int> chain; for (int bb = m.geom_bodyid[g]; bb > 0; bb = m.body_parentid[bb]) chain.push_back(bb);
+    for (int i = (int)chain.size() - 1; i >= 0; i--) { const int bb = chain[i]; double Rb[9], v[3]; detail::q2m_d(Rb, bq);
+      for (int r = 0; r < 3; r++) v[r] = Rb[3 * r] * m.body_pos[3 * bb] + Rb[3 * r + 1] * m.body_pos[3 * bb + 1] + Rb[3 * r + 2] * m.body_pos[3 * bb + 2];
+      for (int r = 0; r < 3; r++) bp[r] += v[r];
+      const double *q2 = &m.body_quat[4 * bb]; const double t[4] = {bq[0] * q2[0] - bq[1] * q2[1] - bq[2] * q2[2] - bq[3] * q2[3], bq[0] * q2[1] + bq[1] * q2[0] + bq[2] * q2[3] - bq[3] * q2[2],
+                                                                    bq[0] * q2[2] - bq[1] * q2[3] + bq[2] * q2[0] + bq[3] * q2[1], bq[0] * q2[3] + bq[1] * q2[2] - bq[2] * q2[1] + bq[3] * q2[0]};
+      for (int r = 0; r < 4; r++) bq[r] = t[r]; } }
+  double Rb[9], W[9], wp[3]; detail::q2m_d(Rb, bq);
+  for (int r = 0; r < 3; r++) { wp[r] = bp[r] + Rb[3 * r] * pos[0] + Rb[3 * r + 1] * pos[1] + Rb[3 * r + 2] * pos[2];
+    for (int c = 0; c < 3; c++) W[3 * r + c] = Rb[3 * r] * R[c] + Rb[3 * r + 1] * R[3 + c] + Rb[3 * r + 2] * R[6 + c]; }
+  for (int r = 0; r < 3; r++) { w[r] = wp[r]; w[3 + r] = W[3 * r + 2]; w[6 + r] = W[3 * r]; w[9 + r] = W[3 * r + 1]; }   // position, z, x, y axes
+}
+
+// one slot of a per-environment static-geom row (GEOM_ENV_W): geom g placed at pos / quat (in its body frame) with size `size`.  A box's bounding radius
+// is recomputed as |size| so that a box enlarged beyond its file size is not culled by a stale bound; a plane keeps the model's (0)
+template <typename real> void env_geom_slot(const HostModel &m, int g, const double *pos, const double *quat, const double *size, real *slot) {
+  double w[12]; static_geom_wpose(m, g, pos, quat, w);
+  for (int c = 0; c < 12; c++) slot[GE_POSE + c] = (real)w[c];
+  for (int c = 0; c < 3; c++) slot[GE_SIZE + c] = (real)size[c];
+  slot[GE_RBOUND] = m.geom_type[g] == GEOM_BOX ? (real)std::sqrt(size[0] * size[0] + size[1] * size[1] + size[2] * size[2]) : (real)m.geom_rbound[g];
+}
+// a row holding the model block's own placement of every static slot
+template <typename real> void init_genv_row(const DevModel<real> &d, real *row) {
+  for (int k = 0; k < MGS; k++) { real *s = row + GE_SLOT * k;
+    for (int c = 0; c < 12; c++) s[GE_POSE + c] = d.geom_wpose[k][c];
+    for (int c = 0; c < 3; c++) s[GE_SIZE + c] = d.geom_size[MG + k][c];
+    s[GE_RBOUND] = d.geom_rbound[MG + k]; }
+}
+// the static collision slot (0 .. MGS-1) of host geom g, or a reason why it has none that a per-environment placement could move
+inline int env_geom_check(const HostModel &m, const int *geom_dev, int g, std::string &err) {
+  if (g < 0 || g >= m.ngeom) { err = "unknown geom"; return -1; }
+  if (m.body_weldid[m.geom_bodyid[g]] != 0) { err = "the geom is on a moving body"; return -1; }
+  if (m.geom_type[g] == GEOM_HFIELD) { err = "the height field's placement is shared by the batch"; return -1; }
+  if (geom_dev[g] < MG) { err = "the geom has no collision slot (visual only)"; return -1; }
+  if (m.geom_type[g] != GEOM_PLANE && m.geom_type[g] != GEOM_BOX) { err = "only planes and boxes can be placed per environment"; return -1; }
+  return geom_dev[g] - MG;
+}
+
 struct BuildInfo { int unsupported_pairs = 0; int collision_geoms = 0; int geom_dev[256]; BuildInfo() { for (int i = 0; i < 256; i++) geom_dev[i] = -1; } };   // geom_dev: host geom id -> collision geom slot of the device block
 
 template <typename real>
@@ -190,19 +233,8 @@ bool build_dev_model(const HostModel &m, DevModel<real> &d, std::string &err, Bu
       for (int c = 0; c < 9; c++) d.geom_mat[k][c] = (real)R[c];
       if (b != xb) { const double *gp = &m.geom_pos[3 * g]; robot_reach = std::max(robot_reach, reach[b] + std::sqrt(gp[0] * gp[0] + gp[1] * gp[1] + gp[2] * gp[2]) + m.geom_rbound[g]); }
     } else {   // world pose: compose the (constant) chain of static bodies
-      double bp[3] = {0, 0, 0}, bq[4] = {1, 0, 0, 0};
-      { std::vector<int> chain; for (int bb = b; bb > 0; bb = m.body_parentid[bb]) chain.push_back(bb);
-        for (int i = (int)chain.size() - 1; i >= 0; i--) { const int bb = chain[i]; double Rb[9], v[3]; detail::q2m_d(Rb, bq);
-          for (int r = 0; r < 3; r++) v[r] = Rb[3 * r] * m.body_pos[3 * bb] + Rb[3 * r + 1] * m.body_pos[3 * bb + 1] + Rb[3 * r + 2] * m.body_pos[3 * bb + 2];
-          for (int r = 0; r < 3; r++) bp[r] += v[r];
-          const double *q2 = &m.body_quat[4 * bb]; const double t[4] = {bq[0] * q2[0] - bq[1] * q2[1] - bq[2] * q2[2] - bq[3] * q2[3], bq[0] * q2[1] + bq[1] * q2[0] + bq[2] * q2[3] - bq[3] * q2[2],
-                                                                        bq[0] * q2[2] - bq[1] * q2[3] + bq[2] * q2[0] + bq[3] * q2[1], bq[0] * q2[3] + bq[1] * q2[2] - bq[2] * q2[1] + bq[3] * q2[0]};
-          for (int r = 0; r < 4; r++) bq[r] = t[r]; } }
-      double Rb[9], W[9], wp[3]; detail::q2m_d(Rb, bq);
-      for (int r = 0; r < 3; r++) { wp[r] = bp[r] + Rb[3 * r] * m.geom_pos[3 * g] + Rb[3 * r + 1] * m.geom_pos[3 * g + 1] + Rb[3 * r + 2] * m.geom_pos[3 * g + 2];
-        for (int c = 0; c < 3; c++) W[3 * r + c] = Rb[3 * r] * R[c] + Rb[3 * r + 1] * R[3 + c] + Rb[3 * r + 2] * R[6 + c]; }
-      real *w = d.geom_wpose[k - MG];
-      for (int r = 0; r < 3; r++) { w[r] = (real)wp[r]; w[3 + r] = (real)W[3 * r + 2]; w[6 + r] = (real)W[3 * r]; w[9 + r] = (real)W[3 * r + 1]; }   // position, z, x, y axes
+      double w[12]; static_geom_wpose(m, g, &m.geom_pos[3 * g], &m.geom_quat[4 * g], w);
+      for (int c = 0; c < 12; c++) d.geom_wpose[k - MG][c] = (real)w[c];
     }
     return k;
   };

@@ -31,6 +31,7 @@ constexpr int YSTRIDE_MAX = 39;   // with the 6 dofs of an extra free body (cass
 
 // model features a kernel instance is compiled for (template parameter FEAT): an instance without a feature carries none of its code
 constexpr int F_XB = 1, F_HFIELD = 2, F_BOX = 4, F_ALL = 7;   // extra free body (cassie_tray_box.xml's cup), height field, box geoms
+constexpr int F_EG = 8;   // the static geoms' world poses, sizes and bounding radii come from per-environment rows (GEOM_ENV_W) instead of the model block
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -157,6 +158,13 @@ constexpr int CE_FRIC = 160;     // [32] sliding friction per collision geom (de
 constexpr int CE_BINVW = 192;    // [32] body_invweight0 (translational)  -- written by the set_const launch
 constexpr int CE_DINVW = 224;    // [32] dof_invweight0                    -- written by the set_const launch
 constexpr int CE_ROOT_MINV = 256, CE_TOT_MINV = 257, CE_PGS_SCALE = 258;   // 1 / main-tree mass, 1 / total mass, 1 / (meaninertia * nv)
+
+// per-environment placement of the static collision geoms (optional, terrain curricula: stairs / tilted floors that differ between environments).
+// Slot k describes device geom MG + k in the layout the collision stage reads: world pose [12] (position, z, x, y axes, as DevModel::geom_wpose), size [3],
+// bounding radius [1].  A model input like the CE rows: snapshots and resets leave it alone.
+constexpr int GE_SLOT = 16;
+constexpr int GEOM_ENV_W = MGS * GE_SLOT;
+constexpr int GE_POSE = 0, GE_SIZE = 12, GE_RBOUND = 15;
 
 // ---- per-warp scratch (in units of `real`)
 constexpr int S_XPOS = 0;                       // [32][3]

@@ -18,6 +18,7 @@ constexpr bool DBG_IN_ALL_INSTANCES = false;
 
 template <typename real> struct EnvArrays {
   real *qpos, *qvel, *qacc_ws, *cst, *pd, *xfrc, *obs, *dbg, *qM, *aux, *cenv, *task, *gait; const real *pd_host; real *obs_host; double *est; int *dfilt, *counters, *ticket; const float *hfield; const unsigned char *mask; int cta_sync, nsub, warp_stride, env0; int n, n_terrain, qpos_w, qvel_w, ystride, xb; size_t hfield_stride;
+  const real *genv;   // [n][GEOM_ENV_W] per-environment static-geom placement or null (read by the F_EG instances only); last, so the other members keep their offsets
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -99,6 +100,7 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     E.obs = A.obs + (size_t)env * OBS_W; E.qM = A.qM + (size_t)env * 2 * NM_MAX; E.dbg = (DBG_IN_ALL_INSTANCES || INST == 1) && A.dbg ? A.dbg + (size_t)env * D_SIZE : nullptr; E.counters = A.counters + (size_t)env * 8;
     E.aux = A.aux ? A.aux + (size_t)env * AUX_W : nullptr; E.cenv = A.cenv ? A.cenv + (size_t)env * CE_W : nullptr; E.cta_sync = sync_on; E.nsub = A.nsub;
     E.est = A.est ? A.est + (size_t)env * EST_W : nullptr; E.est_out = E.obs + OB_EST_OUT;
+    if (FEAT & F_EG) { E.genv = A.genv; E.env = env; }   // the row address is formed where the collision stage reads it: no pointer held across the step
     step_env<real, INST == 1, FEAT, INST >= 1>(cm, sm, E, qvel, qacc_ws, xqvel, xqacc_ws, nticks, mode);
     __syncwarp();
     if (mode >= 2) continue;   // query / set_const: only the aux row / the constant row is written

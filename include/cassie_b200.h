@@ -92,6 +92,19 @@ void cassie_sim_set_geom_name_pos(cassie_sim_t *sim, const char *name, double *p
 void cassie_sim_set_geom_name_quat(cassie_sim_t *sim, const char *name, double *quat);
 void cassie_sim_set_geom_name_size(cassie_sim_t *sim, const char *name, double *size);
 int cassie_batch_set_geom_pose(cassie_batch_t *b, const char *name, const double *pos, const double *quat, const double *size);
+/* Per-environment placement of a static plane or box (src/cassiemujoco.c:1466-1541, one placement per environment): terrain curricula whose stairs
+ * and floor tilt differ between the environments of a batch.  pos [n][3] / quat [n][4] are the geom's frame in its body, as MuJoCo's geom_pos /
+ * geom_quat (the same meaning as in cassie_batch_set_geom_pose); size [n][3].  A NULL part leaves that part alone; mask [n] (or NULL: all) selects
+ * the environments that change, the others keep theirs.  The first call gives every environment a row initialised from the shared placement; only the
+ * touched geom's slot is uploaded.  Unlike the shared verb, a per-environment box's bounding radius is recomputed as |size|, so a box enlarged beyond
+ * its file size is never culled by a stale bound.  The placement is part of the model, not of the state: reset and snapshot restore leave it alone.
+ * cassie_batch_set_geom_pose while rows exist still means one placement for all: it also rewrites that geom's slot in every row.
+ * 0, or -1 with nothing changed (cassie_b200_last_error) for an unknown geom, a geom on a moving body, the height field, or a geom without a
+ * collision slot.  get: the placement each environment sees [n][3] / [n][4] / [n][3] (any part may be NULL), rows or not.  clear: frees the rows,
+ * the batch follows the shared placement again. */
+int cassie_batch_set_env_geom_pose(cassie_batch_t *b, const char *name, const double *pos, const double *quat, const double *size, const unsigned char *mask);
+int cassie_batch_get_env_geom_pose(cassie_batch_t *b, const char *name, double *pos, double *quat, double *size);
+int cassie_batch_clear_env_geom_poses(cassie_batch_t *b);
 /* include/cassiemujoco.h:61-73 (src/cassiemujoco.c:1072-1093): model (per-environment constants, height field, timestep) + full dynamic state */
 cassie_sim_t *cassie_sim_duplicate(const cassie_sim_t *src);
 void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *src);
