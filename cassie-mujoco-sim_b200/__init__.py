@@ -15,6 +15,9 @@ LIB_PATH = os.path.join(_HERE, 'libcassie_b200.so')
 MODEL_DIR = os.path.join(_HERE, 'models')
 FP32, FP64 = 0, 1
 PD_WIDTH, OBS_WIDTH, AUX_WIDTH, EST_WIDTH = 52, 112, 64, 16
+# one frame's slot of a frame row (CASSIE_FRAME_* in include/cassie_b200.h) and the frame kinds of set_frames
+FRAME_WIDTH, FRAME_BODY, FRAME_SITE, FRAME_MAX = 20, 0, 1, 64
+FRAME = dict(pos=slice(0, 3), quat=slice(3, 7), vel=slice(7, 13), cfrc=slice(13, 19))
 # slices of a derived-quantity row (CASSIE_AUX_* in include/cassie_b200.h)
 AUX = dict(foot_force=slice(0, 12), toe_force=slice(12, 18), heel_force=slice(18, 24), foot_pos=slice(24, 30), foot_vel=slice(30, 42),
            cm_pos=slice(42, 45), cm_vel=slice(45, 48), angmom=slice(48, 51), obstacle=51, self_collision=52, group_mask=53, ncon=54)
@@ -453,6 +456,43 @@ class CassieBatch:
         if self.L.cassie_batch_clear_env_geom_poses(self.h) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- frames: named bodies / sites written by every step and forward (reference: xpos, xquat, get_site_xpos, get_site_quat, body_vel,
+    # get_body_contact_force of example/cassiemujoco.py)
+    def set_frames(self, names, kinds=None):
+        """track `names` (bodies, or sites where kinds[i] == FRAME_SITE; kinds=None: all bodies); [] drops the rows.  From the next launch on,
+        frames() holds per environment and frame the pose of the state the last physics sub-step started from and that sub-step's velocity and
+        contact force, laid out as FRAME (pos, quat, vel, cfrc slices of FRAME_WIDTH)."""
+        names = list(names)
+        kinds = [FRAME_BODY] * len(names) if kinds is None else [int(k) for k in kinds]
+        if len(kinds) != len(names):
+            raise ValueError('one kind per frame name')
+        arr = (C.c_char_p * max(1, len(names)))(*[n.encode() for n in names])
+        ks = (C.c_int * max(1, len(kinds)))(*kinds)
+        self.L.cassie_batch_set_frames.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int]
+        if self.L.cassie_batch_set_frames(self.h, arr, ks, len(names)) != 0:
+            raise RuntimeError(_last_error())
+
+    def nframes(self):
+        self.L.cassie_batch_nframes.argtypes = [C.c_void_p]
+        return int(self.L.cassie_batch_nframes(self.h))
+
+    def frame_jacobian(self, i):
+        """(jacp, jacr) [n, 3, nv] of frame i (its index in set_frames) at the CURRENT state, as the reference's get_jacobian_full(_site): one launch
+        that writes nothing else"""
+        jacp, jacr = np.zeros((self.n, 3, self.nv)), np.zeros((self.n, 3, self.nv))
+        self.L.cassie_batch_frame_jacobian.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        if self.L.cassie_batch_frame_jacobian(self.h, int(i), self._dp(jacp), self._dp(jacr)) != 0:
+            raise RuntimeError(_last_error())
+        return jacp, jacr
+
+    def frames(self):
+        """[n, nframes, FRAME_WIDTH] rows of the frames set with set_frames"""
+        out = np.zeros((self.n, self.nframes(), FRAME_WIDTH))
+        self.L.cassie_batch_get_frames.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        if self.L.cassie_batch_get_frames(self.h, self._dp(out)) != 0:
+            raise RuntimeError(_last_error())
+        return out
+
     def query(self):
         """refresh the centre-of-mass slots of the aux rows for the CURRENT state (nothing else is written)."""
         if self.L.cassie_batch_query(self.h) != 0:
@@ -533,19 +573,23 @@ class CassieBatch:
         self.L.cassie_batch_set_stream(self.h, C.c_void_p(cuda_stream_ptr))
 
     def torch_view(self, field):
-        """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112]).
+        """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
+        frame_jac [n, 240]).  set_frames reallocates the frame rows: a view taken before it must not be used after it.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
         call sync() before reading the view: torch ops on another stream are not ordered after an in-flight step."""
         import torch
         self.L.cassie_batch_row_width.argtypes = [C.c_void_p, C.c_char_p]
         width = self.L.cassie_batch_row_width(self.h, field.encode())
+        ptr = self.device_ptr(field)
+        if width <= 0 or not ptr:
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
 
         class _Arr:
             pass
         a = _Arr()
-        a.__cuda_array_interface__ = dict(shape=(self.n, width), typestr=ts, data=(self.device_ptr(field), False), version=2)
+        a.__cuda_array_interface__ = dict(shape=(self.n, width), typestr=ts, data=(ptr, False), version=2)
         return torch.as_tensor(a, device='cuda')
 
 
@@ -844,6 +888,70 @@ class CassieSim:
 
     def angular_momentum(self):
         return list(self._vec(self.L.cassie_sim_angular_momentum, 3))
+
+    # ---- frames (example/cassiemujoco.py:124-130, 184-214, 254-270, 694-721): what the last step / forward left behind; the Jacobians are taken at
+    # the current state.  An unknown name raises (the reference indexes its arrays with -1)
+    def _ptr(self, fn, name, n):
+        fn.restype = C.POINTER(C.c_double)
+        fn.argtypes = [C.c_void_p, C.c_char_p]
+        p = fn(self.c, name.encode())
+        if not p:
+            raise KeyError(name)
+        return np.array(p[:n])
+
+    def _named(self, fn, name, n):
+        a = (C.c_double * n)()
+        fn.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_char_p]
+        fn(self.c, a, name.encode())
+        return np.array(a[:])
+
+    def xpos(self, body_name):
+        return self._ptr(self.L.cassie_sim_xpos, body_name, 3)
+
+    def xquat(self, body_name):
+        return self._ptr(self.L.cassie_sim_xquat, body_name, 4)
+
+    def get_site_xpos(self, name):
+        return self._ptr(self.L.cassie_sim_site_xpos, name, 3)
+
+    def get_site_quat(self, name):
+        a = (C.c_double * 4)()
+        self.L.cassie_sim_site_xquat.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_double)]
+        self.L.cassie_sim_site_xquat(self.c, name.encode(), a)
+        return a[:4]
+
+    def body_vel(self, vel, body_name):
+        """cvel of the body ([angular; linear], com-based) into vel[6]; cassie_sim_body_velocities (the reference wrapper names a function its
+        library does not export)"""
+        vel[:6] = self._named(self.L.cassie_sim_body_velocities, body_name, 6)
+
+    def get_body_contact_force(self, force, body_name):
+        force[:6] = self._named(self.L.cassie_sim_body_contact_force, body_name, 6)
+
+    def get_jacobian(self, name):
+        return self._named(self.L.cassie_sim_get_jacobian, name, 3 * self.nv)
+
+    def _jac_full(self, fn, name):
+        p, r = (C.c_double * (3 * self.nv))(), (C.c_double * (3 * self.nv))()
+        fn.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_char_p]
+        fn(self.c, p, r, name.encode())
+        return np.array(p[:]), np.array(r[:])
+
+    def get_jacobian_full(self, name):
+        return self._jac_full(self.L.cassie_sim_get_jacobian_full, name)
+
+    def get_jacobian_full_site(self, name):
+        return self._jac_full(self.L.cassie_sim_get_jacobian_full_site, name)
+
+    def get_object_relative_pose(self, pose1, pose2, relative_pose):
+        """pose 2 ([pos3, quat4]) in the frame of pose 1, into relative_pose[7]"""
+        d = C.POINTER(C.c_double)
+        a = [(C.c_double * k)(*v) for k, v in ((3, pose1[:3]), (4, pose1[3:7]), (3, pose2[:3]), (4, pose2[3:7]))]
+        pos, quat = (C.c_double * 3)(), (C.c_double * 4)()
+        self.L.cassie_sim_relative_pose.argtypes = [d] * 6
+        self.L.cassie_sim_relative_pose(*a, pos, quat)
+        relative_pose[:3] = pos[:]
+        relative_pose[3:7] = quat[:]
 
     def check_self_collision(self):
         return bool(self.L.cassie_sim_check_self_collision(self.c))

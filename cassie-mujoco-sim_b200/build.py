@@ -22,6 +22,10 @@ INSTANCES = [('f00', 'float', 0, 0), ('f10', 'float', 1, 0), ('f02', 'float', 0,
 # models without boxes, floor tilt only) or every feature, in each instance kind; the tag's last digit is the feature set in hex
 ENV_GEOM_INSTANCES = [('f0c', 'float', 0, 12), ('f1c', 'float', 1, 12), ('f2c', 'float', 2, 12), ('f0f', 'float', 0, 15), ('f1f', 'float', 1, 15), ('f2f', 'float', 2, 15),
                       ('d0f', 'double', 0, 15), ('d1f', 'double', 1, 15), ('d2f', 'double', 2, 15)]
+# the extended kernel with frame rows (feature 16 = F_FR; cassie_batch_set_frames): boxes or every feature, without and with the per-environment static
+# geoms; tag = precision, instance kind, feature set in hex
+FRAME_INSTANCES = [('f114', 'float', 1, 20), ('f117', 'float', 1, 23), ('d117', 'double', 1, 23),
+                   ('f11c', 'float', 1, 28), ('f11f', 'float', 1, 31), ('d11f', 'double', 1, 31)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -55,7 +59,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

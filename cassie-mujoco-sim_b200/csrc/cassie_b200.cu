@@ -27,12 +27,21 @@ CASSIE_STEP_ENTRY(d07) CASSIE_STEP_ENTRY(d17)
 CASSIE_STEP_ENTRY(f20) CASSIE_STEP_ENTRY(f22) CASSIE_STEP_ENTRY(f24) CASSIE_STEP_ENTRY(f25) CASSIE_STEP_ENTRY(f27) CASSIE_STEP_ENTRY(d27)
 CASSIE_STEP_ENTRY(f0c) CASSIE_STEP_ENTRY(f1c) CASSIE_STEP_ENTRY(f2c) CASSIE_STEP_ENTRY(f0f) CASSIE_STEP_ENTRY(f1f) CASSIE_STEP_ENTRY(f2f)
 CASSIE_STEP_ENTRY(d0f) CASSIE_STEP_ENTRY(d1f) CASSIE_STEP_ENTRY(d2f)
+CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_STEP_ENTRY(f11c) CASSIE_STEP_ENTRY(f11f) CASSIE_STEP_ENTRY(d11f)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_FR) {   // frame rows: extended instances only; F_BOX covers models with at most boxes, F_ALL the rest, each with or without F_EG
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value, eg = (feat & F_EG) != 0, box = !dbl && (feat & ~(F_BOX | F_EG | F_FR)) == 0;
+    if (compiled_feat) *compiled_feat = (box ? F_BOX : F_ALL) | F_FR | (eg ? F_EG : 0);
+    if (dbl) return eg ? cassie_step_entry_d11f() : cassie_step_entry_d117();
+    if (box) return eg ? cassie_step_entry_f11c() : cassie_step_entry_f114();
+    return eg ? cassie_step_entry_f11f() : cassie_step_entry_f117();
+  }
   if (feat & F_EG) {   // per-environment static-geom rows: F_BOX | F_EG covers models with at most boxes (a floor without boxes too), F_ALL | F_EG the rest
     const bool box = !std::is_same<real, double>::value && (feat & ~(F_BOX | F_EG)) == 0;
     if (compiled_feat) *compiled_feat = box ? (F_BOX | F_EG) : (F_ALL | F_EG);
@@ -171,11 +180,14 @@ struct Snap {
   enum { R_QPOS, R_QVEL, R_QACC, R_CST, R_XFRC, R_OBS, R_DFILT, R_EST, R_AUX, NROWS };
   int device = 0, n = 0, esz = 4, qw = 0, vw = 0; bool has_est = false, has_aux = false;
   void *rows[NROWS] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  // the frame rows [n][frame_list.size() / 2][FRAME_W] of the batch, with its frame list ((kind, id) pairs); restored only into a batch with the same list
+  void *frames = nullptr; std::vector<int> frame_list;
+  size_t frame_bytes() const { return (size_t)n * (frame_list.size() / 2) * FRAME_W * esz; }
   int width(int r) const { const int w[NROWS] = {qw, vw, vw, CST_W, XFRC_W, OBS_W, DFILT_W, EST_W, AUX_W}; return w[r]; }
   int elem(int r) const { return r == R_DFILT ? 4 : (r == R_EST ? 8 : esz); }
   size_t bytes(int r) const { return (size_t)n * width(r) * elem(r); }
 };
-static void snap_delete(Snap *k) { if (!k) return; cudaSetDevice(k->device); for (int r = 0; r < Snap::NROWS; r++) cudaFree(k->rows[r]); delete k; }
+static void snap_delete(Snap *k) { if (!k) return; cudaSetDevice(k->device); for (int r = 0; r < Snap::NROWS; r++) cudaFree(k->rows[r]); cudaFree(k->frames); delete k; }
 static Snap *snap_new(int device, int n, int esz, int qw, int vw) {
   if (cudaSetDevice(device) != cudaSuccess) return nullptr;
   Snap *k = new Snap(); k->device = device; k->n = n; k->esz = esz; k->qw = qw; k->vw = vw;
@@ -190,6 +202,8 @@ static bool snap_clone_into(Snap *d, const Snap *k) {   // same shape required
     if (!d->rows[r] && cudaMalloc(&d->rows[r], d->bytes(r)) != cudaSuccess) return false;
     if (cudaMemcpy(d->rows[r], k->rows[r], k->bytes(r), cudaMemcpyDefault) != cudaSuccess) return false;
   }
+  if (d->frame_list != k->frame_list) { cudaFree(d->frames); d->frames = nullptr; d->frame_list = k->frame_list; if (k->frames && cudaMalloc(&d->frames, k->frame_bytes()) != cudaSuccess) return false; }
+  if (k->frames && cudaMemcpy(d->frames, k->frames, k->frame_bytes(), cudaMemcpyDefault) != cudaSuccess) return false;
   return true;
 }
 
@@ -237,6 +251,9 @@ struct BatchBase {
   virtual bool get_env_geom(int g, double *pos, double *quat, double *size) = 0;
   virtual bool clear_env_geoms() = 0;
   virtual bool shared_geom_changed(int g) = 0;          // after the shared placement of geom g was rebuilt: its slot in every row follows it
+  virtual bool set_frames(const char *const *names, const int *kinds, int count) = 0;   // frame rows [n][count][FRAME_W]; count 0: none
+  virtual bool frame_jacobian(int frame, double *jacp, double *jacr) = 0;                 // [n][3][nv] each at the current state (launch mode 4); jacr may be null
+  std::vector<int> frame_list;                          // (kind, id) per frame of the current frame table
   int nsub_override = 0;                                // > 0: physics sub-steps per control tick of the next launches (cassie_sim_step_pd_no2khz)
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
 };
@@ -257,7 +274,7 @@ template <typename real> struct Batch : BatchBase {
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_genv);
+    cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -320,6 +337,7 @@ template <typename real> struct Batch : BatchBase {
       { const void *entry = step_entry<real>(ext, feat);
         CUDA_OK(cudaFuncSetAttribute(entry, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
         CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, feat | F_EG), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // same scratch, same shape
+        if (ext == 1) for (int fe : {feat | F_FR, feat | F_EG | F_FR}) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -463,7 +481,7 @@ template <typename real> struct Batch : BatchBase {
     // and stepping, and unpacks chunk c while the later ones are stepping; the kernels of consecutive chunks overlap at their edges (a chunk's CTAs start
     // on the SMs the previous chunk's CTAs have left, while its last observation rows are still draining over PCIe).  Chunks are whole rounds of the
     // resident warps when the batch is worked off in more than two rounds, equal parts otherwise.
-    const int inst = (A.cenv || A.aux || A.task || (A.dbg && !DBG_IN_ALL_INSTANCES)) ? 1 : (A.est ? 2 : 0), slots = cfg[inst].resident_ctas * cfg[inst].wpb;
+    const int inst = (A.cenv || A.aux || A.task || A.frames || (A.dbg && !DBG_IN_ALL_INSTANCES)) ? 1 : (A.est ? 2 : 0), slots = cfg[inst].resident_ctas * cfg[inst].wpb;
     int nchunk = 1, c0[AOS_MAXC + 1] = {0};
     if (state_out && n >= 1024 && aos_chunks > 1) {
       if (n <= 2 * slots) { nchunk = aos_chunks; for (int c = 1; c < nchunk; c++) c0[c] = (int)((size_t)n * c / nchunk + 31) / 32 * 32; }
@@ -613,6 +631,8 @@ template <typename real> struct Batch : BatchBase {
       if (!k->rows[r]) CUDA_OK(cudaMalloc(&k->rows[r], k->bytes(r)));
       CUDA_OK(cudaMemcpyAsync(k->rows[r], snap_src(r), k->bytes(r), cudaMemcpyDeviceToDevice, stream));
     }
+    if (k->frame_list != frame_list) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(k->frames)); k->frames = nullptr; k->frame_list = frame_list; if (A.frames) CUDA_OK(cudaMalloc(&k->frames, k->frame_bytes())); }
+    if (A.frames) CUDA_OK(cudaMemcpyAsync(k->frames, A.frames, k->frame_bytes(), cudaMemcpyDeviceToDevice, stream));
     return sync();
   }
   bool snap_set(const Snap *k, const unsigned char *mask) override {
@@ -629,6 +649,15 @@ template <typename real> struct Batch : BatchBase {
       if (k->elem(r) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)snap_src(r), (const unsigned long long *)k->rows[r], w, dm, n);
       else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)snap_src(r), (const unsigned int *)k->rows[r], w, dm, n);
       CUDA_OK(cudaGetLastError());
+    }
+    if (A.frames && k->frames && k->frame_list == frame_list) {   // frame rows: only between batches with the same frame list, like the aux rows
+      if (!dm) CUDA_OK(cudaMemcpyAsync(A.frames, k->frames, k->frame_bytes(), cudaMemcpyDeviceToDevice, stream));
+      else {
+        const int w = (int)(frame_list.size() / 2) * FRAME_W;
+        if (sizeof(real) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)A.frames, (const unsigned long long *)k->frames, w, dm, n);
+        else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)A.frames, (const unsigned int *)k->frames, w, dm, n);
+        CUDA_OK(cudaGetLastError());
+      }
     }
     return sync();
   }
@@ -727,6 +756,44 @@ template <typename real> struct Batch : BatchBase {
     for (int e = 0; e < n; e++) memcpy(&slots[(size_t)e * GE_SLOT], &row[GE_SLOT * k], sizeof(real) * GE_SLOT);
     return put_genv_slot(k, slots);
   }
+  // ---- frame rows: the table is checked as a whole before anything changes; the rows start at zero and are filled by the next step / forward launch
+  bool set_frames(const char *const *names, const int *kinds, int count) override {
+    if (count < 0 || count > FRAME_MAX || (count > 0 && (!names || !kinds))) { set_err("cassie_batch_set_frames: between 0 and " + std::to_string(FRAME_MAX) + " frames, with names and kinds"); return false; }
+    std::vector<real> tab((size_t)count * FT_W); std::vector<int> list;
+    for (int f = 0; f < count; f++) {
+      std::string err; const int id = frame_table_row(hm, names[f], kinds[f], &tab[(size_t)f * FT_W], err);
+      if (id < 0) { set_err("cassie_batch_set_frames: " + err); return false; }
+      list.push_back(kinds[f]); list.push_back(id);
+    }
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(A.frames)); CUDA_OK(cudaFree((void *)A.ftab)); A.frames = nullptr; A.ftab = nullptr; A.nfr = 0; frame_list.clear();
+    if (count == 0) return true;
+    real *t = nullptr;
+    CUDA_OK(cudaMalloc(&t, sizeof(real) * tab.size())); A.ftab = t;
+    CUDA_OK(cudaMemcpy(t, tab.data(), sizeof(real) * tab.size(), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc(&A.frames, sizeof(real) * n * count * FRAME_W)); CUDA_OK(cudaMemset(A.frames, 0, sizeof(real) * n * count * FRAME_W));
+    A.nfr = count; frame_list = list;
+    return true;
+  }
+  // the Jacobian of frame `frame` at the current state of every environment: one mode-4 launch (kinematics and centre of mass only, nothing else
+  // written), then a synchronous copy; the Jacobian rows are allocated on first use
+  bool frame_jacobian(int frame, double *jacp, double *jacr) override {
+    if (frame < 0 || frame >= A.nfr) { set_err("cassie_batch_frame_jacobian: frame " + std::to_string(frame) + " of " + std::to_string(A.nfr)); return false; }
+    if (!jacp) { set_err("cassie_batch_frame_jacobian: jacp is required"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    if (!A.jac) { CUDA_OK(cudaMalloc(&A.jac, sizeof(real) * n * FRAME_JAC_W)); CUDA_OK(cudaMemsetAsync(A.jac, 0, sizeof(real) * n * FRAME_JAC_W, stream)); }
+    A.jfr = frame;
+    if (!step(0, 4)) return false;
+    h_tmp.resize((size_t)n * FRAME_JAC_W);
+    CUDA_OK(cudaMemcpyAsync(h_tmp.data(), A.jac, sizeof(real) * n * FRAME_JAC_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    const int nv = hm.nv;
+    for (int e = 0; e < n; e++) for (int k = 0; k < 3; k++) for (int j = 0; j < nv; j++) {
+      const real *r = &h_tmp[(size_t)e * FRAME_JAC_W];
+      jacp[((size_t)e * 3 + k) * nv + j] = (double)r[k * FJ_COLS + j];
+      if (jacr) jacr[((size_t)e * 3 + k) * nv + j] = (double)r[(3 + k) * FJ_COLS + j];
+    }
+    return true;
+  }
   // open-loop sinusoidal gait on the motor-PD targets (BASELINE config 5 "random PD gaits"): evaluated in the kernel every control tick, so
   // multi-tick launches follow it without a host round trip; installing it restarts the tick clock
   bool set_pd_gait(const double *amp, const double *freq, const double *phase) override {
@@ -743,16 +810,18 @@ template <typename real> struct Batch : BatchBase {
   bool step_range(int nticks, int mode, int env0, int count, cudaStream_t on) {   // the launch covers environments [env0, env0 + count)
     CUDA_OK(cudaSetDevice(device));
     if (mode == 2 && !A.aux) { set_err("query needs the derived-quantity rows (cassie_batch_enable_aux)"); return false; }
+    if (mode == 4 && (!A.frames || !A.jac)) { set_err("the frame Jacobian needs frames (cassie_batch_set_frames)"); return false; }
     A.nsub = nsub_override;
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
-    const int ext = (A.cenv || A.aux || A.task || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode == 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    const int ext = (A.cenv || A.aux || A.task || A.frames || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.frames ? F_FR : 0);   // frame rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
-      CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, A.genv ? feat | F_EG : feat), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
+      CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
     CUDA_OK(cudaGetLastError());
     return true;
@@ -786,6 +855,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "xfrc")) return d2h(A.xfrc, XFRC_W, XFRC_W, 0, out);
     if (!strcmp(f, "est_out")) { if (!A.est) { set_err("the in-kernel estimator is not enabled (cassie_batch_enable_estimator_device)"); return false; } return d2h(A.obs, OBS_W, EO_W, OB_EST_OUT, out); }
     if (!strcmp(f, "aux")) { if (!A.aux) { set_err("derived quantities are not enabled (cassie_batch_enable_aux)"); return false; } return d2h(A.aux, AUX_W, AUX_W, 0, out); }
+    if (!strcmp(f, "frames")) { if (!A.frames) { set_err("no frames are set (cassie_batch_set_frames)"); return false; } return d2h(A.frames, A.nfr * FRAME_W, A.nfr * FRAME_W, 0, out); }
     set_err(std::string("unknown field ") + f); return false;
   }
   bool h2d(real *dst, int w, int take, int off, const double *in) {
@@ -814,6 +884,7 @@ template <typename real> struct Batch : BatchBase {
   void *dev_ptr(const char *f) override {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
+    if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -836,10 +907,15 @@ template <typename real> struct Batch : BatchBase {
 
 // ====================================================================== C-ABI
 using namespace cassie;
+static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
+static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
 struct cassie_batch { BatchBase *impl; std::vector<double> obs, radio; };
 struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[64], qvel_dev[64], time_dev, aux[AUX_W]; std::vector<float> hfield, hfield_dev; std::string path; double timestep = 0, timestep_dev = 0;
   std::vector<double> m_mass, m_ipos, m_damp, m_fric, m_mass_dev, m_ipos_dev, m_damp_dev, m_fric_dev;
-  std::vector<double> m_gpos, m_gquat, m_gsize, m_gpos_dev, m_gquat_dev, m_gsize_dev; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
+  std::vector<double> m_gpos, m_gquat, m_gsize, m_gpos_dev, m_gquat_dev, m_gsize_dev;
+  // every body and every site is a frame of the simulator's batch (bodies first); host mirrors laid out like mjData's xpos[nbody][3], xquat[nbody][4],
+  // site_xpos[nsite][3], so that the borrowed pointers of cassie_sim_xpos / xquat / site_xpos index across bodies as &d->xpos[3 * id] does
+  std::vector<double> frames, xpos, xquat, site_xpos; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
 
 // cassie_state_t (include/cassiemujoco.h:434-463): a device-resident snapshot of one simulator's rows plus the host mirrors the reference hands out as
 // borrowed pointers (time, qpos, qvel); the snapshot is allocated by the first cassie_get_state, which also fixes the owning simulator's sizes
@@ -874,7 +950,8 @@ int cassie_batch_nv(const cassie_batch_t *b) { return b->impl->hm.nv; }
 int cassie_batch_precision(const cassie_batch_t *b) { return b->impl->precision; }
 int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "qpos")) return b->impl->hm.nq > 36 ? QPOS_W_XB : QPOS_W_MAIN; if (!strcmp(field, "qvel")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN;
-  if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W; return -1;
+  if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
+  if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W; return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
 void cassie_batch_reset(cassie_batch_t *b, const unsigned char *mask) { b->impl->reset(mask); b->impl->sync(); b->impl->reset_estimator(mask); b->impl->reset_estimator_device(mask); }   // a fresh cassie_sim_t has a fresh estimator
@@ -953,6 +1030,11 @@ bool cassie_mujoco_init(const char *modelfile) {
 void cassie_cleanup(void) { std::lock_guard<std::mutex> g(g_model_mutex); g_model_path.clear(); }
 static void sim_pull(cassie_sim_t *c) {
   c->b->impl->get("qpos", c->qpos); c->b->impl->get("qvel", c->qvel); c->b->impl->get("time", &c->time); if (c->b->impl->has_aux()) c->b->impl->get("aux", c->aux);
+  if (!c->frames.empty() && c->b->impl->get("frames", c->frames.data())) {   // the sizes were fixed at init: the borrowed pointers stay valid
+    const int nb = (int)c->xquat.size() / 4, ns = (int)c->site_xpos.size() / 3;
+    for (int b = 0; b < nb; b++) { const double *f = &c->frames[(size_t)b * FRAME_W]; for (int k = 0; k < 3; k++) c->xpos[3 * b + k] = f[FR_POS + k]; for (int k = 0; k < 4; k++) c->xquat[4 * b + k] = f[FR_QUAT + k]; }
+    for (int s = 0; s < ns; s++) for (int k = 0; k < 3; k++) c->site_xpos[3 * s + k] = c->frames[(size_t)(nb + s) * FRAME_W + FR_POS + k];
+  }
   memcpy(c->qpos_dev, c->qpos, sizeof c->qpos); memcpy(c->qvel_dev, c->qvel, sizeof c->qvel); c->time_dev = c->time;
 }
 static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote through the borrowed pointers
@@ -975,7 +1057,13 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   cassie_batch_t *b = cassie_batch_init(path.c_str(), 1, 0, CASSIE_B200_FP64);
   if (!b) return nullptr;
   cassie_sim_t *c = new cassie_sim(); memset(c->qpos, 0, sizeof c->qpos); memset(c->qvel, 0, sizeof c->qvel); memset(c->aux, 0, sizeof c->aux); c->b = b; c->path = path; c->timestep = c->timestep_dev = b->impl->hm.timestep;
-  b->impl->enable_aux(true); b->impl->step(0, 1);   // a single environment always carries the derived-quantity row; populate it like the sensordata
+  b->impl->enable_aux(true);   // a single environment always carries the derived-quantity row ...
+  { const HostModel &hm = b->impl->hm; std::vector<const char *> names; std::vector<int> kinds;   // ... and a frame per body and site (cassie_sim_xpos & co.)
+    for (const std::string &s : hm.names_body) { names.push_back(s.c_str()); kinds.push_back(0); }
+    for (const std::string &s : hm.names_site) { names.push_back(s.c_str()); kinds.push_back(1); }
+    if ((int)names.size() <= FRAME_MAX && (int)hm.names_body.size() == hm.nbody && b->impl->set_frames(names.data(), kinds.data(), (int)names.size())) {
+      c->frames.assign(names.size() * FRAME_W, 0.0); c->xpos.assign(3 * hm.names_body.size(), 0.0); c->xquat.assign(4 * hm.names_body.size(), 0.0); c->site_xpos.assign(3 * hm.names_site.size(), 0.0); } }
+  b->impl->step(0, 1);   // populate them like the sensordata
   b->impl->enable_estimator_device(true);   // ... and the estimator (toe / heel forces, filters) inside the kernel, as state_output_step runs in every cassie_sim_step_pd (src/cassiemujoco.c:1156)
   sim_pull(c);
   { const HostModel &hm = b->impl->hm; c->m_mass = hm.body_mass; c->m_ipos = hm.body_ipos; c->m_damp = hm.dof_damping; c->m_fric = hm.geom_friction;
@@ -1016,6 +1104,57 @@ void cassie_sim_angular_momentum(const cassie_sim_t *c, double Lcm[3]) { sim_que
 bool cassie_sim_check_obstacle_collision(const cassie_sim_t *c) { return sim_aux(c)[AX_OBSTACLE] != 0; }
 bool cassie_sim_check_self_collision(const cassie_sim_t *c) { return sim_aux(c)[AX_SELF] != 0; }
 bool cassie_sim_geom_collision(const cassie_sim_t *c, int geom_group) { return geom_group >= 0 && geom_group < 16 && (((int)sim_aux(c)[AX_GROUPMASK] >> geom_group) & 1); }
+// ---- frames (src/cassiemujoco.c:1242-1301, 1543-1562, 1752-1809): poses, cvel and contact forces are the frame rows the last step / forward left
+// behind, kept in the simulator's mirrors; the Jacobians recompute the kinematics of the CURRENT state in a launch that writes nothing else (the
+// reference's mj_kinematics there also overwrites d->xpos; the mirrors keep the last step's poses, as cassie_sim_cm_position leaves them).  An unknown
+// name returns NULL / zeros and records an error (the reference indexes its arrays with -1).
+static int sim_body(const cassie_sim_t *c, const char *name, const char *verb) {
+  const int id = name && !c->frames.empty() ? c->b->impl->hm.body_id(name) : -1;
+  if (id < 0) set_err(std::string(verb) + ": unknown body " + (name ? name : "(null)"));
+  return id;
+}
+static int sim_site(const cassie_sim_t *c, const char *name, const char *verb) {
+  const int id = name && !c->frames.empty() ? c->b->impl->hm.site_id(name) : -1;
+  if (id < 0) set_err(std::string(verb) + ": unknown site " + (name ? name : "(null)"));
+  return id;
+}
+static const double *sim_frame(const cassie_sim_t *c, int f) { return &c->frames[(size_t)f * FRAME_W]; }
+double *cassie_sim_xpos(cassie_sim_t *c, const char *name) { const int b = sim_body(c, name, "cassie_sim_xpos"); return b < 0 ? nullptr : &c->xpos[3 * b]; }
+double *cassie_sim_xquat(cassie_sim_t *c, const char *name) { const int b = sim_body(c, name, "cassie_sim_xquat"); return b < 0 ? nullptr : &c->xquat[4 * b]; }
+double *cassie_sim_site_xpos(cassie_sim_t *c, const char *name) { const int s = sim_site(c, name, "cassie_sim_site_xpos"); return s < 0 ? nullptr : &c->site_xpos[3 * s]; }
+void cassie_sim_site_xquat(cassie_sim_t *c, const char *name, double *xquat) {
+  const int s = sim_site(c, name, "cassie_sim_site_xquat");
+  for (int k = 0; k < 4; k++) xquat[k] = s < 0 ? 0.0 : sim_frame(c, (int)c->xquat.size() / 4 + s)[FR_QUAT + k];
+}
+void cassie_sim_body_velocities(const cassie_sim_t *c, double cvel[6], const char *name) {
+  const int b = sim_body(c, name, "cassie_sim_body_velocities");
+  for (int k = 0; k < 6; k++) cvel[k] = b < 0 ? 0.0 : sim_frame(c, b)[FR_VEL + k];
+}
+void cassie_sim_body_contact_force(const cassie_sim_t *c, double cfrc[6], const char *name) {
+  const int b = sim_body(c, name, "cassie_sim_body_contact_force");
+  for (int k = 0; k < 6; k++) cfrc[k] = b < 0 ? 0.0 : sim_frame(c, b)[FR_CFRC + k];
+}
+static void sim_jacobian(cassie_sim_t *c, int f, double *jac, double *jac_rot) {
+  const int nv = c->b->impl->hm.nv;
+  if (f < 0) { for (int i = 0; i < 3 * nv; i++) { jac[i] = 0; if (jac_rot) jac_rot[i] = 0; } return; }
+  sim_push(c); c->b->impl->frame_jacobian(f, jac, jac_rot);
+}
+void cassie_sim_get_jacobian(cassie_sim_t *c, double *jac, const char *name) { sim_jacobian(c, sim_body(c, name, "cassie_sim_get_jacobian"), jac, nullptr); }
+void cassie_sim_get_jacobian_full(cassie_sim_t *c, double *jac, double *jac_rot, const char *name) { sim_jacobian(c, sim_body(c, name, "cassie_sim_get_jacobian_full"), jac, jac_rot); }
+void cassie_sim_get_jacobian_full_site(cassie_sim_t *c, double *jac, double *jac_rot, const char *name) {
+  const int s = sim_site(c, name, "cassie_sim_get_jacobian_full_site");
+  sim_jacobian(c, s < 0 ? -1 : (int)c->xquat.size() / 4 + s, jac, jac_rot);
+}
+// pose 2 in the frame of pose 1: mju_negPose, then mju_mulPose (host arithmetic, unit quaternions)
+void cassie_sim_relative_pose(double pos1[3], double quat1[4], double pos2[3], double quat2[4], double pos2_in_pos1[3], double quat2_in_quat1[4]) {
+  const double w = quat1[0], x = -quat1[1], y = -quat1[2], z = -quat1[3];   // the conjugate of quat1 and its rotation matrix
+  const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y), 2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x),
+                       2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)};
+  const double *q = quat2, d[3] = {pos2[0] - pos1[0], pos2[1] - pos1[1], pos2[2] - pos1[2]};
+  double r[4] = {w * q[0] - x * q[1] - y * q[2] - z * q[3], w * q[1] + x * q[0] + y * q[3] - z * q[2], w * q[2] - x * q[3] + y * q[0] + z * q[1], w * q[3] + x * q[2] - y * q[1] + z * q[0]};
+  for (int k = 0; k < 4; k++) quat2_in_quat1[k] = r[k];
+  for (int k = 0; k < 3; k++) pos2_in_pos1[k] = R[3 * k] * d[0] + R[3 * k + 1] * d[1] + R[3 * k + 2] * d[2];   // R (pos2 - pos1) = R pos2 + (-R pos1)
+}
 // ---- model constants (domain randomisation).  include/cassiemujoco.h / src/cassiemujoco.c:1303-1436: the reference hands out pointers into
 // its private mjModel copy; here they point into host mirrors that are uploaded before the next step / query / set_const.
 void cassie_sim_params(cassie_sim_t *c, int *params) { const HostModel &hm = c->b->impl->hm; params[0] = hm.nq; params[1] = hm.nv; params[2] = hm.nu; params[3] = 29; params[4] = hm.nbody; params[5] = hm.ngeom; }
@@ -1093,6 +1232,10 @@ int cassie_batch_get_env_geom_pose(cassie_batch_t *b, const char *name, double *
   return b->impl->get_env_geom(b->impl->hm.geom_id(name ? name : ""), pos, quat, size) ? 0 : -1;
 }
 int cassie_batch_clear_env_geom_poses(cassie_batch_t *b) { return b->impl->clear_env_geoms() ? 0 : -1; }
+int cassie_batch_set_frames(cassie_batch_t *b, const char *const *names, const int *kinds, int count) { return b->impl->set_frames(names, kinds, count) ? 0 : -1; }
+int cassie_batch_nframes(const cassie_batch_t *b) { return (int)(b->impl->frame_list.size() / 2); }
+int cassie_batch_get_frames(cassie_batch_t *b, double *out) { return b->impl->get("frames", out) ? 0 : -1; }
+int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, double *jacr) { return b->impl->frame_jacobian(frame, jacp, jacr) ? 0 : -1; }
 
 // ---- legacy verbs RL wrappers call around cassie_sim_step_pd (src/cassiemujoco.c:1072-1093, 1137-1145, 1159-1181, 1196-1225, 1974-2000, 2086-2092, 3380-3452)
 // the dynamic subset of cassie_out_t from an observation row, the rest as cassie_out_init leaves it (:672-734)

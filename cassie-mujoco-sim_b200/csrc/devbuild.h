@@ -64,6 +64,29 @@ inline int env_geom_check(const HostModel &m, const int *geom_dev, int g, std::s
   return geom_dev[g] - MG;
 }
 
+// one row of a batch's frame table (FT_W) for body (kind 0) or site (kind 1) `name`; its id, or -1 with a reason for an unknown name or kind
+template <typename real> int frame_table_row(const HostModel &m, const char *name, int kind, real *row, std::string &err) {
+  for (int c = 0; c < FT_W; c++) row[c] = 0;
+  row[FT_QUAT] = 1;
+  if (!name) { err = "frame name missing"; return -1; }
+  if (kind == 0) {
+    const int b = m.body_id(name);
+    if (b < 0) { err = std::string("unknown body ") + name; return -1; }
+    row[FT_BODY] = (real)b;
+    return b;
+  }
+  if (kind == 1) {
+    const int s = m.site_id(name);
+    if (s < 0) { err = std::string("unknown site ") + name; return -1; }
+    row[FT_BODY] = (real)m.site_bodyid[s]; row[FT_KIND] = 1;
+    for (int c = 0; c < 3; c++) row[FT_POS + c] = (real)m.site_pos[3 * s + c];
+    for (int c = 0; c < 4; c++) row[FT_QUAT + c] = (real)m.site_quat[4 * s + c];
+    return s;
+  }
+  err = "unknown frame kind " + std::to_string(kind) + " (0 body, 1 site)";
+  return -1;
+}
+
 struct BuildInfo { int unsupported_pairs = 0; int collision_geoms = 0; int geom_dev[256]; BuildInfo() { for (int i = 0; i < 256; i++) geom_dev[i] = -1; } };   // geom_dev: host geom id -> collision geom slot of the device block
 
 template <typename real>

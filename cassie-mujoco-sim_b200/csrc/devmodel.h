@@ -32,6 +32,7 @@ constexpr int YSTRIDE_MAX = 39;   // with the 6 dofs of an extra free body (cass
 // model features a kernel instance is compiled for (template parameter FEAT): an instance without a feature carries none of its code
 constexpr int F_XB = 1, F_HFIELD = 2, F_BOX = 4, F_ALL = 7;   // extra free body (cassie_tray_box.xml's cup), height field, box geoms
 constexpr int F_EG = 8;   // the static geoms' world poses, sizes and bounding radii come from per-environment rows (GEOM_ENV_W) instead of the model block
+constexpr int F_FR = 16;  // frame rows (FRAME_W per named body / site) are filled in the last sub-step of a launch (extended instances only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -165,6 +166,20 @@ constexpr int CE_ROOT_MINV = 256, CE_TOT_MINV = 257, CE_PGS_SCALE = 258;   // 1 
 constexpr int GE_SLOT = 16;
 constexpr int GEOM_ENV_W = MGS * GE_SLOT;
 constexpr int GE_POSE = 0, GE_SIZE = 12, GE_RBOUND = 15;
+
+// frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
+// after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and
+// contact forces of that sub-step.  Site slots carry zero velocity and force.
+constexpr int FRAME_W = 20;
+constexpr int FR_POS = 0, FR_QUAT = 3, FR_VEL = 7, FR_CFRC = 13;   // [3] xpos / site_xpos, [4] xquat / mat2quat(site_xmat), [6] cvel, [6] contact force (3..5 zero)
+constexpr int FRAME_MAX = 64;
+// the batch's frame table (global memory, one per batch): per frame body id, kind (0 body, 1 site), the site's position and orientation in its body frame
+constexpr int FT_W = 12;
+constexpr int FT_BODY = 0, FT_KIND = 1, FT_POS = 2, FT_QUAT = 5;
+// Jacobian of one frame at the current state (launch mode 4, cassie_batch_frame_jacobian): per environment [6][FJ_COLS], rows jacp x y z then jacr x y z,
+// column = dof in the reference's order (main tree 0..31, the extra free body 32..37), unused columns zero
+constexpr int FJ_COLS = 40;
+constexpr int FRAME_JAC_W = 6 * FJ_COLS;
 
 // ---- per-warp scratch (in units of `real`)
 constexpr int S_XPOS = 0;                       // [32][3]

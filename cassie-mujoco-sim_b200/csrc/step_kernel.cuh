@@ -19,6 +19,8 @@ constexpr bool DBG_IN_ALL_INSTANCES = false;
 template <typename real> struct EnvArrays {
   real *qpos, *qvel, *qacc_ws, *cst, *pd, *xfrc, *obs, *dbg, *qM, *aux, *cenv, *task, *gait; const real *pd_host; real *obs_host; double *est; int *dfilt, *counters, *ticket; const float *hfield; const unsigned char *mask; int cta_sync, nsub, warp_stride, env0; int n, n_terrain, qpos_w, qvel_w, ystride, xb; size_t hfield_stride;
   const real *genv;   // [n][GEOM_ENV_W] per-environment static-geom placement or null (read by the F_EG instances only); last, so the other members keep their offsets
+  const real *ftab; real *frames; int nfr;   // frame table [nfr][FT_W] and rows [n][nfr][FRAME_W] (read by the F_FR instances only); after genv for the same reason
+  real *jac; int jfr;                         // mode 4: Jacobian rows [n][FRAME_JAC_W] of frame jfr (F_FR instances)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -42,7 +44,7 @@ __device__ __forceinline__ void tma_stage(void *dst_smem, const void *src_gmem, 
 template <typename real> __host__ __device__ constexpr size_t model_bytes() { return (sizeof(DevModel<real>) + 127) / 128 * 128; }
 template <typename real> __host__ __device__ constexpr size_t warp_bytes(int ystride, bool ext) { return ((size_t)(ext ? scratch_reals_ext(ystride) : scratch_reals(ystride)) * sizeof(real) + 127) / 128 * 128; }
 
-// mode 0: step nticks; mode 1: mj_forward only.  INST: 0 plain instance, 1 extended instance (per-env constants, derived quantities, task PD, set_const,
+// mode 0: step nticks; mode 1: mj_forward only; 2 / 3 / 4: query, set_const, frame Jacobian (see mj_substep).  INST: 0 plain instance, 1 extended instance (per-env constants, derived quantities, task PD, set_const,
 // estimator), 2 plain instance + estimator stage (what cassie_sim_step_pd_batch runs when nothing else asks for the extended one)
 template <typename real, int INST, int FEAT>
 __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *__restrict__ gmodel, EnvArrays<real> A, int nticks, int mode) {
@@ -101,6 +103,7 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     E.aux = A.aux ? A.aux + (size_t)env * AUX_W : nullptr; E.cenv = A.cenv ? A.cenv + (size_t)env * CE_W : nullptr; E.cta_sync = sync_on; E.nsub = A.nsub;
     E.est = A.est ? A.est + (size_t)env * EST_W : nullptr; E.est_out = E.obs + OB_EST_OUT;
     if (FEAT & F_EG) { E.genv = A.genv; E.env = env; }   // the row address is formed where the collision stage reads it: no pointer held across the step
+    if (FEAT & F_FR) { E.ftab = A.ftab; E.frames = A.frames; E.nfr = A.nfr; E.jac = A.jac; E.jfr = A.jfr; E.env = env; }   // likewise the frame rows, at each frame stage
     step_env<real, INST == 1, FEAT, INST >= 1>(cm, sm, E, qvel, qacc_ws, xqvel, xqacc_ws, nticks, mode);
     __syncwarp();
     if (mode >= 2) continue;   // query / set_const: only the aux row / the constant row is written

@@ -105,6 +105,40 @@ int cassie_batch_set_geom_pose(cassie_batch_t *b, const char *name, const double
 int cassie_batch_set_env_geom_pose(cassie_batch_t *b, const char *name, const double *pos, const double *quat, const double *size, const unsigned char *mask);
 int cassie_batch_get_env_geom_pose(cassie_batch_t *b, const char *name, double *pos, double *quat, double *size);
 int cassie_batch_clear_env_geom_poses(cassie_batch_t *b);
+
+/* Frames: named bodies and sites of the model ("world" included) whose state every step / forward launch writes as a by-product, for rewards and
+ * observations built from the robot's own frames.  Per environment a row [count][CASSIE_FRAME_WIDTH] in the batch precision (environment slowest);
+ * per frame, what the reference's queries return after cassie_sim_step_pd / cassie_sim_forward (src/cassiemujoco.c:1242-1252, 1543-1553,
+ * 1752-1809):
+ *   CASSIE_FRAME_POS  [3] body: xpos; site: site_xpos                               } of the state the last physics sub-step started from
+ *   CASSIE_FRAME_QUAT [4] body: xquat; site: mju_mat2Quat(site_xmat)                }
+ *   CASSIE_FRAME_VEL  [6] body: cvel (cassie_sim_body_velocities: com-based [angular; linear], the new qvel with that sub-step's cdof); site: 0
+ *   CASSIE_FRAME_CFRC [6] body: cassie_sim_body_contact_force (world force of the contacts touching the body, -/+ for body 1 / 2; slots 3..5
+ *                         zero, as in the reference); site: 0
+ * set: names[count] with kinds[count] (CASSIE_FRAME_BODY / CASSIE_FRAME_SITE), at most CASSIE_FRAME_MAX; the rows start at zero and are filled from the
+ * next launch on.  count = 0 frees the rows.  0, or -1 with nothing changed (cassie_b200_last_error) for an unknown name or kind or too many frames.
+ * get: synchronous host copy [n][count][CASSIE_FRAME_WIDTH] doubles; device pointer: cassie_batch_device_ptr(b, "frames").  Every successful set
+ * reallocates the rows: a device pointer (or zero-copy view) taken before it is no longer valid.  Snapshots carry the rows and restore them into a batch
+ * with the same frame list. */
+#define CASSIE_FRAME_WIDTH 20
+#define CASSIE_FRAME_POS 0
+#define CASSIE_FRAME_QUAT 3
+#define CASSIE_FRAME_VEL 7
+#define CASSIE_FRAME_CFRC 13
+#define CASSIE_FRAME_MAX 64
+#define CASSIE_FRAME_BODY 0
+#define CASSIE_FRAME_SITE 1
+int cassie_batch_set_frames(cassie_batch_t *b, const char *const *names, const int *kinds, int count);
+int cassie_batch_nframes(const cassie_batch_t *b);
+int cassie_batch_get_frames(cassie_batch_t *b, double *out);
+/* The Jacobian of frame `frame` (0 .. count-1) at the CURRENT state of every environment, as the reference's cassie_sim_get_jacobian_full(_site)
+ * (src/cassiemujoco.c:1254-1301: kinematics and centre of mass recomputed, then mj_jacBody at xpos or mj_jacSite): jacp, jacr [n][3][nv] (nv = 32,
+ * or 38 with the extra free body; jacr may be NULL).  One launch, synchronous; it writes nothing else (the frame rows keep the last step's poses).
+ * Device rows: cassie_batch_device_ptr(b, "frame_jac") [n][6][CASSIE_FRAME_JAC_COLS] (jacp x y z, jacr x y z; column = dof, unused columns zero),
+ * allocated by the first call.  0, or -1 (cassie_b200_last_error) for a frame out of range. */
+#define CASSIE_FRAME_JAC_COLS 40
+#define CASSIE_FRAME_JAC_WIDTH 240
+int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, double *jacr);
 /* include/cassiemujoco.h:61-73 (src/cassiemujoco.c:1072-1093): model (per-environment constants, height field, timestep) + full dynamic state */
 cassie_sim_t *cassie_sim_duplicate(const cassie_sim_t *src);
 void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *src);
@@ -146,6 +180,19 @@ void cassie_sim_foot_velocities(const cassie_sim_t *c, double cvel[12]);
 void cassie_sim_cm_position(const cassie_sim_t *c, double cm_pos[3]);
 void cassie_sim_cm_velocity(const cassie_sim_t *c, double cm_vel[3]);
 void cassie_sim_angular_momentum(const cassie_sim_t *c, double Lcm[3]);
+/* frames of the simulator (every body and site, cassie_batch_set_frames): poses, cvel and contact forces the last step / forward left behind; host
+ * mirrors laid out like mjData's xpos / xquat / site_xpos, refreshed after every step, forward and state restore.  The Jacobians run a query launch
+ * at the current state.  An unknown name gives NULL / zeros and records an error.  src/cassiemujoco.c:1242-1301, 1543-1562, 1752-1809 */
+double *cassie_sim_xpos(cassie_sim_t *c, const char *name);
+double *cassie_sim_xquat(cassie_sim_t *c, const char *name);
+double *cassie_sim_site_xpos(cassie_sim_t *c, const char *name);
+void cassie_sim_site_xquat(cassie_sim_t *c, const char *name, double *xquat);
+void cassie_sim_body_velocities(const cassie_sim_t *c, double cvel[6], const char *name);
+void cassie_sim_body_contact_force(const cassie_sim_t *c, double cfrc[6], const char *name);
+void cassie_sim_get_jacobian(cassie_sim_t *c, double *jac, const char *name);
+void cassie_sim_get_jacobian_full(cassie_sim_t *c, double *jac, double *jac_rot, const char *name);
+void cassie_sim_get_jacobian_full_site(cassie_sim_t *c, double *jac, double *jac_rot, const char *name);
+void cassie_sim_relative_pose(double pos1[3], double quat1[4], double pos2[3], double quat2[4], double pos2_in_pos1[3], double quat2_in_quat1[4]);
 /* model constants for domain randomisation (SURVEY.md 8f-3).  src/cassiemujoco.c:1303-1436, 949-977 (most are defined there without a header
  * declaration; example/cassiemujoco.py:517-610 calls them).  The pointer-returning verbs hand out borrowed read-write host mirrors
  * ([nv], [nbody], [3 nbody], [3 ngeom] doubles, numbered like the reference's mjModel incl. its visual mesh geoms); writes are uploaded
@@ -322,7 +369,8 @@ int cassie_batch_hfield_nrow(const cassie_batch_t *b);
 int cassie_batch_hfield_ncol(const cassie_batch_t *b);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64]) in the batch precision; the stream all work is enqueued on (cudaStream_t). */
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20]) in the batch precision; the stream all work is enqueued on
+ * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
 void *cassie_batch_get_stream(cassie_batch_t *b);
