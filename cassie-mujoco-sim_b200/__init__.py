@@ -18,6 +18,9 @@ PD_WIDTH, OBS_WIDTH, AUX_WIDTH, EST_WIDTH = 52, 112, 64, 16
 # one frame's slot of a frame row (CASSIE_FRAME_* in include/cassie_b200.h) and the frame kinds of set_frames
 FRAME_WIDTH, FRAME_BODY, FRAME_SITE, FRAME_MAX = 20, 0, 1, 64
 FRAME = dict(pos=slice(0, 3), quat=slice(3, 7), vel=slice(7, 13), cfrc=slice(13, 19))
+# dynamics row (include/cassie_b200.h CASSIE_DYN_*): M [40][40], bias [40], connect rows [12][40], their errors [12], centre-of-mass offset [3]
+DYN_WIDTH, DYN_COLS = 2144, 40
+DYN = dict(M=slice(0, 1600), bias=slice(1600, 1640), J_eq=slice(1640, 2120), eq_err=slice(2120, 2132), rcm=slice(2132, 2135))
 # slices of a derived-quantity row (CASSIE_AUX_* in include/cassie_b200.h)
 AUX = dict(foot_force=slice(0, 12), toe_force=slice(12, 18), heel_force=slice(18, 24), foot_pos=slice(24, 30), foot_vel=slice(30, 42),
            cm_pos=slice(42, 45), cm_vel=slice(45, 48), angmom=slice(48, 51), obstacle=51, self_collision=52, group_mask=53, ncon=54)
@@ -493,6 +496,30 @@ class CassieBatch:
             raise RuntimeError(_last_error())
         return out
 
+    # ---- dynamics at the current state (reference: full_mass_matrix, constraint_jacobian / constraint_error, centroid_inertia of
+    # example/cassiemujoco.py): mass matrix, bias forces, connect-equality rows
+    def compute_dynamics(self):
+        """enqueue one dynamics launch on the batch's stream (asynchronous): M, bias, connect rows and the centre-of-mass offset of the CURRENT state
+        into the device rows (torch_view('dyn')); nothing else is written"""
+        self.L.cassie_batch_dynamics.argtypes = [C.c_void_p]
+        if self.L.cassie_batch_dynamics(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def neq(self):
+        self.L.cassie_batch_neq.argtypes = [C.c_void_p]
+        return int(self.L.cassie_batch_neq(self.h))
+
+    def dynamics(self):
+        """what the last compute_dynamics() wrote, as numpy arrays: M [n, nv, nv], bias [n, nv] (qfrc_bias), J_eq [n, 3 neq, nv] and eq_err [n, 3 neq]
+        (the connect equalities' efc_J / efc_pos rows), Icm [n, 3, 3] (the reference's centroid_inertia formula)"""
+        ne = 3 * self.neq()
+        out = dict(M=np.zeros((self.n, self.nv, self.nv)), bias=np.zeros((self.n, self.nv)), J_eq=np.zeros((self.n, ne, self.nv)), eq_err=np.zeros((self.n, ne)),
+                   Icm=np.zeros((self.n, 3, 3)))
+        self.L.cassie_batch_get_dynamics.argtypes = [C.c_void_p] + [C.POINTER(C.c_double)] * 5
+        if self.L.cassie_batch_get_dynamics(self.h, *(self._dp(out[k]) for k in ('M', 'bias', 'J_eq', 'eq_err', 'Icm'))) != 0:
+            raise RuntimeError(_last_error())
+        return out
+
     def query(self):
         """refresh the centre-of-mass slots of the aux rows for the CURRENT state (nothing else is written)."""
         if self.L.cassie_batch_query(self.h) != 0:
@@ -574,7 +601,8 @@ class CassieBatch:
 
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
-        frame_jac [n, 240]).  set_frames reallocates the frame rows: a view taken before it must not be used after it.
+        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN).  set_frames reallocates the frame rows: a view taken before it must not be used after
+        it.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
         call sync() before reading the view: torch ops on another stream are not ordered after an in-flight step."""
@@ -583,7 +611,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
 
         class _Arr:
@@ -952,6 +980,46 @@ class CassieSim:
         self.L.cassie_sim_relative_pose(*a, pos, quat)
         relative_pose[:3] = pos[:]
         relative_pose[3:7] = quat[:]
+
+    # ---- dynamics at the current state (example/cassiemujoco.py:292-375): one dynamics launch each
+    def _dyn(self, fn, *sizes):
+        bufs = [(C.c_double * k)() for k in sizes]
+        fn.argtypes = [C.c_void_p] + [C.POINTER(C.c_double)] * len(sizes)
+        fn.restype = None
+        fn(self.c, *bufs)
+        return [np.array(b[:]) for b in bufs]
+
+    def centroid_inertia(self):
+        """3 x 3 rotational inertia about the centre of mass in the pelvis frame, flattened (9 values), with the reference's formula"""
+        return list(self._dyn(self.L.cassie_sim_centroid_inertia, 9)[0])
+
+    def full_mass_matrix(self):
+        """the 32 x 32 mass matrix of the robot's dofs"""
+        return self._dyn(self.L.cassie_sim_full_mass_matrix, 32 * 32)[0].reshape(32, 32)
+
+    def constraint_jacobian(self):
+        """[6, 32]: the rows of the left and right achilles-rod connects"""
+        return self._dyn(self.L.cassie_sim_loop_constraint_info, 6 * 32, 6)[0].reshape(6, 32)
+
+    def constraint_error(self):
+        """[6, 1]: their position errors"""
+        return self._dyn(self.L.cassie_sim_loop_constraint_info, 6 * 32, 6)[1].reshape(6, 1)
+
+    def minimal_mass_matrix(self):
+        """16 x 16 mass matrix of the floating base and the 10 motors: the full matrix projected onto these independent coordinates through the
+        achilles constraints, as the reference's wrapper does it.  The dependent coordinates (knee, shin, tarsus, heel-spring side of each leg's
+        four-bar) follow from the independent ones by the least-squares solution G of J_dep G = -J_ind; with P = [I; G], M_min = P' M P.  The
+        constraint Jacobian's floating-base columns are zeroed and so is every entry below 1e-5 (negative ones too), like the reference."""
+        ind = [0, 1, 2, 3, 4, 5, 6, 7, 8, 12, 18, 19, 20, 21, 25, 31]
+        dep = [9, 10, 11, 14, 22, 23, 24, 27]
+        J = self.constraint_jacobian()
+        J[:, 0:6] = 0
+        Jd = J[:, ind + dep]
+        Jd[Jd < 1e-5] = 0
+        M = self.full_mass_matrix()[np.ix_(ind + dep, ind + dep)]
+        G = np.linalg.lstsq(Jd[:, 16:], -Jd[:, :16], rcond=None)[0]
+        P = np.vstack([np.eye(16), G])
+        return P.T @ M @ P
 
     def check_self_collision(self):
         return bool(self.L.cassie_sim_check_self_collision(self.c))

@@ -62,6 +62,22 @@ template <typename real> static const void *step_entry(int inst, int feat, int *
   }
 }
 
+// cassie_sim_centroid_inertia (src/cassiemujoco.c:1647-1687) from one dynamics row: m = M[0][0], I_p = M[3:6, 3:6], r = the row's centre-of-mass offset
+// (DY_RCM).  The diagonal is I_p - m (r_j^2 + r_k^2); the off-diagonals are I_p[i][j] - m r_i r_j, with the reference's sign (the parallel-axis
+// theorem has + there), taken from the lower triangle as the reference does.
+template <typename real> static void centroid_inertia(const real *row, double Icm[9]) {
+  double Ip[3][3], r[3]; const double m = (double)row[DY_M];
+  for (int i = 0; i < 3; i++) { r[i] = (double)row[DY_RCM + i]; for (int j = 0; j < 3; j++) Ip[i][j] = (double)row[DY_M + (i + 3) * DY_COLS + j + 3]; }
+  double Ic[3][3];
+  Ic[0][0] = Ip[0][0] - m * (r[1] * r[1] + r[2] * r[2]);
+  Ic[1][1] = Ip[1][1] - m * (r[2] * r[2] + r[0] * r[0]);
+  Ic[2][2] = Ip[2][2] - m * (r[0] * r[0] + r[1] * r[1]);
+  Ic[0][1] = Ic[1][0] = Ip[1][0] - m * r[1] * r[0];
+  Ic[1][2] = Ic[2][1] = Ip[2][1] - m * r[2] * r[1];
+  Ic[2][0] = Ic[0][2] = Ip[2][0] - m * r[2] * r[0];
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) Icm[3 * i + j] = Ic[i][j];
+}
+
 static thread_local std::string g_err;
 static void set_err(const std::string &e) { g_err = e; fprintf(stderr, "cassie_b200: %s\n", e.c_str()); }
 #define CUDA_OK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { set_err(std::string(#call) + ": " + cudaGetErrorString(e_)); return false; } } while (0)
@@ -253,6 +269,9 @@ struct BatchBase {
   virtual bool shared_geom_changed(int g) = 0;          // after the shared placement of geom g was rebuilt: its slot in every row follows it
   virtual bool set_frames(const char *const *names, const int *kinds, int count) = 0;   // frame rows [n][count][FRAME_W]; count 0: none
   virtual bool frame_jacobian(int frame, double *jacp, double *jacr) = 0;                 // [n][3][nv] each at the current state (launch mode 4); jacr may be null
+  virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
+  virtual bool get_dynamics(double *M, double *bias, double *J_eq, double *eq_err, double *Icm) = 0;   // what the last mode-5 launch wrote; any pointer may be null
+  bool dyn_done = false;                                // a mode-5 launch was enqueued since the rows were allocated
   std::vector<int> frame_list;                          // (kind, id) per frame of the current frame table
   int nsub_override = 0;                                // > 0: physics sub-steps per control tick of the next launches (cassie_sim_step_pd_no2khz)
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
@@ -274,7 +293,7 @@ template <typename real> struct Batch : BatchBase {
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac);
+    cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -794,6 +813,31 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
+  // dynamics at the current state of every environment: one mode-5 launch on the batch stream (kinematics, centre of mass, CRB and the bias forces;
+  // nothing else written).  The rows are allocated on first use; snapshots and resets leave them alone (a query result, not state).
+  bool dynamics() override {
+    CUDA_OK(cudaSetDevice(device));
+    if (!A.dyn) CUDA_OK(cudaMalloc(&A.dyn, sizeof(real) * n * DYN_W));
+    if (!step(0, 5)) return false;
+    dyn_done = true;
+    return true;
+  }
+  bool get_dynamics(double *M, double *bias, double *J_eq, double *eq_err, double *Icm) override {
+    if (!dyn_done) { set_err("cassie_batch_get_dynamics: no dynamics launch yet (cassie_batch_dynamics)"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    h_tmp.resize((size_t)n * DYN_W);
+    CUDA_OK(cudaMemcpyAsync(h_tmp.data(), A.dyn, sizeof(real) * n * DYN_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    const int nv = hm.nv, ne = 3 * hm.neq;
+    for (int e = 0; e < n; e++) {
+      const real *r = &h_tmp[(size_t)e * DYN_W];
+      if (M) for (int i = 0; i < nv; i++) for (int j = 0; j < nv; j++) M[((size_t)e * nv + i) * nv + j] = (double)r[DY_M + i * DY_COLS + j];
+      if (bias) for (int i = 0; i < nv; i++) bias[(size_t)e * nv + i] = (double)r[DY_BIAS + i];
+      if (J_eq) for (int i = 0; i < ne; i++) for (int j = 0; j < nv; j++) J_eq[((size_t)e * ne + i) * nv + j] = (double)r[DY_JEQ + i * DY_COLS + j];
+      if (eq_err) for (int i = 0; i < ne; i++) eq_err[(size_t)e * ne + i] = (double)r[DY_EQPOS + i];
+      if (Icm) centroid_inertia(r, &Icm[(size_t)e * 9]);
+    }
+    return true;
+  }
   // open-loop sinusoidal gait on the motor-PD targets (BASELINE config 5 "random PD gaits"): evaluated in the kernel every control tick, so
   // multi-tick launches follow it without a host round trip; installing it restarts the tick clock
   bool set_pd_gait(const double *amp, const double *freq, const double *phase) override {
@@ -811,6 +855,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     if (mode == 2 && !A.aux) { set_err("query needs the derived-quantity rows (cassie_batch_enable_aux)"); return false; }
     if (mode == 4 && (!A.frames || !A.jac)) { set_err("the frame Jacobian needs frames (cassie_batch_set_frames)"); return false; }
+    if (mode == 5 && !A.dyn) { set_err("the dynamics launch needs its rows (cassie_batch_dynamics)"); return false; }
     A.nsub = nsub_override;
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
@@ -819,7 +864,8 @@ template <typename real> struct Batch : BatchBase {
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.frames ? F_FR : 0);   // frame rows: the extended F_FR instance (set_const launches too: they write no frames)
+    if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
+    const int lf = (A.genv ? feat | F_EG : feat) | ((A.frames || mode == 5) ? F_FR : 0);   // frame rows and the dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -884,7 +930,7 @@ template <typename real> struct Batch : BatchBase {
   void *dev_ptr(const char *f) override {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
-    if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac;
+    if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -908,6 +954,7 @@ template <typename real> struct Batch : BatchBase {
 // ====================================================================== C-ABI
 using namespace cassie;
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
+static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
 static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
 struct cassie_batch { BatchBase *impl; std::vector<double> obs, radio; };
 struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[64], qvel_dev[64], time_dev, aux[AUX_W]; std::vector<float> hfield, hfield_dev; std::string path; double timestep = 0, timestep_dev = 0;
@@ -951,7 +998,8 @@ int cassie_batch_precision(const cassie_batch_t *b) { return b->impl->precision;
 int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "qpos")) return b->impl->hm.nq > 36 ? QPOS_W_XB : QPOS_W_MAIN; if (!strcmp(field, "qvel")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN;
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
-  if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W; return -1;
+  if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
+  if (!strcmp(field, "dyn")) return DYN_W; return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
 void cassie_batch_reset(cassie_batch_t *b, const unsigned char *mask) { b->impl->reset(mask); b->impl->sync(); b->impl->reset_estimator(mask); b->impl->reset_estimator_device(mask); }   // a fresh cassie_sim_t has a fresh estimator
@@ -1145,6 +1193,41 @@ void cassie_sim_get_jacobian_full_site(cassie_sim_t *c, double *jac, double *jac
   const int s = sim_site(c, name, "cassie_sim_get_jacobian_full_site");
   sim_jacobian(c, s < 0 ? -1 : (int)c->xquat.size() / 4 + s, jac, jac_rot);
 }
+// ---- dynamics (src/cassiemujoco.c:1647-1749): one dynamics launch at the CURRENT state, then host arithmetic.  The reference's mj_fwdPosition there also
+// rewrites d->xpos & co.; the mirrors keep the last step's poses, as with the Jacobians.  M is [nv][nv] (nv = 32, or 38 with the extra free body).
+static bool sim_dynamics(const cassie_sim_t *cc, std::vector<double> &M, std::vector<double> *J, std::vector<double> *err, double *Icm) {
+  cassie_sim_t *c = const_cast<cassie_sim_t *>(cc); sim_push(c);
+  const int nv = c->b->impl->hm.nv, ne = 3 * c->b->impl->hm.neq;
+  M.assign((size_t)nv * nv, 0.0); if (J) J->assign((size_t)ne * nv, 0.0); if (err) err->assign(ne, 0.0);
+  return c->b->impl->dynamics() && c->b->impl->get_dynamics(M.data(), nullptr, J ? J->data() : nullptr, err ? err->data() : nullptr, Icm);
+}
+void cassie_sim_full_mass_matrix(const cassie_sim_t *c, double M[1024]) {
+  std::vector<double> F; const int nv = c->b->impl->hm.nv; sim_dynamics(c, F, nullptr, nullptr, nullptr);
+  for (int i = 0; i < 32; i++) for (int j = 0; j < 32; j++) M[i * 32 + j] = F[(size_t)i * nv + j];
+}
+void cassie_sim_minimal_mass_matrix(const cassie_sim_t *c, double M[256]) {
+  static const int IND[16] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 12, 18, 19, 20, 21, 25, 31};   // the floating base, then the 10 motors
+  std::vector<double> F; const int nv = c->b->impl->hm.nv; sim_dynamics(c, F, nullptr, nullptr, nullptr);
+  for (int i = 0; i < 16; i++) for (int j = 0; j < 16; j++) M[i * 16 + j] = F[(size_t)IND[i] * nv + IND[j]];
+}
+// the reference picks the rows of the equalities named left- / right-achilles-rod-eq; the compiled model keeps no equality names, so the connects are
+// picked by their body1 instead (the same rows in the models that name them)
+void cassie_sim_loop_constraint_info(const cassie_sim_t *c, double J_cl[192], double err_cl[6]) {
+  for (int i = 0; i < 192; i++) J_cl[i] = 0; for (int i = 0; i < 6; i++) err_cl[i] = 0;
+  const HostModel &hm = c->b->impl->hm; const int nv = hm.nv, lb = hm.body_id("left-achilles-rod"), rb = hm.body_id("right-achilles-rod");
+  std::vector<int> eqs; for (int e = 0; e < hm.neq; e++) if (hm.eq_obj1id[e] >= 0 && (hm.eq_obj1id[e] == lb || hm.eq_obj1id[e] == rb)) eqs.push_back(e);
+  if (eqs.empty()) { set_err("cassie_sim_loop_constraint_info: no connect equality on left- / right-achilles-rod"); return; }
+  std::vector<double> F, J, err; if (!sim_dynamics(c, F, &J, &err, nullptr)) return;
+  int row = 0;
+  for (int e : eqs) for (int k = 0; k < 3 && row < 6; k++, row++) {
+    for (int j = 0; j < 32; j++) J_cl[row * 32 + j] = J[(size_t)(3 * e + k) * nv + j];
+    err_cl[row] = err[3 * e + k];
+  }
+}
+void cassie_sim_centroid_inertia(const cassie_sim_t *c, double Icm[9]) {
+  std::vector<double> F; for (int i = 0; i < 9; i++) Icm[i] = 0;
+  sim_dynamics(c, F, nullptr, nullptr, Icm);
+}
 // pose 2 in the frame of pose 1: mju_negPose, then mju_mulPose (host arithmetic, unit quaternions)
 void cassie_sim_relative_pose(double pos1[3], double quat1[4], double pos2[3], double quat2[4], double pos2_in_pos1[3], double quat2_in_quat1[4]) {
   const double w = quat1[0], x = -quat1[1], y = -quat1[2], z = -quat1[3];   // the conjugate of quat1 and its rotation matrix
@@ -1236,6 +1319,9 @@ int cassie_batch_set_frames(cassie_batch_t *b, const char *const *names, const i
 int cassie_batch_nframes(const cassie_batch_t *b) { return (int)(b->impl->frame_list.size() / 2); }
 int cassie_batch_get_frames(cassie_batch_t *b, double *out) { return b->impl->get("frames", out) ? 0 : -1; }
 int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, double *jacr) { return b->impl->frame_jacobian(frame, jacp, jacr) ? 0 : -1; }
+int cassie_batch_dynamics(cassie_batch_t *b) { return b->impl->dynamics() ? 0 : -1; }
+int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm) { return b->impl->get_dynamics(M, bias, J_eq, eq_err, Icm) ? 0 : -1; }
+int cassie_batch_neq(const cassie_batch_t *b) { return b->impl->hm.neq; }
 
 // ---- legacy verbs RL wrappers call around cassie_sim_step_pd (src/cassiemujoco.c:1072-1093, 1137-1145, 1159-1181, 1196-1225, 1974-2000, 2086-2092, 3380-3452)
 // the dynamic subset of cassie_out_t from an observation row, the rest as cassie_out_init leaves it (:672-734)

@@ -180,6 +180,13 @@ constexpr int FT_BODY = 0, FT_KIND = 1, FT_POS = 2, FT_QUAT = 5;
 // column = dof in the reference's order (main tree 0..31, the extra free body 32..37), unused columns zero
 constexpr int FJ_COLS = 40;
 constexpr int FRAME_JAC_W = 6 * FJ_COLS;
+// dynamics at the current state (launch mode 5, cassie_batch_dynamics): per environment the dense mass matrix (mj_fullM of qM, armature included), the
+// bias forces qfrc_bias, the 3 neq rows of the connect equalities (efc_J's first rows, j1 - j2) and their p1 - p2 (efc_pos), and the offset of the
+// centre of mass from the pelvis at identity pelvis orientation (cassie_sim_centroid_inertia).  Column = dof in the reference's order (main tree 0..31,
+// the extra free body 32..37), unused entries zero; the row is padded to a multiple of 32
+constexpr int DY_COLS = 40, DY_EQ_ROWS = 3 * ME;
+constexpr int DY_M = 0, DY_BIAS = DY_M + DY_COLS * DY_COLS, DY_JEQ = DY_BIAS + DY_COLS, DY_EQPOS = DY_JEQ + DY_EQ_ROWS * DY_COLS, DY_RCM = DY_EQPOS + DY_EQ_ROWS;
+constexpr int DYN_W = (DY_RCM + 3 + 31) / 32 * 32;
 
 // ---- per-warp scratch (in units of `real`)
 constexpr int S_XPOS = 0;                       // [32][3]

@@ -21,6 +21,7 @@ template <typename real> struct EnvArrays {
   const real *genv;   // [n][GEOM_ENV_W] per-environment static-geom placement or null (read by the F_EG instances only); last, so the other members keep their offsets
   const real *ftab; real *frames; int nfr;   // frame table [nfr][FT_W] and rows [n][nfr][FRAME_W] (read by the F_FR instances only); after genv for the same reason
   real *jac; int jfr;                         // mode 4: Jacobian rows [n][FRAME_JAC_W] of frame jfr (F_FR instances)
+  real *dyn;                                  // mode 5: dynamics rows [n][DYN_W] (F_FR instances)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -44,7 +45,7 @@ __device__ __forceinline__ void tma_stage(void *dst_smem, const void *src_gmem, 
 template <typename real> __host__ __device__ constexpr size_t model_bytes() { return (sizeof(DevModel<real>) + 127) / 128 * 128; }
 template <typename real> __host__ __device__ constexpr size_t warp_bytes(int ystride, bool ext) { return ((size_t)(ext ? scratch_reals_ext(ystride) : scratch_reals(ystride)) * sizeof(real) + 127) / 128 * 128; }
 
-// mode 0: step nticks; mode 1: mj_forward only; 2 / 3 / 4: query, set_const, frame Jacobian (see mj_substep).  INST: 0 plain instance, 1 extended instance (per-env constants, derived quantities, task PD, set_const,
+// mode 0: step nticks; mode 1: mj_forward only; 2 / 3 / 4 / 5: query, set_const, frame Jacobian, dynamics row (see mj_substep).  INST: 0 plain instance, 1 extended instance (per-env constants, derived quantities, task PD, set_const,
 // estimator), 2 plain instance + estimator stage (what cassie_sim_step_pd_batch runs when nothing else asks for the extended one)
 template <typename real, int INST, int FEAT>
 __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *__restrict__ gmodel, EnvArrays<real> A, int nticks, int mode) {
@@ -106,7 +107,10 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     if (FEAT & F_FR) { E.ftab = A.ftab; E.frames = A.frames; E.nfr = A.nfr; E.jac = A.jac; E.jfr = A.jfr; E.env = env; }   // likewise the frame rows, at each frame stage
     step_env<real, INST == 1, FEAT, INST >= 1>(cm, sm, E, qvel, qacc_ws, xqvel, xqacc_ws, nticks, mode);
     __syncwarp();
-    if (mode >= 2) continue;   // query / set_const: only the aux row / the constant row is written
+    if (mode >= 2) {   // query / set_const / frame Jacobian / dynamics: only the aux row / the constant row / the Jacobian row / the dynamics row is written
+      if constexpr ((FEAT & F_FR) != 0) { if (mode == 5) dynamics_row(cm, sm, A.dyn, A.cenv, env, (FEAT & F_XB) ? cm.xb : -1); }   // from what mode 5's sub-step left in shared memory
+      continue;
+    }
     for (int i = l; i < qw; i += 32) A.qpos[(size_t)env * qw + i] = sm[S_QPOS + i];
     A.qvel[(size_t)env * vw + l] = qvel; A.qacc_ws[(size_t)env * vw + l] = qacc_ws;
     if ((FEAT & F_XB) && A.xb >= 0 && l < 6) { A.qvel[(size_t)env * vw + 32 + l] = xqvel; A.qacc_ws[(size_t)env * vw + 32 + l] = xqacc_ws; }

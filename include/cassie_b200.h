@@ -139,6 +139,32 @@ int cassie_batch_get_frames(cassie_batch_t *b, double *out);
 #define CASSIE_FRAME_JAC_COLS 40
 #define CASSIE_FRAME_JAC_WIDTH 240
 int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, double *jacr);
+/* Dynamics at the CURRENT state of every environment, for model-based controllers (operational-space control, whole-body QPs, inverse dynamics):
+ * the joint-space mass matrix M(q) (mj_fullM of qM, armature included), the bias forces qfrc_bias(q, qdot) (Coriolis, centrifugal, gravity), and
+ * Cassie's closed-chain constraints, the Jacobian and position error of the connect equalities (efc_J / efc_pos's first 3 neq rows), with each
+ * environment's own masses and inertial offsets (cassie_batch_set_body_mass / _ipos).  The extra free body's block of M is its constant
+ * diag(m, m, m, I1, I2, I3), its bias [-m g; w x I w] (translation in the world frame, rotation in the body frame).
+ * cassie_batch_dynamics: one launch on the batch stream (asynchronous, like cassie_batch_query); it writes nothing else (state, observations, aux,
+ * frame rows, counters).  The rows are allocated by the first call, freed with the batch; snapshots and resets leave them alone.
+ * cassie_batch_get_dynamics: synchronous copy of what the last dynamics launch wrote: M [n][nv][nv], bias [n][nv], J_eq [n][3 neq][nv],
+ * eq_err [n][3 neq], Icm [n][9] (cassie_sim_centroid_inertia's formula, see below); any pointer may be NULL.  -1 (cassie_b200_last_error) before
+ * any dynamics launch.  Device rows: cassie_batch_device_ptr(b, "dyn") [n][CASSIE_DYN_WIDTH] in the batch precision, column = dof (main tree
+ * 0..31, the extra free body 32..37), unused entries zero:
+ *   CASSIE_DYN_M     [40][40] dense symmetric M
+ *   CASSIE_DYN_BIAS  [40]     qfrc_bias
+ *   CASSIE_DYN_JEQ   [12][40] connect rows j1 - j2, in equality order
+ *   CASSIE_DYN_EQPOS [12]     their p1 - p2
+ *   CASSIE_DYN_RCM   [3]      the subtree com of the world body with the pelvis turned to the identity, minus the pelvis position */
+#define CASSIE_DYN_COLS 40
+#define CASSIE_DYN_M 0
+#define CASSIE_DYN_BIAS 1600
+#define CASSIE_DYN_JEQ 1640
+#define CASSIE_DYN_EQPOS 2120
+#define CASSIE_DYN_RCM 2132
+#define CASSIE_DYN_WIDTH 2144
+int cassie_batch_dynamics(cassie_batch_t *b);
+int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm);
+int cassie_batch_neq(const cassie_batch_t *b);
 /* include/cassiemujoco.h:61-73 (src/cassiemujoco.c:1072-1093): model (per-environment constants, height field, timestep) + full dynamic state */
 cassie_sim_t *cassie_sim_duplicate(const cassie_sim_t *src);
 void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *src);
@@ -193,6 +219,15 @@ void cassie_sim_get_jacobian(cassie_sim_t *c, double *jac, const char *name);
 void cassie_sim_get_jacobian_full(cassie_sim_t *c, double *jac, double *jac_rot, const char *name);
 void cassie_sim_get_jacobian_full_site(cassie_sim_t *c, double *jac, double *jac_rot, const char *name);
 void cassie_sim_relative_pose(double pos1[3], double quat1[4], double pos2[3], double quat2[4], double pos2_in_pos1[3], double quat2_in_quat1[4]);
+/* dynamics of the simulator at its current state (src/cassiemujoco.c:1647-1749), one dynamics launch each, then host arithmetic: the 32 x 32 main-tree
+ * block of M; its rows / columns {0..8, 12, 18..21, 25, 31}; the 3 + 3 rows (32 columns) of the connects whose body1 is left- / right-achilles-rod
+ * and their errors (zeros and an error recorded when the model has none); and the reference's centroid inertia, m = M[0][0], I_p = M[3:6, 3:6],
+ * diagonal I_p - m (r_j^2 + r_k^2), off-diagonals I_p[i][j] - m r_i r_j (the reference's sign), r = the centre of mass at identity pelvis orientation
+ * minus the pelvis position.  The reference's mj_fwdPosition also rewrites d->xpos & co.; the frame mirrors keep the last step's poses. */
+void cassie_sim_full_mass_matrix(const cassie_sim_t *c, double M[1024]);
+void cassie_sim_minimal_mass_matrix(const cassie_sim_t *c, double M[256]);
+void cassie_sim_loop_constraint_info(const cassie_sim_t *c, double J_cl[192], double err_cl[6]);
+void cassie_sim_centroid_inertia(const cassie_sim_t *c, double Icm[9]);
 /* model constants for domain randomisation (SURVEY.md 8f-3).  src/cassiemujoco.c:1303-1436, 949-977 (most are defined there without a header
  * declaration; example/cassiemujoco.py:517-610 calls them).  The pointer-returning verbs hand out borrowed read-write host mirrors
  * ([nv], [nbody], [3 nbody], [3 ngeom] doubles, numbered like the reference's mjModel incl. its visual mesh geoms); writes are uploaded
