@@ -20,6 +20,10 @@ FRAME_WIDTH, FRAME_BODY, FRAME_SITE, FRAME_MAX = 20, 0, 1, 64
 FRAME = dict(pos=slice(0, 3), quat=slice(3, 7), vel=slice(7, 13), cfrc=slice(13, 19))
 # dynamics row (include/cassie_b200.h CASSIE_DYN_*): M [40][40], bias [40], connect rows [12][40], their errors [12], centre-of-mass offset [3]
 DYN_WIDTH, DYN_COLS = 2144, 40
+# terrain rays (include/cassie_b200.h CASSIE_RAY_*): frame kinds of set_rays, and per ray and environment distance (-1: none), world z of the hit (of
+# the ray's end point when none), static geom slot (-1: none), pad
+RAY_HEADING, RAY_ROOT, RAY_WORLD, RAY_MAX, RAY_SLOT = 0, 1, 2, 1024, 4
+RAY_FRAMES = dict(heading=RAY_HEADING, root=RAY_ROOT, world=RAY_WORLD)
 DYN = dict(M=slice(0, 1600), bias=slice(1600, 1640), J_eq=slice(1640, 2120), eq_err=slice(2120, 2132), rcm=slice(2132, 2135))
 # slices of a derived-quantity row (CASSIE_AUX_* in include/cassie_b200.h)
 AUX = dict(foot_force=slice(0, 12), toe_force=slice(12, 18), heel_force=slice(18, 24), foot_pos=slice(24, 30), foot_vel=slice(30, 42),
@@ -520,6 +524,54 @@ class CassieBatch:
             raise RuntimeError(_last_error())
         return out
 
+    # ---- terrain rays (height scans; the reference's rangefinders, example/cassiemujoco.py sense_ground): cast against each environment's static
+    # geoms (floor, height field, boxes, with its own placement and terrain) at the CURRENT state; the robot and the extra free body are not seen
+    def set_rays(self, origin, direction, frame='heading', max_dist=3.0):
+        """origin / direction [k, 3] (directions are normalised), frame 'heading' (root position and yaw, level), 'root' (root pose) or 'world' (or
+        RAY_HEADING / RAY_ROOT / RAY_WORLD), or one kind per ray ([k] of those), max_dist scalar or [k]; k = 0 drops the table.  Reallocates the rows: a torch_view('rays') taken
+        before it must not be used after it."""
+        o = np.ascontiguousarray(np.asarray(origin, dtype=np.float64).reshape(-1, 3))
+        k = len(o)
+        d = np.ascontiguousarray(np.broadcast_to(np.asarray(direction, dtype=np.float64), (k, 3)))
+        if isinstance(frame, (str, int, np.integer)):
+            frame = [frame] * k
+        f = [RAY_FRAMES[x] if isinstance(x, str) else int(x) for x in frame]
+        if len(f) != k:
+            raise ValueError('one frame kind per ray')
+        fr = (C.c_int * max(1, k))(*f)
+        m = np.ascontiguousarray(np.broadcast_to(np.asarray(max_dist, dtype=np.float64), (k,)))
+        self.L.cassie_batch_set_rays.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int]
+        if self.L.cassie_batch_set_rays(self.h, fr, self._dp(o), self._dp(d), self._dp(m), k) != 0:
+            raise RuntimeError(_last_error())
+
+    def set_height_scan(self, xs, ys, z_start=1.0, max_dist=3.0):
+        """a height scan: the grid xs x ys (x slowest) in the heading frame, rays along -z from z_start above the root"""
+        gx, gy = np.meshgrid(np.asarray(xs, dtype=np.float64), np.asarray(ys, dtype=np.float64), indexing='ij')
+        org = np.stack([gx.ravel(), gy.ravel(), np.full(gx.size, float(z_start))], axis=1)
+        self.set_rays(org, [0.0, 0.0, -1.0], 'heading', max_dist)
+
+    def nrays(self):
+        self.L.cassie_batch_nrays.argtypes = [C.c_void_p]
+        return int(self.L.cassie_batch_nrays(self.h))
+
+    def raycast(self):
+        """enqueue one cast of every ray of every environment on the batch's stream (asynchronous), at the CURRENT state; nothing else is written"""
+        self.L.cassie_batch_raycast.argtypes = [C.c_void_p]
+        if self.L.cassie_batch_raycast(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def rays(self):
+        """[n, k, RAY_SLOT] rows of the last raycast(): distance (-1: none), world z of the hit (end point when none), static geom slot (-1), 0"""
+        out = np.zeros((self.n, self.nrays(), RAY_SLOT))
+        self.L.cassie_batch_get_rays.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        if self.L.cassie_batch_get_rays(self.h, self._dp(out)) != 0:
+            raise RuntimeError(_last_error())
+        return out
+
+    def height_scan(self):
+        """[n, k] torch view (no copy) of the world z of each ray's hit, or of its end point when it hits nothing, from the last raycast()"""
+        return self.torch_view('rays')[:, 1::RAY_SLOT]
+
     def query(self):
         """refresh the centre-of-mass slots of the aux rows for the CURRENT state (nothing else is written)."""
         if self.L.cassie_batch_query(self.h) != 0:
@@ -601,8 +653,8 @@ class CassieBatch:
 
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
-        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN).  set_frames reallocates the frame rows: a view taken before it must not be used after
-        it.  The dynamics rows stay put once compute_dynamics() has allocated them.
+        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT]).  set_frames / set_rays reallocate the frame / ray rows: a view
+        taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
         call sync() before reading the view: torch ops on another stream are not ordered after an in-flight step."""
@@ -611,7 +663,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
 
         class _Arr:
@@ -941,6 +993,15 @@ class CassieSim:
 
     def get_site_xpos(self, name):
         return self._ptr(self.L.cassie_sim_site_xpos, name, 3)
+
+    def sense_ground(self):
+        """the six rangefinders (example/cassiemujoco.py:175-181): distance along each rangefinder site's z axis to the static terrain, capped at the
+        sensor's cutoff, -1 for no hit"""
+        percept = (C.c_double * 6)()
+        self.L.cassie_sim_read_rangefinder.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        self.L.cassie_sim_read_rangefinder.restype = None
+        self.L.cassie_sim_read_rangefinder(self.c, percept)
+        return np.array(percept[:6])
 
     def get_site_quat(self, name):
         a = (C.c_double * 4)()

@@ -4,6 +4,7 @@
 // a TMA bulk copy (cp.async.bulk + mbarrier, SASS: UBLKCP), then every warp loads its environment's state rows from HBM
 // (coalesced, one row per array), advances `nticks` control ticks entirely on chip (step_core.inl) and writes the rows back.
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -19,6 +20,7 @@
 #include "devbuild.h"
 #include "estimator_host.h"
 #include "step_kernel.cuh"
+#include "raycast.inl"
 
 // the step-kernel instances live in their own translation units (step_inst.cu, one compilation per instance)
 #define CASSIE_STEP_ENTRY(tag) extern "C" const void *cassie_step_entry_##tag(void);
@@ -31,6 +33,8 @@ CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_S
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
+
+template <typename real> cudaError_t launch_raycast(const RayArgs<real> &A, int device, cudaStream_t stream);   // raycast.cu
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
@@ -272,6 +276,12 @@ struct BatchBase {
   virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
   virtual bool get_dynamics(double *M, double *bias, double *J_eq, double *eq_err, double *Icm) = 0;   // what the last mode-5 launch wrote; any pointer may be null
   bool dyn_done = false;                                // a mode-5 launch was enqueued since the rows were allocated
+  // terrain rays (raycast.inl): the table is checked as a whole before anything changes; k = 0 drops it.  The rows [n][k][RAY_SLOT] are allocated by
+  // the first cast after a set and are a query result, not state
+  virtual bool set_rays(const int *frame, const double *origin, const double *dir, const double *max_dist, int k) = 0;
+  virtual bool raycast() = 0;                           // one launch (asynchronous) at the current qpos
+  virtual bool get_rays(double *out) = 0;               // [n][k][RAY_SLOT] of the last cast
+  int nray = 0; bool rays_done = false;                 // rays in the table; a cast was enqueued since the table was set
   std::vector<int> frame_list;                          // (kind, id) per frame of the current frame table
   int nsub_override = 0;                                // > 0: physics sub-steps per control tick of the next launches (cassie_sim_step_pd_no2khz)
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
@@ -289,11 +299,12 @@ template <typename real> struct Batch : BatchBase {
   cudaStream_t aos_stream[AOS_MAXC] = {};                              // their streams
   bool task_from_aos = false;   // the task-PD rows were created by the AoS entry point's forwarding (not by cassie_batch_set_task_pd)
   float *d_hfield = nullptr; unsigned char *d_mask = nullptr; DevModel<real> h_model_copy{}; int geom_dev[256]; void *d_row = nullptr;
+  real *d_rtab = nullptr, *d_rays = nullptr;   // ray table (RT_HDR + nray RT_W) and the rows of the last cast
   real *d_genv = nullptr;                  // A.genv: [n][GEOM_ENV_W] per-environment static-geom placement, allocated by the first per-environment placement
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -838,6 +849,32 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
+  bool set_rays(const int *frame, const double *origin, const double *dir, const double *max_dist, int k) override {
+    std::vector<double> tab; std::string err;
+    if (!ray_table(frame, origin, dir, max_dist, k, tab, err)) { set_err("cassie_batch_set_rays: " + err); return false; }
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_rtab)); CUDA_OK(cudaFree(d_rays)); d_rtab = d_rays = nullptr; nray = 0; rays_done = false;
+    if (k == 0) return true;
+    std::vector<real> t(tab.begin(), tab.end());
+    CUDA_OK(cudaMalloc(&d_rtab, sizeof(real) * t.size())); CUDA_OK(cudaMemcpy(d_rtab, t.data(), sizeof(real) * t.size(), cudaMemcpyHostToDevice));
+    nray = k;
+    return true;
+  }
+  bool raycast() override {
+    if (!nray) { set_err("cassie_batch_raycast: no rays are set (cassie_batch_set_rays)"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    if (!d_rays) CUDA_OK(cudaMalloc(&d_rays, sizeof(real) * n * nray * RAY_SLOT));
+    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride;
+    R.tab = d_rtab; R.k = nray; R.out = d_rays; R.n = n;
+    CUDA_OK(launch_raycast<real>(R, device, stream));
+    launches++; rays_done = true;
+    return true;
+  }
+  bool get_rays(double *out) override {
+    if (!rays_done) { set_err("cassie_batch_get_rays: no cast since the rays were set (cassie_batch_raycast)"); return false; }
+    if (!out) { set_err("cassie_batch_get_rays: out is required"); return false; }
+    return d2h(d_rays, nray * RAY_SLOT, nray * RAY_SLOT, 0, out);
+  }
   // open-loop sinusoidal gait on the motor-PD targets (BASELINE config 5 "random PD gaits"): evaluated in the kernel every control tick, so
   // multi-tick launches follow it without a host round trip; installing it restarts the tick clock
   bool set_pd_gait(const double *amp, const double *freq, const double *phase) override {
@@ -931,6 +968,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn;
+    if (!strcmp(f, "rays")) return d_rays;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -953,6 +991,7 @@ template <typename real> struct Batch : BatchBase {
 
 // ====================================================================== C-ABI
 using namespace cassie;
+static_assert(CASSIE_RAY_MAX == RAY_MAX && CASSIE_RAY_SLOT == RAY_SLOT && CASSIE_RAY_HEADING == RAY_HEADING && CASSIE_RAY_ROOT == RAY_ROOT && CASSIE_RAY_WORLD == RAY_WORLD, "ray table and rows");
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
 static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
@@ -999,7 +1038,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "qpos")) return b->impl->hm.nq > 36 ? QPOS_W_XB : QPOS_W_MAIN; if (!strcmp(field, "qvel")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN;
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
-  if (!strcmp(field, "dyn")) return DYN_W; return -1;
+  if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT; return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
 void cassie_batch_reset(cassie_batch_t *b, const unsigned char *mask) { b->impl->reset(mask); b->impl->sync(); b->impl->reset_estimator(mask); b->impl->reset_estimator_device(mask); }   // a fresh cassie_sim_t has a fresh estimator
@@ -1174,6 +1213,24 @@ void cassie_sim_site_xquat(cassie_sim_t *c, const char *name, double *xquat) {
   const int s = sim_site(c, name, "cassie_sim_site_xquat");
   for (int k = 0; k < 4; k++) xquat[k] = s < 0 ? 0.0 : sim_frame(c, (int)c->xquat.size() / 4 + s)[FR_QUAT + k];
 }
+// the six rangefinders (src/cassiemujoco.c:776-778, sensordata[29..35)): each site's ray along its z axis from the mirrors' site poses (those of the state
+// the last sub-step started from, when MuJoCo evaluates mj_sensorPos), one world-frame cast on the simulator's batch of one, then MuJoCo's cutoff for a
+// positive-type sensor: min(cutoff, d) where cutoff > 0 (a miss, -1, stays -1); no noise, as in the reference.  Slots without a rangefinder read 0.
+// The rays see the static geoms only (DESIGN.md section 3).  A model without rangefinders gets zeros and a recorded error.
+void cassie_sim_read_rangefinder(cassie_sim_t *c, double ranges[6]) {
+  for (int i = 0; i < 6; i++) ranges[i] = 0;
+  const HostModel &hm = c->b->impl->hm; const int k = std::min((int)hm.rangefinder_site.size(), 6), nb = (int)c->xquat.size() / 4;
+  if (!k || c->frames.empty()) { set_err("cassie_sim_read_rangefinder: the model has no rangefinders"); return; }
+  int kind[6]; double org[18], dir[18], maxd[6], out[6 * RAY_SLOT];
+  for (int i = 0; i < k; i++) {
+    const double *f = sim_frame(c, nb + hm.rangefinder_site[i]), *q = f + FR_QUAT;
+    kind[i] = RAY_WORLD; maxd[i] = 1e6;   // mj_ray has no range limit
+    for (int j = 0; j < 3; j++) org[3 * i + j] = f[FR_POS + j];
+    dir[3 * i] = 2 * (q[1] * q[3] + q[0] * q[2]); dir[3 * i + 1] = 2 * (q[2] * q[3] - q[0] * q[1]); dir[3 * i + 2] = q[0] * q[0] - q[1] * q[1] - q[2] * q[2] + q[3] * q[3];
+  }
+  if (!c->b->impl->set_rays(kind, org, dir, maxd, k) || !c->b->impl->raycast() || !c->b->impl->get_rays(out)) return;
+  for (int i = 0; i < k; i++) { const double d = out[RAY_SLOT * i], cut = hm.rangefinder_cutoff[i]; ranges[i] = (cut > 0 && d >= 0) ? std::min(cut, d) : d; }
+}
 void cassie_sim_body_velocities(const cassie_sim_t *c, double cvel[6], const char *name) {
   const int b = sim_body(c, name, "cassie_sim_body_velocities");
   for (int k = 0; k < 6; k++) cvel[k] = b < 0 ? 0.0 : sim_frame(c, b)[FR_VEL + k];
@@ -1319,6 +1376,10 @@ int cassie_batch_set_frames(cassie_batch_t *b, const char *const *names, const i
 int cassie_batch_nframes(const cassie_batch_t *b) { return (int)(b->impl->frame_list.size() / 2); }
 int cassie_batch_get_frames(cassie_batch_t *b, double *out) { return b->impl->get("frames", out) ? 0 : -1; }
 int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, double *jacr) { return b->impl->frame_jacobian(frame, jacp, jacr) ? 0 : -1; }
+int cassie_batch_set_rays(cassie_batch_t *b, const int *frame, const double *origin, const double *dir, const double *max_dist, int k) { return b->impl->set_rays(frame, origin, dir, max_dist, k) ? 0 : -1; }
+int cassie_batch_nrays(const cassie_batch_t *b) { return b->impl->nray; }
+int cassie_batch_raycast(cassie_batch_t *b) { return b->impl->raycast() ? 0 : -1; }
+int cassie_batch_get_rays(cassie_batch_t *b, double *out) { return b->impl->get_rays(out) ? 0 : -1; }
 int cassie_batch_dynamics(cassie_batch_t *b) { return b->impl->dynamics() ? 0 : -1; }
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm) { return b->impl->get_dynamics(M, bias, J_eq, eq_err, Icm) ? 0 : -1; }
 int cassie_batch_neq(const cassie_batch_t *b) { return b->impl->hm.neq; }

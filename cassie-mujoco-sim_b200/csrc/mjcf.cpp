@@ -499,7 +499,12 @@ bool compile_mjcf(const std::string &xml_path, HostModel &m, std::string &err) {
     else if (x->tag == "gyro") { t = SENS_GYRO; obj = m.site_id(x->get("site") ? x->get("site") : ""); }
     else if (x->tag == "accelerometer") { t = SENS_ACCEL; obj = m.site_id(x->get("site") ? x->get("site") : ""); }
     else if (x->tag == "magnetometer") { t = SENS_MAG; obj = m.site_id(x->get("site") ? x->get("site") : ""); }
-    else if (x->tag == "rangefinder") continue;   // cassie_no_grav.xml: six rangefinders after the 29 numbers the hot path reads; not modelled
+    else if (x->tag == "rangefinder") {   // cassie_no_grav.xml: six rangefinders after the 29 numbers the hot path reads; recorded apart (cassie_sim_read_rangefinder)
+      const int site = m.site_id(x->get("site") ? x->get("site") : "");
+      if (site < 0) { err = "sensor <rangefinder> refers to an unknown site"; return false; }
+      m.rangefinder_site.push_back(site); m.rangefinder_cutoff.push_back(x->get("cutoff") ? atof(x->get("cutoff")) : 0);
+      continue;
+    }
     else { err = "unsupported sensor <" + x->tag + ">"; return false; }
     if (obj < 0) { err = "sensor <" + x->tag + "> refers to an unknown object"; return false; }
     m.sensor_type.push_back(t); m.sensor_objid.push_back(obj);
@@ -535,6 +540,7 @@ bool save_cmodel(const HostModel &m, const std::string &path) {
   PVI(site_bodyid); PVF(site_pos); PVF(site_quat); PVI(eq_obj1id); PVI(eq_obj2id); PVF(eq_data); PVF(eq_solref); PVF(eq_solimp);
   PVI(actuator_jntid); PVI(actuator_ctrllimited); PVF(actuator_gear); PVF(actuator_ctrlrange); PVF(actuator_user);
   PVI(sensor_type); PVI(sensor_objid); PVF(sensor_user); PVF(sensor_cutoff); PVI(hfield_nrow); PVI(hfield_ncol); PVF(hfield_size);
+  if (!m.rangefinder_site.empty()) { PVI(rangefinder_site); PVF(rangefinder_cutoff); }   // optional: tables of models without rangefinders are unchanged
   puts_(o, "names_body", m.names_body); puts_(o, "names_site", m.names_site); puts_(o, "names_geom", m.names_geom); puts_(o, "names_joint", m.names_joint);
   return (bool)o;
 }
@@ -565,11 +571,14 @@ bool load_cmodel(const std::string &path, HostModel &m, std::string &err) {
     LVI(site_bodyid); LVF(site_pos); LVF(site_quat); LVI(eq_obj1id); LVI(eq_obj2id); LVF(eq_data); LVF(eq_solref); LVF(eq_solimp);
     LVI(actuator_jntid); LVI(actuator_ctrllimited); LVF(actuator_gear); LVF(actuator_ctrlrange); LVF(actuator_user);
     LVI(sensor_type); LVI(sensor_objid); LVF(sensor_user); LVF(sensor_cutoff); LVI(hfield_nrow); LVI(hfield_ncol); LVF(hfield_size);
+    LVI(rangefinder_site); LVF(rangefinder_cutoff);
     else if (key == "names_body") m.names_body = vs; else if (key == "names_site") m.names_site = vs;
     else if (key == "names_geom") m.names_geom = vs; else if (key == "names_joint") m.names_joint = vs;
   }
   if (m.nv <= 0 || (int)m.dof_parentid.size() != m.nv || (int)m.body_parentid.size() != m.nbody) { err = "malformed model table " + path; return false; }
   m.geom_user.resize(m.ngeom, 0); m.geom_group.resize(m.ngeom, 0);   // tables written before these columns existed
+  if (m.rangefinder_cutoff.size() != m.rangefinder_site.size()) { err = "malformed rangefinder entries in " + path; return false; }
+  for (int s : m.rangefinder_site) if (s < 0 || s >= m.nsite) { err = "a rangefinder refers to an unknown site in " + path; return false; }
   return true;
 }
 bool load_model_any(const std::string &path, HostModel &out, std::string &err) {

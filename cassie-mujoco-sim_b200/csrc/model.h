@@ -46,6 +46,9 @@ struct HostModel {
   // sensors
   std::vector<int> sensor_type, sensor_objid;
   std::vector<double> sensor_user, sensor_cutoff;
+  // rangefinders (<rangefinder site= cutoff=>): kept apart from the sensor table, whose 29 numbers the step kernel reads; optional table entries
+  std::vector<int> rangefinder_site;
+  std::vector<double> rangefinder_cutoff;
   // height field (at most one)
   std::vector<int> hfield_nrow, hfield_ncol;
   std::vector<double> hfield_size;

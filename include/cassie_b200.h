@@ -165,6 +165,30 @@ int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, doub
 int cassie_batch_dynamics(cassie_batch_t *b);
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm);
 int cassie_batch_neq(const cassie_batch_t *b);
+/* Terrain sensing: rays cast against each environment's STATIC collision geoms (floor plane, height field, boxes, with the environment's own placement
+ * and terrain) at the CURRENT qpos -- height scans around the pelvis for terrain curricula, and the reference's rangefinders
+ * (cassie_sim_read_rangefinder below; mj_ray).  Moving geoms (the robot's own, the extra free body) are not seen.
+ * cassie_batch_set_rays: k rays (0 .. CASSIE_RAY_MAX; 0 drops the table), ray i from origin[3 i] along dir[3 i] (normalised here) up to max_dist[i],
+ * in frame[i]:
+ *   CASSIE_RAY_HEADING  the root body's position and yaw (the yaw of its x axis on the world xy plane): turns with the heading, stays level
+ *   CASSIE_RAY_ROOT     the root body's pose
+ *   CASSIE_RAY_WORLD    world coordinates, the same for every environment
+ * 0, or -1 with nothing changed (cassie_b200_last_error) for an unknown frame kind, a zero direction, max_dist <= 0 or k out of range.  Every
+ * successful set drops the rows: a device pointer taken before it is no longer valid.
+ * cassie_batch_raycast: one launch on the batch stream (asynchronous) that casts every ray of every environment; it writes nothing but the rows
+ * [n][k][CASSIE_RAY_SLOT] in the batch precision (allocated by the first cast; snapshots, resets and cassie_sim_copy leave them alone):
+ *   distance to the first hit (-1: none within max_dist), world z of the hit (of the ray's end point when none), static geom slot 0..15 (-1), 0
+ * cassie_batch_get_rays: synchronous copy [n][k][CASSIE_RAY_SLOT] doubles; -1 before the first cast after a set.  Device rows:
+ * cassie_batch_device_ptr(b, "rays"), row width k CASSIE_RAY_SLOT. */
+#define CASSIE_RAY_MAX 1024
+#define CASSIE_RAY_SLOT 4
+#define CASSIE_RAY_HEADING 0
+#define CASSIE_RAY_ROOT 1
+#define CASSIE_RAY_WORLD 2
+int cassie_batch_set_rays(cassie_batch_t *b, const int *frame, const double *origin, const double *dir, const double *max_dist, int k);
+int cassie_batch_nrays(const cassie_batch_t *b);
+int cassie_batch_raycast(cassie_batch_t *b);
+int cassie_batch_get_rays(cassie_batch_t *b, double *out);
 /* include/cassiemujoco.h:61-73 (src/cassiemujoco.c:1072-1093): model (per-environment constants, height field, timestep) + full dynamic state */
 cassie_sim_t *cassie_sim_duplicate(const cassie_sim_t *src);
 void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *src);
@@ -228,6 +252,12 @@ void cassie_sim_full_mass_matrix(const cassie_sim_t *c, double M[1024]);
 void cassie_sim_minimal_mass_matrix(const cassie_sim_t *c, double M[256]);
 void cassie_sim_loop_constraint_info(const cassie_sim_t *c, double J_cl[192], double err_cl[6]);
 void cassie_sim_centroid_inertia(const cassie_sim_t *c, double Icm[9]);
+/* the six rangefinders (src/cassiemujoco.c:776-778; example/cassiemujoco.py:175-181 sense_ground): model rangefinder i (<rangefinder site= cutoff=>,
+ * recorded apart from the 29-number sensor table) casts from its site along the site's z axis, at the site poses of the mirrors (the state the last
+ * physics sub-step started from, when MuJoCo evaluates the sensor), as one CASSIE_RAY_WORLD cast on the simulator's batch of one; the distance to the
+ * static terrain, min(cutoff, d) where cutoff > 0, -1 for no hit; no noise, as in the reference.  Slots past the model's rangefinders read 0; a model
+ * without rangefinders gets zeros and a recorded error. */
+void cassie_sim_read_rangefinder(cassie_sim_t *c, double ranges[6]);
 /* model constants for domain randomisation (SURVEY.md 8f-3).  src/cassiemujoco.c:1303-1436, 949-977 (most are defined there without a header
  * declaration; example/cassiemujoco.py:517-610 calls them).  The pointer-returning verbs hand out borrowed read-write host mirrors
  * ([nv], [nbody], [3 nbody], [3 ngeom] doubles, numbered like the reference's mjModel incl. its visual mesh geoms); writes are uploaded
