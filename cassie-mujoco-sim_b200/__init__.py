@@ -25,6 +25,15 @@ DYN_WIDTH, DYN_COLS = 2144, 40
 RAY_HEADING, RAY_ROOT, RAY_WORLD, RAY_MAX, RAY_SLOT = 0, 1, 2, 1024, 4
 RAY_FRAMES = dict(heading=RAY_HEADING, root=RAY_ROOT, world=RAY_WORLD)
 DYN = dict(M=slice(0, 1600), bias=slice(1600, 1640), J_eq=slice(1640, 2120), eq_err=slice(2120, 2132), rcm=slice(2132, 2135))
+# acceleration row (include/cassie_b200.h CASSIE_ACC_*): qacc [40] (column = dof), then per frame f a slot of ACC_SLOT at ACC_QCOLS + ACC_SLOT f holding
+# cacc [6] (com-based [angular; linear]) and 2 pad.  ACC['qacc'] slices the row, ACC['cacc'] a frame's slot
+ACC_QCOLS, ACC_SLOT = 40, 8
+ACC = dict(qacc=slice(0, 40), cacc=slice(0, 6))
+
+
+def acc_width(nframes):
+    """width of an acceleration row with `nframes` frames"""
+    return ACC_QCOLS + ACC_SLOT * nframes
 # slices of a derived-quantity row (CASSIE_AUX_* in include/cassie_b200.h)
 AUX = dict(foot_force=slice(0, 12), toe_force=slice(12, 18), heel_force=slice(18, 24), foot_pos=slice(24, 30), foot_vel=slice(30, 42),
            cm_pos=slice(42, 45), cm_vel=slice(45, 48), angmom=slice(48, 51), obstacle=51, self_collision=52, group_mask=53, ncon=54)
@@ -500,6 +509,31 @@ class CassieBatch:
             raise RuntimeError(_last_error())
         return out
 
+    # ---- accelerations (reference: qacc, get_body_acceleration of example/cassiemujoco.py): by-products of every step and forward
+    def enable_accelerations(self, on=True):
+        """allocate (on) or drop the acceleration rows.  From the next step or forward on, qacc() holds the constraint-solved qacc of the last physics
+        sub-step and body_accelerations() the cacc of every frame of set_frames (zeros for sites); set_frames reallocates the rows to its width"""
+        self.L.cassie_batch_enable_accelerations.argtypes = [C.c_void_p, C.c_int]
+        if self.L.cassie_batch_enable_accelerations(self.h, 1 if on else 0) != 0:
+            raise RuntimeError(_last_error())
+
+    def _accelerations(self, qacc, cacc):
+        self.L.cassie_batch_get_accelerations.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        if self.L.cassie_batch_get_accelerations(self.h, self._dp(qacc) if qacc is not None else None, self._dp(cacc) if cacc is not None else None) != 0:
+            raise RuntimeError(_last_error())
+
+    def qacc(self):
+        """[n, nv] qacc of the last step / forward (after a step: the value the warm start keeps, before the implicit-damping correction)"""
+        out = np.zeros((self.n, self.nv))
+        self._accelerations(out, None)
+        return out
+
+    def body_accelerations(self):
+        """[n, nframes, 6] cacc of the frames (com-based [angular; linear], gravity included as cacc(world) = (0, 0, 0, -g); sites read zero)"""
+        out = np.zeros((self.n, self.nframes(), 6))
+        self._accelerations(None, out)
+        return out
+
     # ---- dynamics at the current state (reference: full_mass_matrix, constraint_jacobian / constraint_error, centroid_inertia of
     # example/cassiemujoco.py): mass matrix, bias forces, connect-equality rows
     def compute_dynamics(self):
@@ -653,8 +687,8 @@ class CassieBatch:
 
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
-        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT]).  set_frames / set_rays reallocate the frame / ray rows: a view
-        taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
+        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC).  set_frames /
+        set_rays reallocate the frame, acceleration and ray rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
         call sync() before reading the view: torch ops on another stream are not ordered after an in-flight step."""
@@ -663,7 +697,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
 
         class _Arr:
@@ -1008,6 +1042,24 @@ class CassieSim:
         self.L.cassie_sim_site_xquat.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_double)]
         self.L.cassie_sim_site_xquat(self.c, name.encode(), a)
         return a[:4]
+
+    def qacc(self):
+        """qacc of the last step / forward (nv entries)"""
+        self.L.cassie_sim_qacc.restype = C.POINTER(C.c_double)
+        self.L.cassie_sim_qacc.argtypes = [C.c_void_p]
+        return np.array(self.L.cassie_sim_qacc(self.c)[:self.nv])
+
+    def get_body_acceleration(self, accel, body_name):
+        """cacc of the body ([angular; linear], com-based) after the last step / forward into accel[6]"""
+        accel[:6] = self._named(self.L.cassie_sim_body_acceleration, body_name, 6)
+
+    def foot_quat(self, quat):
+        """the right-foot-middle site's quaternion into quat[4] (cassie_sim_foot_orient)"""
+        a = (C.c_double * 4)()
+        self.L.cassie_sim_foot_orient.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        self.L.cassie_sim_foot_orient.restype = None
+        self.L.cassie_sim_foot_orient(self.c, a)
+        quat[:4] = a[:4]
 
     def body_vel(self, vel, body_name):
         """cvel of the body ([angular; linear], com-based) into vel[6]; cassie_sim_body_velocities (the reference wrapper names a function its

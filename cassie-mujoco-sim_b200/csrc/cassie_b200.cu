@@ -203,11 +203,14 @@ struct Snap {
   // the frame rows [n][frame_list.size() / 2][FRAME_W] of the batch, with its frame list ((kind, id) pairs); restored only into a batch with the same list
   void *frames = nullptr; std::vector<int> frame_list;
   size_t frame_bytes() const { return (size_t)n * (frame_list.size() / 2) * FRAME_W * esz; }
+  // the acceleration rows [n][acc_width(count)] of the batch (mjData's qacc and the cacc of its frames), if it had them; restored like the frame rows
+  void *acc = nullptr;
+  size_t acc_bytes() const { return (size_t)n * acc_width((int)(frame_list.size() / 2)) * esz; }
   int width(int r) const { const int w[NROWS] = {qw, vw, vw, CST_W, XFRC_W, OBS_W, DFILT_W, EST_W, AUX_W}; return w[r]; }
   int elem(int r) const { return r == R_DFILT ? 4 : (r == R_EST ? 8 : esz); }
   size_t bytes(int r) const { return (size_t)n * width(r) * elem(r); }
 };
-static void snap_delete(Snap *k) { if (!k) return; cudaSetDevice(k->device); for (int r = 0; r < Snap::NROWS; r++) cudaFree(k->rows[r]); cudaFree(k->frames); delete k; }
+static void snap_delete(Snap *k) { if (!k) return; cudaSetDevice(k->device); for (int r = 0; r < Snap::NROWS; r++) cudaFree(k->rows[r]); cudaFree(k->frames); cudaFree(k->acc); delete k; }
 static Snap *snap_new(int device, int n, int esz, int qw, int vw) {
   if (cudaSetDevice(device) != cudaSuccess) return nullptr;
   Snap *k = new Snap(); k->device = device; k->n = n; k->esz = esz; k->qw = qw; k->vw = vw;
@@ -222,8 +225,10 @@ static bool snap_clone_into(Snap *d, const Snap *k) {   // same shape required
     if (!d->rows[r] && cudaMalloc(&d->rows[r], d->bytes(r)) != cudaSuccess) return false;
     if (cudaMemcpy(d->rows[r], k->rows[r], k->bytes(r), cudaMemcpyDefault) != cudaSuccess) return false;
   }
-  if (d->frame_list != k->frame_list) { cudaFree(d->frames); d->frames = nullptr; d->frame_list = k->frame_list; if (k->frames && cudaMalloc(&d->frames, k->frame_bytes()) != cudaSuccess) return false; }
+  if (d->frame_list != k->frame_list) { cudaFree(d->frames); cudaFree(d->acc); d->frames = d->acc = nullptr; d->frame_list = k->frame_list; if (k->frames && cudaMalloc(&d->frames, k->frame_bytes()) != cudaSuccess) return false; }
   if (k->frames && cudaMemcpy(d->frames, k->frames, k->frame_bytes(), cudaMemcpyDefault) != cudaSuccess) return false;
+  if (!k->acc) { cudaFree(d->acc); d->acc = nullptr; }
+  else if ((!d->acc && cudaMalloc(&d->acc, k->acc_bytes()) != cudaSuccess) || cudaMemcpy(d->acc, k->acc, k->acc_bytes(), cudaMemcpyDefault) != cudaSuccess) return false;
   return true;
 }
 
@@ -276,6 +281,9 @@ struct BatchBase {
   virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
   virtual bool get_dynamics(double *M, double *bias, double *J_eq, double *eq_err, double *Icm) = 0;   // what the last mode-5 launch wrote; any pointer may be null
   bool dyn_done = false;                                // a mode-5 launch was enqueued since the rows were allocated
+  // acceleration rows [n][acc_width(count)]: allocated (zero) by enable_accelerations(true), filled by every step / forward launch, reallocated by set_frames
+  virtual bool enable_accelerations(bool on) = 0;
+  virtual bool get_accelerations(double *qacc, double *cacc) = 0;   // qacc [n][nv], cacc [n][count][6]; either may be null
   // terrain rays (raycast.inl): the table is checked as a whole before anything changes; k = 0 drops it.  The rows [n][k][RAY_SLOT] are allocated by
   // the first cast after a set and are a query result, not state
   virtual bool set_rays(const int *frame, const double *origin, const double *dir, const double *max_dist, int k) = 0;
@@ -304,7 +312,7 @@ template <typename real> struct Batch : BatchBase {
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -511,7 +519,7 @@ template <typename real> struct Batch : BatchBase {
     // and stepping, and unpacks chunk c while the later ones are stepping; the kernels of consecutive chunks overlap at their edges (a chunk's CTAs start
     // on the SMs the previous chunk's CTAs have left, while its last observation rows are still draining over PCIe).  Chunks are whole rounds of the
     // resident warps when the batch is worked off in more than two rounds, equal parts otherwise.
-    const int inst = (A.cenv || A.aux || A.task || A.frames || (A.dbg && !DBG_IN_ALL_INSTANCES)) ? 1 : (A.est ? 2 : 0), slots = cfg[inst].resident_ctas * cfg[inst].wpb;
+    const int inst = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES)) ? 1 : (A.est ? 2 : 0), slots = cfg[inst].resident_ctas * cfg[inst].wpb;
     int nchunk = 1, c0[AOS_MAXC + 1] = {0};
     if (state_out && n >= 1024 && aos_chunks > 1) {
       if (n <= 2 * slots) { nchunk = aos_chunks; for (int c = 1; c < nchunk; c++) c0[c] = (int)((size_t)n * c / nchunk + 31) / 32 * 32; }
@@ -661,8 +669,10 @@ template <typename real> struct Batch : BatchBase {
       if (!k->rows[r]) CUDA_OK(cudaMalloc(&k->rows[r], k->bytes(r)));
       CUDA_OK(cudaMemcpyAsync(k->rows[r], snap_src(r), k->bytes(r), cudaMemcpyDeviceToDevice, stream));
     }
-    if (k->frame_list != frame_list) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(k->frames)); k->frames = nullptr; k->frame_list = frame_list; if (A.frames) CUDA_OK(cudaMalloc(&k->frames, k->frame_bytes())); }
+    if (k->frame_list != frame_list) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(k->frames)); CUDA_OK(cudaFree(k->acc)); k->frames = k->acc = nullptr; k->frame_list = frame_list; if (A.frames) CUDA_OK(cudaMalloc(&k->frames, k->frame_bytes())); }
     if (A.frames) CUDA_OK(cudaMemcpyAsync(k->frames, A.frames, k->frame_bytes(), cudaMemcpyDeviceToDevice, stream));
+    if (A.acc) { if (!k->acc) CUDA_OK(cudaMalloc(&k->acc, k->acc_bytes())); CUDA_OK(cudaMemcpyAsync(k->acc, A.acc, k->acc_bytes(), cudaMemcpyDeviceToDevice, stream)); }
+    else if (k->acc) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(k->acc)); k->acc = nullptr; }
     return sync();
   }
   bool snap_set(const Snap *k, const unsigned char *mask) override {
@@ -686,6 +696,15 @@ template <typename real> struct Batch : BatchBase {
         const int w = (int)(frame_list.size() / 2) * FRAME_W;
         if (sizeof(real) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)A.frames, (const unsigned long long *)k->frames, w, dm, n);
         else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)A.frames, (const unsigned int *)k->frames, w, dm, n);
+        CUDA_OK(cudaGetLastError());
+      }
+    }
+    if (A.acc && k->acc && k->frame_list == frame_list) {   // acceleration rows: likewise
+      if (!dm) CUDA_OK(cudaMemcpyAsync(A.acc, k->acc, k->acc_bytes(), cudaMemcpyDeviceToDevice, stream));
+      else {
+        const int w = acc_width(A.nfr);
+        if (sizeof(real) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)A.acc, (const unsigned long long *)k->acc, w, dm, n);
+        else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)A.acc, (const unsigned int *)k->acc, w, dm, n);
         CUDA_OK(cudaGetLastError());
       }
     }
@@ -796,13 +815,36 @@ template <typename real> struct Batch : BatchBase {
       list.push_back(kinds[f]); list.push_back(id);
     }
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
-    CUDA_OK(cudaFree(A.frames)); CUDA_OK(cudaFree((void *)A.ftab)); A.frames = nullptr; A.ftab = nullptr; A.nfr = 0; frame_list.clear();
-    if (count == 0) return true;
-    real *t = nullptr;
-    CUDA_OK(cudaMalloc(&t, sizeof(real) * tab.size())); A.ftab = t;
-    CUDA_OK(cudaMemcpy(t, tab.data(), sizeof(real) * tab.size(), cudaMemcpyHostToDevice));
-    CUDA_OK(cudaMalloc(&A.frames, sizeof(real) * n * count * FRAME_W)); CUDA_OK(cudaMemset(A.frames, 0, sizeof(real) * n * count * FRAME_W));
-    A.nfr = count; frame_list = list;
+    const bool acc_on = A.acc != nullptr;
+    CUDA_OK(cudaFree(A.frames)); CUDA_OK(cudaFree((void *)A.ftab)); CUDA_OK(cudaFree(A.acc)); A.frames = nullptr; A.ftab = nullptr; A.acc = nullptr; A.nfr = 0; frame_list.clear();
+    if (count > 0) {
+      real *t = nullptr;
+      CUDA_OK(cudaMalloc(&t, sizeof(real) * tab.size())); A.ftab = t;
+      CUDA_OK(cudaMemcpy(t, tab.data(), sizeof(real) * tab.size(), cudaMemcpyHostToDevice));
+      CUDA_OK(cudaMalloc(&A.frames, sizeof(real) * n * count * FRAME_W)); CUDA_OK(cudaMemset(A.frames, 0, sizeof(real) * n * count * FRAME_W));
+      A.nfr = count; frame_list = list;
+    }
+    return !acc_on || enable_accelerations(true);   // the acceleration rows follow the new frame list: its width, zero until the next launch
+  }
+  // ---- acceleration rows (qacc and the cacc of every frame), filled by every step / forward launch from then on
+  bool enable_accelerations(bool on) override {
+    CUDA_OK(cudaSetDevice(device));
+    const size_t bytes = sizeof(real) * n * acc_width(A.nfr);
+    if (on && !A.acc) { CUDA_OK(cudaMalloc(&A.acc, bytes)); CUDA_OK(cudaMemsetAsync(A.acc, 0, bytes, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
+    if (!on && A.acc) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.acc)); A.acc = nullptr; }
+    return true;
+  }
+  bool get_accelerations(double *qacc, double *cacc) override {
+    if (!A.acc) { set_err("cassie_batch_get_accelerations: no acceleration rows (cassie_batch_enable_accelerations)"); return false; }
+    const int w = acc_width(A.nfr), nv = hm.nv;
+    CUDA_OK(cudaSetDevice(device));
+    h_tmp.resize((size_t)n * w);
+    CUDA_OK(cudaMemcpyAsync(h_tmp.data(), A.acc, sizeof(real) * n * w, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    for (int e = 0; e < n; e++) {
+      const real *r = &h_tmp[(size_t)e * w];
+      if (qacc) for (int i = 0; i < nv; i++) qacc[(size_t)e * nv + i] = (double)r[AC_QACC + i];
+      if (cacc) for (int f = 0; f < A.nfr; f++) for (int k = 0; k < 6; k++) cacc[((size_t)e * A.nfr + f) * 6 + k] = (double)r[AC_CACC + AC_SLOT * f + k];
+    }
     return true;
   }
   // the Jacobian of frame `frame` at the current state of every environment: one mode-4 launch (kinematics and centre of mass only, nothing else
@@ -896,13 +938,13 @@ template <typename real> struct Batch : BatchBase {
     A.nsub = nsub_override;
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
-    const int ext = (A.cenv || A.aux || A.task || A.frames || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    const int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | ((A.frames || mode == 5) ? F_FR : 0);   // frame rows and the dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -939,6 +981,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "est_out")) { if (!A.est) { set_err("the in-kernel estimator is not enabled (cassie_batch_enable_estimator_device)"); return false; } return d2h(A.obs, OBS_W, EO_W, OB_EST_OUT, out); }
     if (!strcmp(f, "aux")) { if (!A.aux) { set_err("derived quantities are not enabled (cassie_batch_enable_aux)"); return false; } return d2h(A.aux, AUX_W, AUX_W, 0, out); }
     if (!strcmp(f, "frames")) { if (!A.frames) { set_err("no frames are set (cassie_batch_set_frames)"); return false; } return d2h(A.frames, A.nfr * FRAME_W, A.nfr * FRAME_W, 0, out); }
+    if (!strcmp(f, "acc")) { if (!A.acc) { set_err("no acceleration rows (cassie_batch_enable_accelerations)"); return false; } return d2h(A.acc, acc_width(A.nfr), acc_width(A.nfr), 0, out); }
     set_err(std::string("unknown field ") + f); return false;
   }
   bool h2d(real *dst, int w, int take, int off, const double *in) {
@@ -955,6 +998,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "time")) return h2d(A.cst, CST_W, 1, CS_TIME, in);
     if (!strcmp(f, "sto")) return h2d(A.cst, CST_W, 1, CS_STO, in);
     if (!strcmp(f, "cst")) return h2d(A.cst, CST_W, CST_W, 0, in);
+    if (!strcmp(f, "acc")) { if (!A.acc) { set_err("no acceleration rows (cassie_batch_enable_accelerations)"); return false; } return h2d(A.acc, acc_width(A.nfr), acc_width(A.nfr), 0, in); }
     set_err(std::string("unknown field ") + f); return false;
   }
   bool set_xfrc(const double *xfrc, int body) override {
@@ -967,7 +1011,7 @@ template <typename real> struct Batch : BatchBase {
   void *dev_ptr(const char *f) override {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
-    if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn;
+    if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays;
     return nullptr;
   }
@@ -994,6 +1038,7 @@ using namespace cassie;
 static_assert(CASSIE_RAY_MAX == RAY_MAX && CASSIE_RAY_SLOT == RAY_SLOT && CASSIE_RAY_HEADING == RAY_HEADING && CASSIE_RAY_ROOT == RAY_ROOT && CASSIE_RAY_WORLD == RAY_WORLD, "ray table and rows");
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
+static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
 static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
 struct cassie_batch { BatchBase *impl; std::vector<double> obs, radio; };
 struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[64], qvel_dev[64], time_dev, aux[AUX_W]; std::vector<float> hfield, hfield_dev; std::string path; double timestep = 0, timestep_dev = 0;
@@ -1001,7 +1046,9 @@ struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[6
   std::vector<double> m_gpos, m_gquat, m_gsize, m_gpos_dev, m_gquat_dev, m_gsize_dev;
   // every body and every site is a frame of the simulator's batch (bodies first); host mirrors laid out like mjData's xpos[nbody][3], xquat[nbody][4],
   // site_xpos[nsite][3], so that the borrowed pointers of cassie_sim_xpos / xquat / site_xpos index across bodies as &d->xpos[3 * id] does
-  std::vector<double> frames, xpos, xquat, site_xpos; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
+  std::vector<double> frames, xpos, xquat, site_xpos;
+  // the acceleration row of the simulator's batch (qacc, then the cacc of every body and site frame) and the nv-entry qacc mirror cassie_sim_qacc lends out
+  std::vector<double> acc, qacc; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
 
 // cassie_state_t (include/cassiemujoco.h:434-463): a device-resident snapshot of one simulator's rows plus the host mirrors the reference hands out as
 // borrowed pointers (time, qpos, qvel); the snapshot is allocated by the first cassie_get_state, which also fixes the owning simulator's sizes
@@ -1038,7 +1085,8 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "qpos")) return b->impl->hm.nq > 36 ? QPOS_W_XB : QPOS_W_MAIN; if (!strcmp(field, "qvel")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN;
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
-  if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT; return -1;
+  if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
+  if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
 void cassie_batch_reset(cassie_batch_t *b, const unsigned char *mask) { b->impl->reset(mask); b->impl->sync(); b->impl->reset_estimator(mask); b->impl->reset_estimator_device(mask); }   // a fresh cassie_sim_t has a fresh estimator
@@ -1122,6 +1170,7 @@ static void sim_pull(cassie_sim_t *c) {
     for (int b = 0; b < nb; b++) { const double *f = &c->frames[(size_t)b * FRAME_W]; for (int k = 0; k < 3; k++) c->xpos[3 * b + k] = f[FR_POS + k]; for (int k = 0; k < 4; k++) c->xquat[4 * b + k] = f[FR_QUAT + k]; }
     for (int s = 0; s < ns; s++) for (int k = 0; k < 3; k++) c->site_xpos[3 * s + k] = c->frames[(size_t)(nb + s) * FRAME_W + FR_POS + k];
   }
+  if (!c->acc.empty() && c->b->impl->get("acc", c->acc.data())) for (int i = 0; i < c->b->impl->hm.nv; i++) c->qacc[i] = c->acc[AC_QACC + i];
   memcpy(c->qpos_dev, c->qpos, sizeof c->qpos); memcpy(c->qvel_dev, c->qvel, sizeof c->qvel); c->time_dev = c->time;
 }
 static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote through the borrowed pointers
@@ -1150,6 +1199,8 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
     for (const std::string &s : hm.names_site) { names.push_back(s.c_str()); kinds.push_back(1); }
     if ((int)names.size() <= FRAME_MAX && (int)hm.names_body.size() == hm.nbody && b->impl->set_frames(names.data(), kinds.data(), (int)names.size())) {
       c->frames.assign(names.size() * FRAME_W, 0.0); c->xpos.assign(3 * hm.names_body.size(), 0.0); c->xquat.assign(4 * hm.names_body.size(), 0.0); c->site_xpos.assign(3 * hm.names_site.size(), 0.0); } }
+  c->qacc.assign(64, 0.0);   // ... and the acceleration row (cassie_sim_qacc, cassie_sim_body_acceleration)
+  if (b->impl->enable_accelerations(true)) c->acc.assign(acc_width((int)(c->frames.size() / FRAME_W)), 0.0);
   b->impl->step(0, 1);   // populate them like the sensordata
   b->impl->enable_estimator_device(true);   // ... and the estimator (toe / heel forces, filters) inside the kernel, as state_output_step runs in every cassie_sim_step_pd (src/cassiemujoco.c:1156)
   sim_pull(c);
@@ -1234,6 +1285,17 @@ void cassie_sim_read_rangefinder(cassie_sim_t *c, double ranges[6]) {
 void cassie_sim_body_velocities(const cassie_sim_t *c, double cvel[6], const char *name) {
   const int b = sim_body(c, name, "cassie_sim_body_velocities");
   for (int k = 0; k < 6; k++) cvel[k] = b < 0 ? 0.0 : sim_frame(c, b)[FR_VEL + k];
+}
+// ---- accelerations (src/cassiemujoco.c:1216-1219, 1762-1779): the acceleration row the last step / forward left behind, like the velocities above.  The
+// reference reruns mj_comVel + mj_rnePostConstraint on mjData at call time; the two differ only when qvel was written through the borrowed pointer since.
+double *cassie_sim_qacc(cassie_sim_t *c) { return c->qacc.data(); }
+void cassie_sim_body_acceleration(const cassie_sim_t *c, double accel[6], const char *name) {
+  const int b = sim_body(c, name, "cassie_sim_body_acceleration");
+  for (int k = 0; k < 6; k++) accel[k] = (b < 0 || c->acc.empty()) ? 0.0 : c->acc[AC_CACC + AC_SLOT * b + k];
+}
+void cassie_sim_foot_orient(const cassie_sim_t *c, double corient[4]) {
+  const int s = sim_site(c, "right-foot-middle", "cassie_sim_foot_orient");
+  for (int k = 0; k < 4; k++) corient[k] = s < 0 ? 0.0 : sim_frame(c, (int)c->xquat.size() / 4 + s)[FR_QUAT + k];
 }
 void cassie_sim_body_contact_force(const cassie_sim_t *c, double cfrc[6], const char *name) {
   const int b = sim_body(c, name, "cassie_sim_body_contact_force");
@@ -1329,6 +1391,11 @@ void cassie_sim_full_reset(cassie_sim_t *c) {
   c->b->impl->set("cst", cst.data());
   memcpy(c->qpos, q, sizeof q); memset(c->qvel, 0, sizeof c->qvel);   // 35 entries only (:2025): qpos beyond them (the cup of cassie_tray_box.xml) keeps its values
   c->b->impl->set("qpos", c->qpos); c->b->impl->set("qvel", c->qvel); cassie_batch_clear_forces(c->b);
+  if (!c->acc.empty()) {   // qacc <- 0 (:2025): what the reference's query then gives, with qvel = qacc = 0, is cacc = (0, 0, 0, -g) for every body
+    const HostModel &hm = c->b->impl->hm; std::vector<double> row(c->acc.size(), 0.0);
+    for (int b = 0; b < (int)c->xquat.size() / 4; b++) for (int k = 0; k < 3; k++) row[AC_CACC + AC_SLOT * b + 3 + k] = -hm.gravity[k];
+    c->b->impl->set("acc", row.data());
+  }
   c->b->impl->reset_estimator(nullptr); c->b->impl->reset_estimator_device(nullptr);   // state_output_setup (src/cassiemujoco.c:2032) restarts the estimator's filters
   sim_pull(c);
 }
@@ -1383,6 +1450,8 @@ int cassie_batch_get_rays(cassie_batch_t *b, double *out) { return b->impl->get_
 int cassie_batch_dynamics(cassie_batch_t *b) { return b->impl->dynamics() ? 0 : -1; }
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm) { return b->impl->get_dynamics(M, bias, J_eq, eq_err, Icm) ? 0 : -1; }
 int cassie_batch_neq(const cassie_batch_t *b) { return b->impl->hm.neq; }
+int cassie_batch_enable_accelerations(cassie_batch_t *b, int on) { return b->impl->enable_accelerations(on != 0) ? 0 : -1; }
+int cassie_batch_get_accelerations(cassie_batch_t *b, double *qacc, double *cacc) { return b->impl->get_accelerations(qacc, cacc) ? 0 : -1; }
 
 // ---- legacy verbs RL wrappers call around cassie_sim_step_pd (src/cassiemujoco.c:1072-1093, 1137-1145, 1159-1181, 1196-1225, 1974-2000, 2086-2092, 3380-3452)
 // the dynamic subset of cassie_out_t from an observation row, the rest as cassie_out_init leaves it (:672-734)

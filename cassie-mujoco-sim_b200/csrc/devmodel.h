@@ -187,6 +187,13 @@ constexpr int FRAME_JAC_W = 6 * FJ_COLS;
 constexpr int DY_COLS = 40, DY_EQ_ROWS = 3 * ME;
 constexpr int DY_M = 0, DY_BIAS = DY_M + DY_COLS * DY_COLS, DY_JEQ = DY_BIAS + DY_COLS, DY_EQPOS = DY_JEQ + DY_EQ_ROWS * DY_COLS, DY_RCM = DY_EQPOS + DY_EQ_ROWS;
 constexpr int DYN_W = (DY_RCM + 3 + 31) / 32 * 32;
+// accelerations (optional, cassie_batch_enable_accelerations): per environment a row [ACC_W(count)] filled in the last sub-step of a step or forward
+// launch (F_FR instances): the constraint-solved qacc (cassie_sim_qacc, src/cassiemujoco.c:1216-1219; column = dof as in the dynamics row, zeros beyond
+// nv), then per frame of the batch's frame list cacc after mj_comVel + mj_rnePostConstraint (cassie_sim_body_acceleration, :1762-1771) in com-based
+// coordinates (angular 3, linear 3) and 2 pad.  Site slots read zero; a body without dofs reads its parent's cacc.
+constexpr int AC_QCOLS = 40, AC_SLOT = 8;
+constexpr int AC_QACC = 0, AC_CACC = AC_QCOLS;
+CASSIE_HD inline constexpr int acc_width(int nframes) { return AC_QCOLS + AC_SLOT * nframes; }
 
 // ---- per-warp scratch (in units of `real`)
 constexpr int S_XPOS = 0;                       // [32][3]
@@ -197,7 +204,7 @@ constexpr int S_QLD = S_CDOF + 192;             // [320] (qM itself lives in a g
 constexpr int S_DINV = S_QLD + NM_MAX;          // [32]
 constexpr int S_DSQI = S_DINV + 32;             // [32]
 constexpr int S_QPOS = S_DSQI + 32;             // [44]
-constexpr int S_VEC = S_QPOS + 44;              // [6][32] general vectors ([96..127]: IMU stash; [128..159]: exchange buffer; [160..183]: extra-body qvel / qacc_smooth / qacc_ws / qacc; [184..186]: centre of mass)
+constexpr int S_VEC = S_QPOS + 44;              // [6][32] general vectors ([96..127]: IMU stash; [128..159]: exchange buffer; [160..183]: extra-body qvel / qacc_smooth / qacc_ws / qacc (F_FR instances, for the acceleration row); [184..186]: centre of mass)
 constexpr int S_CON = S_VEC + 192;              // [MAXCON][16]
 constexpr int S_EFC = S_CON + MAXCON * 16;               // [NEFC][4]: row-build scalars {.., pos, src, ineq} then solver constants {b, 1/A, A, +-R}
 constexpr int S_Y = S_EFC + 4 * NEFC;           // [NEFC][ystride] constraint matrix; before the constraint stage it holds the temporaries below

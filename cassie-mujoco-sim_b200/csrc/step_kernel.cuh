@@ -22,6 +22,7 @@ template <typename real> struct EnvArrays {
   const real *ftab; real *frames; int nfr;   // frame table [nfr][FT_W] and rows [n][nfr][FRAME_W] (read by the F_FR instances only); after genv for the same reason
   real *jac; int jfr;                         // mode 4: Jacobian rows [n][FRAME_JAC_W] of frame jfr (F_FR instances)
   real *dyn;                                  // mode 5: dynamics rows [n][DYN_W] (F_FR instances)
+  real *acc;                                  // modes 0 / 1: acceleration rows [n][acc_width(nfr)] or null (F_FR instances)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -117,6 +118,7 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     // ... and its observation row goes back the same way as soon as the environment is done, overlapped with the environments still stepping (sending it
     // right after the controller stage, before the physics, was measured: no end-to-end gain, -2.8 % on every instance from the longer-lived pointer)
     if (A.obs_host) { for (int i = l; i < OBS_W; i += 32) A.obs_host[(size_t)env * OBS_W + i] = A.obs[(size_t)env * OBS_W + i]; }
+    if constexpr ((FEAT & F_FR) != 0) { if (A.acc) accel_row(cm, sm, A.acc, A.ftab, A.frames, A.nfr, env, (FEAT & F_XB) ? cm.xb : -1); }   // from what the last sub-step left in shared memory
     __syncwarp();
   }
 }

@@ -165,6 +165,27 @@ int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, doub
 int cassie_batch_dynamics(cassie_batch_t *b);
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm);
 int cassie_batch_neq(const cassie_batch_t *b);
+/* Accelerations, as step / forward by-products (joint-acceleration penalties, impact rewards, IMU-like observations at any body, acceleration-level
+ * controllers): per environment a row [CASSIE_ACC_WIDTH(count)] in the batch precision, count = cassie_batch_nframes, filled in the last physics sub-step
+ * of every step and forward launch (also the forward of cassie_batch_reset):
+ *   CASSIE_ACC_QACC [40]  qacc (cassie_sim_qacc): the constraint-solved acceleration of that sub-step -- after a step the value the warm start keeps,
+ *                         before mj_Euler's implicit-damping correction; after a forward the solved qacc, warm start untouched.  Column = dof (main
+ *                         tree 0..31, the extra free body 32..37), zeros beyond nv
+ *   CASSIE_ACC_CACC + CASSIE_ACC_SLOT f  [6] per frame f of the frame list: body: cacc (cassie_sim_body_acceleration: mj_comVel + mj_rnePostConstraint
+ *                         on the state the step left -- the new qvel, that sub-step's cdof, its qacc -- com-based [angular; linear], gravity included as
+ *                         cacc(world) = (0, 0, 0, -g)); a body without dofs reads its parent's; site: 0.  Then 2 pad
+ * cassie_batch_enable_accelerations: on = 1 allocates the rows (zero until the next step or forward), 0 drops them; 0 / -1.  A batch with rows runs the
+ * extended frame instance of the step kernel.  cassie_batch_set_frames reallocates them to the new width, zeroed.  Snapshots carry them and restore
+ * them into a batch with the same frame list and rows.
+ * cassie_batch_get_accelerations: synchronous copy, qacc [n][nv], cacc [n][count][6]; either may be NULL; -1 (error recorded, nothing copied) without
+ * rows.  Device rows: cassie_batch_device_ptr(b, "acc"), width cassie_batch_row_width(b, "acc"). */
+#define CASSIE_ACC_QACC 0
+#define CASSIE_ACC_QCOLS 40
+#define CASSIE_ACC_CACC 40
+#define CASSIE_ACC_SLOT 8
+#define CASSIE_ACC_WIDTH(count) (40 + 8 * (count))
+int cassie_batch_enable_accelerations(cassie_batch_t *b, int on);
+int cassie_batch_get_accelerations(cassie_batch_t *b, double *qacc, double *cacc);
 /* Terrain sensing: rays cast against each environment's STATIC collision geoms (floor plane, height field, boxes, with the environment's own placement
  * and terrain) at the CURRENT qpos -- height scans around the pelvis for terrain curricula, and the reference's rangefinders
  * (cassie_sim_read_rangefinder below; mj_ray).  Moving geoms (the robot's own, the extra free body) are not seen.
@@ -243,6 +264,13 @@ void cassie_sim_get_jacobian(cassie_sim_t *c, double *jac, const char *name);
 void cassie_sim_get_jacobian_full(cassie_sim_t *c, double *jac, double *jac_rot, const char *name);
 void cassie_sim_get_jacobian_full_site(cassie_sim_t *c, double *jac, double *jac_rot, const char *name);
 void cassie_sim_relative_pose(double pos1[3], double quat1[4], double pos2[3], double quat2[4], double pos2_in_pos1[3], double quat2_in_quat1[4]);
+/* accelerations of the simulator (src/cassiemujoco.c:1216-1219, 1762-1779), from its acceleration row: what the last step / forward left behind, like
+ * cassie_sim_body_velocities.  cassie_sim_qacc: borrowed nv-entry host mirror.  cassie_sim_body_acceleration: cacc of the body (com-based [angular;
+ * linear]); an unknown name gives zeros and records an error.  cassie_sim_foot_orient: the right-foot-middle site quaternion, as cassie_sim_site_xquat
+ * gives it; zeros and an error for a model without that site.  cassie_sim_full_reset zeroes qacc and sets every body to (0, 0, 0, -g). */
+double *cassie_sim_qacc(cassie_sim_t *c);
+void cassie_sim_body_acceleration(const cassie_sim_t *c, double accel[6], const char *name);
+void cassie_sim_foot_orient(const cassie_sim_t *c, double corient[4]);
 /* dynamics of the simulator at its current state (src/cassiemujoco.c:1647-1749), one dynamics launch each, then host arithmetic: the 32 x 32 main-tree
  * block of M; its rows / columns {0..8, 12, 18..21, 25, 31}; the 3 + 3 rows (32 columns) of the connects whose body1 is left- / right-achilles-rod
  * and their errors (zeros and an error recorded when the model has none); and the reference's centroid inertia, m = M[0][0], I_p = M[3:6, 3:6],
@@ -434,7 +462,7 @@ int cassie_batch_hfield_nrow(const cassie_batch_t *b);
 int cassie_batch_hfield_ncol(const cassie_batch_t *b);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20]) in the batch precision; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count]) in the batch precision; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
