@@ -24,6 +24,8 @@ DYN_WIDTH, DYN_COLS = 2144, 40
 # the ray's end point when none), static geom slot (-1: none), pad
 RAY_HEADING, RAY_ROOT, RAY_WORLD, RAY_MAX, RAY_SLOT = 0, 1, 2, 1024, 4
 RAY_FRAMES = dict(heading=RAY_HEADING, root=RAY_ROOT, world=RAY_WORLD)
+# depth camera (include/cassie_b200.h CASSIE_CAM_*): largest image side
+CAM_MAXDIM = 256
 DYN = dict(M=slice(0, 1600), bias=slice(1600, 1640), J_eq=slice(1640, 2120), eq_err=slice(2120, 2132), rcm=slice(2132, 2135))
 # acceleration row (include/cassie_b200.h CASSIE_ACC_*): qacc [40] (column = dof), then per frame f a slot of ACC_SLOT at ACC_QCOLS + ACC_SLOT f holding
 # cacc [6] (com-based [angular; linear]) and 2 pad.  ACC['qacc'] slices the row, ACC['cacc'] a frame's slot
@@ -606,6 +608,41 @@ class CassieBatch:
         """[n, k] torch view (no copy) of the world z of each ray's hit, or of its end point when it hits nothing, from the last raycast()"""
         return self.torch_view('rays')[:, 1::RAY_SLOT]
 
+    # ---- depth camera (the reference's CassieVis attach_cam / init_depth / draw_depth, example/cassietest_depth.py): one camera per batch, rendered at
+    # the CURRENT state of every environment; the static geoms with each environment's own placement and terrain, and the robot's collision geoms
+    def set_camera(self, name=None, body=None, pos=None, quat=None, fovy=45.0, width=64, height=64, zfar=5.0):
+        """a fixed <camera> of the model by name (e.g. 'egocentric' of cassie_depth.xml), or a camera mounted on a body: pos / quat in the body frame,
+        fovy the full vertical angle in degrees.  The camera looks along its -z axis with +y up.  width = 0 drops the camera.  Reallocates the rows: a
+        torch_view('depth') taken before it must not be used after it."""
+        if width == 0 or name is not None:
+            self.L.cassie_batch_set_camera.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_double]
+            rc = self.L.cassie_batch_set_camera(self.h, None if name is None else name.encode(), int(width), int(height), float(zfar))
+        else:
+            if body is None:
+                raise ValueError('set_camera needs a camera name or a body to mount the camera on')
+            p = np.ascontiguousarray(np.zeros(3) if pos is None else np.asarray(pos, dtype=np.float64).reshape(3))
+            q = np.ascontiguousarray(np.array([1.0, 0, 0, 0]) if quat is None else np.asarray(quat, dtype=np.float64).reshape(4))
+            self.L.cassie_batch_set_camera_mount.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, C.c_int, C.c_int, C.c_double]
+            rc = self.L.cassie_batch_set_camera_mount(self.h, body.encode(), self._dp(p), self._dp(q), float(fovy), int(width), int(height), float(zfar))
+        if rc != 0:
+            raise RuntimeError(_last_error())
+        self._cam_hw = (int(height), int(width)) if width else None
+
+    def render_depth(self):
+        """enqueue one depth render of every environment on the batch's stream (asynchronous), at the CURRENT state; nothing else is written"""
+        self.L.cassie_batch_render_depth.argtypes = [C.c_void_p]
+        if self.L.cassie_batch_render_depth(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def depth(self):
+        """[n, height, width] z-depths (metres, row 0 at the top; zfar where nothing is hit) of the last render_depth()"""
+        hw = getattr(self, '_cam_hw', None)
+        out = np.zeros((self.n,) + (hw or (0, 0)))
+        self.L.cassie_batch_get_depth.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        if hw is None or self.L.cassie_batch_get_depth(self.h, self._dp(out)) != 0:
+            raise RuntimeError(_last_error() if hw else 'no camera is set (set_camera)')
+        return out
+
     def query(self):
         """refresh the centre-of-mass slots of the aux rows for the CURRENT state (nothing else is written)."""
         if self.L.cassie_batch_query(self.h) != 0:
@@ -687,8 +724,8 @@ class CassieBatch:
 
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
-        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC).  set_frames /
-        set_rays reallocate the frame, acceleration and ray rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
+        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width]).  set_frames /
+        set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
         call sync() before reading the view: torch ops on another stream are not ordered after an in-flight step."""
@@ -697,14 +734,15 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
 
         class _Arr:
             pass
         a = _Arr()
         a.__cuda_array_interface__ = dict(shape=(self.n, width), typestr=ts, data=(ptr, False), version=2)
-        return torch.as_tensor(a, device='cuda')
+        t = torch.as_tensor(a, device='cuda')
+        return t.view(self.n, *self._cam_hw) if field == 'depth' else t
 
 
 class cassie_user_in_t(C.Structure):

@@ -21,6 +21,7 @@
 #include "estimator_host.h"
 #include "step_kernel.cuh"
 #include "raycast.inl"
+#include "camera.inl"
 
 // the step-kernel instances live in their own translation units (step_inst.cu, one compilation per instance)
 #define CASSIE_STEP_ENTRY(tag) extern "C" const void *cassie_step_entry_##tag(void);
@@ -35,6 +36,7 @@ CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_S
 namespace cassie {
 
 template <typename real> cudaError_t launch_raycast(const RayArgs<real> &A, int device, cudaStream_t stream);   // raycast.cu
+template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int device, cudaStream_t stream);   // camera.cu
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
@@ -290,6 +292,13 @@ struct BatchBase {
   virtual bool raycast() = 0;                           // one launch (asynchronous) at the current qpos
   virtual bool get_rays(double *out) = 0;               // [n][k][RAY_SLOT] of the last cast
   int nray = 0; bool rays_done = false;                 // rays in the table; a cast was enqueued since the table was set
+  // the depth camera (camera.inl): one per batch, mounted on a body; a set is checked before anything changes, width 0 drops it.  The rows
+  // [n][height][width] are allocated by the first render after a set and are a query result, not state
+  struct Camera { int body = -1, width = 0, height = 0; double pos[3] = {0, 0, 0}, quat[4] = {1, 0, 0, 0}, fovy = 45, zfar = 1; } cam;
+  bool depth_done = false;                              // a render was enqueued since the camera was set
+  virtual bool set_camera(int body, const double *pos, const double *quat, double fovy, int width, int height, double zfar, const char *verb) = 0;
+  virtual bool render_depth() = 0;                      // one launch (asynchronous) at the current qpos
+  virtual bool get_depth(double *out) = 0;              // [n][height][width] of the last render
   std::vector<int> frame_list;                          // (kind, id) per frame of the current frame table
   int nsub_override = 0;                                // > 0: physics sub-steps per control tick of the next launches (cassie_sim_step_pd_no2khz)
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
@@ -308,11 +317,12 @@ template <typename real> struct Batch : BatchBase {
   bool task_from_aos = false;   // the task-PD rows were created by the AoS entry point's forwarding (not by cassie_batch_set_task_pd)
   float *d_hfield = nullptr; unsigned char *d_mask = nullptr; DevModel<real> h_model_copy{}; int geom_dev[256]; void *d_row = nullptr;
   real *d_rtab = nullptr, *d_rays = nullptr;   // ray table (RT_HDR + nray RT_W) and the rows of the last cast
+  real *d_depth = nullptr;                     // depth rows of the last render
   real *d_genv = nullptr;                  // A.genv: [n][GEOM_ENV_W] per-environment static-geom placement, allocated by the first per-environment placement
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -917,6 +927,38 @@ template <typename real> struct Batch : BatchBase {
     if (!out) { set_err("cassie_batch_get_rays: out is required"); return false; }
     return d2h(d_rays, nray * RAY_SLOT, nray * RAY_SLOT, 0, out);
   }
+  bool set_camera(int body, const double *pos, const double *quat, double fovy, int width, int height, double zfar, const char *verb) override {
+    Camera c; std::string err;
+    if (width != 0) {
+      if (body < 0 || body >= hm.nbody) { set_err(std::string(verb) + ": unknown body"); return false; }
+      if (!camera_check(pos, quat, fovy, width, height, zfar, c.quat, err)) { set_err(std::string(verb) + ": " + err); return false; }
+      c.body = body; c.width = width; c.height = height; c.fovy = fovy; c.zfar = zfar;
+      for (int i = 0; i < 3; i++) c.pos[i] = pos[i];
+    }
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_depth)); d_depth = nullptr; depth_done = false;
+    cam = c;
+    return true;
+  }
+  bool render_depth() override {
+    if (!cam.width) { set_err("cassie_batch_render_depth: no camera is set (cassie_batch_set_camera)"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    if (!d_depth) CUDA_OK(cudaMalloc(&d_depth, sizeof(real) * n * cam.width * cam.height));
+    CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride;
+    C.body = cam.body; C.width = cam.width; C.height = cam.height; C.tan_half = (real)std::tan(cam.fovy * M_PI / 360); C.zfar = (real)cam.zfar;
+    for (int i = 0; i < 3; i++) C.pos[i] = (real)cam.pos[i];
+    for (int i = 0; i < 4; i++) C.quat[i] = (real)cam.quat[i];
+    C.out = d_depth; C.n = n;
+    CUDA_OK(launch_camera<real>(C, device, stream));
+    launches++; depth_done = true;
+    return true;
+  }
+  bool get_depth(double *out) override {
+    if (!depth_done) { set_err("cassie_batch_get_depth: no render since the camera was set (cassie_batch_render_depth)"); return false; }
+    if (!out) { set_err("cassie_batch_get_depth: out is required"); return false; }
+    const int w = cam.width * cam.height;
+    return d2h(d_depth, w, w, 0, out);
+  }
   // open-loop sinusoidal gait on the motor-PD targets (BASELINE config 5 "random PD gaits"): evaluated in the kernel every control tick, so
   // multi-tick launches follow it without a host round trip; installing it restarts the tick clock
   bool set_pd_gait(const double *amp, const double *freq, const double *phase) override {
@@ -1012,7 +1054,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -1035,6 +1077,7 @@ template <typename real> struct Batch : BatchBase {
 
 // ====================================================================== C-ABI
 using namespace cassie;
+static_assert(CASSIE_CAM_MAXDIM == CAM_MAXDIM, "camera image size");
 static_assert(CASSIE_RAY_MAX == RAY_MAX && CASSIE_RAY_SLOT == RAY_SLOT && CASSIE_RAY_HEADING == RAY_HEADING && CASSIE_RAY_ROOT == RAY_ROOT && CASSIE_RAY_WORLD == RAY_WORLD, "ray table and rows");
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
@@ -1086,6 +1129,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
+  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -1447,6 +1491,25 @@ int cassie_batch_set_rays(cassie_batch_t *b, const int *frame, const double *ori
 int cassie_batch_nrays(const cassie_batch_t *b) { return b->impl->nray; }
 int cassie_batch_raycast(cassie_batch_t *b) { return b->impl->raycast() ? 0 : -1; }
 int cassie_batch_get_rays(cassie_batch_t *b, double *out) { return b->impl->get_rays(out) ? 0 : -1; }
+int cassie_batch_set_camera(cassie_batch_t *b, const char *camera, int width, int height, double zfar) {
+  const HostModel &hm = b->impl->hm;
+  if (width == 0) return b->impl->set_camera(-1, nullptr, nullptr, 0, 0, 0, 0, "cassie_batch_set_camera") ? 0 : -1;
+  const int k = camera ? hm.camera_id(camera) : -1;
+  if (k < 0) {
+    std::string names; for (const std::string &c : hm.names_camera) names += (names.empty() ? "" : ", ") + c;
+    set_err("cassie_batch_set_camera: unknown camera '" + std::string(camera ? camera : "") + "' (the model's cameras: " + (names.empty() ? "none" : names) + ")"); return -1;
+  }
+  if (hm.camera_mode[k] != CAM_FIXED) { set_err("cassie_batch_set_camera: camera '" + std::string(camera) + "' is not a fixed camera (track / target modes are not rendered)"); return -1; }
+  return b->impl->set_camera(hm.camera_body[k], &hm.camera_pos[3 * k], &hm.camera_quat[4 * k], hm.camera_fovy[k], width, height, zfar, "cassie_batch_set_camera") ? 0 : -1;
+}
+int cassie_batch_set_camera_mount(cassie_batch_t *b, const char *body, const double pos[3], const double quat[4], double fovy, int width, int height, double zfar) {
+  if (width == 0) return b->impl->set_camera(-1, nullptr, nullptr, 0, 0, 0, 0, "cassie_batch_set_camera_mount") ? 0 : -1;
+  const int id = body ? b->impl->hm.body_id(body) : -1;
+  if (id < 0) { set_err("cassie_batch_set_camera_mount: unknown body '" + std::string(body ? body : "") + "'"); return -1; }
+  return b->impl->set_camera(id, pos, quat, fovy, width, height, zfar, "cassie_batch_set_camera_mount") ? 0 : -1;
+}
+int cassie_batch_render_depth(cassie_batch_t *b) { return b->impl->render_depth() ? 0 : -1; }
+int cassie_batch_get_depth(cassie_batch_t *b, double *out) { return b->impl->get_depth(out) ? 0 : -1; }
 int cassie_batch_dynamics(cassie_batch_t *b) { return b->impl->dynamics() ? 0 : -1; }
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm) { return b->impl->get_dynamics(M, bias, J_eq, eq_err, Icm) ? 0 : -1; }
 int cassie_batch_neq(const cassie_batch_t *b) { return b->impl->hm.neq; }

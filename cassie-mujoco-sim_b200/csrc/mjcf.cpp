@@ -4,8 +4,9 @@
 // followed by mj_setConst (:952): default-class inheritance (model/cassie.xml:14-35), xyaxes / fromto / fullinertia
 // conversions, ref offsets, connect anchors at qpos0, dof tree tables, and the constants that feed constraint
 // regularisation (dof_invweight0, body_invweight0, stat.meaninertia).  Supported: compiler(angle), option, default,
-// asset/hfield, worldbody/body/inertial/joint/freejoint/geom/site, equality/connect, actuator/motor, sensor/*.
-// Everything visual (meshes, materials, cameras, lights) is ignored -- it has no effect on the stepped state.
+// asset/hfield, worldbody/body/inertial/joint/freejoint/geom/site/camera, equality/connect, actuator/motor, sensor/*.
+// Everything else visual (meshes, materials, lights) is ignored -- it has no effect on the stepped state.  Cameras are recorded (pose in their body
+// frame, fovy, mode) for the depth renderer; they do not touch the stepped state either.
 #include "model.h"
 
 #include <cmath>
@@ -176,11 +177,12 @@ struct Body { std::string name; int parent; double pos[3], quat[4], ipos[3], iqu
 struct Joint { std::string name; int type, body, limited; double pos[3], axis[3], range[2], ref, springref, stiffness, damping, armature, margin, solref[2], solimp[5]; int qposadr, dofadr; };
 struct Geom { std::string name; int type, body, contype, conaffinity, condim, priority, hfid, user, group; double pos[3], quat[4], size[3], rbound, friction[3], solmix, solref[2], solimp[5], margin, gap, mass; bool has_mass; };
 struct Site { std::string name; int body; double pos[3], quat[4]; };
+struct Camera { std::string name; int body, mode; double pos[3], quat[4], fovy; };
 void solimp5(const Attrs &a, const char *key, double out[5]) { vec v = Av(a, key, "0.9 0.95 0.001"); double d[5] = {0.9, 0.95, 0.001, 0.5, 2}; for (size_t i = 0; i < v.size() && i < 5; i++) d[i] = v[i]; memcpy(out, d, sizeof d); }
 
 struct Compiler {
   Defaults dfl; double ang = M_PI / 180;
-  std::vector<Body> bodies; std::vector<Joint> joints; std::vector<Geom> geoms; std::vector<Site> sites;
+  std::vector<Body> bodies; std::vector<Joint> joints; std::vector<Geom> geoms; std::vector<Site> sites; std::vector<Camera> cameras;
   std::vector<std::string> hf_names; std::vector<int> hf_nrow, hf_ncol; std::vector<double> hf_size;
   std::string err;
 
@@ -227,6 +229,16 @@ struct Compiler {
       if (A(a, "fromto")) { vec ft = nums(A(a, "fromto")); double v[3] = {ft[0] - ft[3], ft[1] - ft[4], ft[2] - ft[5]}; for (int i = 0; i < 3; i++) S.pos[i] = 0.5 * (ft[i] + ft[3 + i]); z2quat(S.quat, v); }
       else { vec p = Av(a, "pos", "0 0 0"); memcpy(S.pos, p.data(), sizeof S.pos); orientation(a, S.quat); }
       sites.push_back(S);
+    }
+    for (auto &c : node->kids) if (c->tag == "camera") {   // numbered in document order, like MuJoCo's
+      static const std::map<std::string, int> modes = {{"fixed", CAM_FIXED}, {"track", CAM_TRACK}, {"trackcom", CAM_TRACKCOM}, {"targetbody", CAM_TARGETBODY}, {"targetbodycom", CAM_TARGETBODYCOM}};
+      Attrs a = merged(dfl, c->get("class") ? c->get("class") : childclass, "camera", c.get());
+      Camera K{}; K.name = A(a, "name") ? A(a, "name") : ""; K.body = parent; K.fovy = Ad(a, "fovy", 45);
+      const std::string ms = A(a, "mode") ? A(a, "mode") : "fixed";
+      if (!modes.count(ms)) { err = "unknown camera mode " + ms; return false; }
+      K.mode = modes.at(ms);
+      vec p = Av(a, "pos", "0 0 0"); memcpy(K.pos, p.data(), sizeof K.pos); orientation(a, K.quat);
+      cameras.push_back(K);
     }
     for (auto &c : node->kids) if (c->tag == "body") {
       const XNode *b = c.get(); int bid = (int)bodies.size();
@@ -462,6 +474,10 @@ bool compile_mjcf(const std::string &xml_path, HostModel &m, std::string &err) {
     m.geom_margin.push_back(G.margin); m.geom_gap.push_back(G.gap); m.names_geom.push_back(G.name);
   }
   for (const Site &S : C.sites) { m.site_bodyid.push_back(S.body); m.site_pos.insert(m.site_pos.end(), S.pos, S.pos + 3); m.site_quat.insert(m.site_quat.end(), S.quat, S.quat + 4); m.names_site.push_back(S.name); }
+  for (const Camera &K : C.cameras) {
+    m.camera_body.push_back(K.body); m.camera_mode.push_back(K.mode); m.camera_pos.insert(m.camera_pos.end(), K.pos, K.pos + 3);
+    m.camera_quat.insert(m.camera_quat.end(), K.quat, K.quat + 4); m.camera_fovy.push_back(K.fovy); m.names_camera.push_back(K.name);
+  }
   m.nhfield = (int)C.hf_names.size(); m.hfield_nrow = C.hf_nrow; m.hfield_ncol = C.hf_ncol; m.hfield_size = C.hf_size;
   // equality: anchors of body2 computed in the qpos0 configuration
   Kin k; host_fk(m, m.qpos0.data(), k);
@@ -541,7 +557,9 @@ bool save_cmodel(const HostModel &m, const std::string &path) {
   PVI(actuator_jntid); PVI(actuator_ctrllimited); PVF(actuator_gear); PVF(actuator_ctrlrange); PVF(actuator_user);
   PVI(sensor_type); PVI(sensor_objid); PVF(sensor_user); PVF(sensor_cutoff); PVI(hfield_nrow); PVI(hfield_ncol); PVF(hfield_size);
   if (!m.rangefinder_site.empty()) { PVI(rangefinder_site); PVF(rangefinder_cutoff); }   // optional: tables of models without rangefinders are unchanged
+  if (!m.camera_body.empty()) { PVI(camera_body); PVI(camera_mode); PVF(camera_pos); PVF(camera_quat); PVF(camera_fovy); }   // optional, like the rangefinders
   puts_(o, "names_body", m.names_body); puts_(o, "names_site", m.names_site); puts_(o, "names_geom", m.names_geom); puts_(o, "names_joint", m.names_joint);
+  if (!m.names_camera.empty()) puts_(o, "names_camera", m.names_camera);
   return (bool)o;
 }
 bool load_cmodel(const std::string &path, HostModel &m, std::string &err) {
@@ -572,6 +590,8 @@ bool load_cmodel(const std::string &path, HostModel &m, std::string &err) {
     LVI(actuator_jntid); LVI(actuator_ctrllimited); LVF(actuator_gear); LVF(actuator_ctrlrange); LVF(actuator_user);
     LVI(sensor_type); LVI(sensor_objid); LVF(sensor_user); LVF(sensor_cutoff); LVI(hfield_nrow); LVI(hfield_ncol); LVF(hfield_size);
     LVI(rangefinder_site); LVF(rangefinder_cutoff);
+    LVI(camera_body); LVI(camera_mode); LVF(camera_pos); LVF(camera_quat); LVF(camera_fovy);
+    else if (key == "names_camera") m.names_camera = vs;
     else if (key == "names_body") m.names_body = vs; else if (key == "names_site") m.names_site = vs;
     else if (key == "names_geom") m.names_geom = vs; else if (key == "names_joint") m.names_joint = vs;
   }
@@ -579,6 +599,10 @@ bool load_cmodel(const std::string &path, HostModel &m, std::string &err) {
   m.geom_user.resize(m.ngeom, 0); m.geom_group.resize(m.ngeom, 0);   // tables written before these columns existed
   if (m.rangefinder_cutoff.size() != m.rangefinder_site.size()) { err = "malformed rangefinder entries in " + path; return false; }
   for (int s : m.rangefinder_site) if (s < 0 || s >= m.nsite) { err = "a rangefinder refers to an unknown site in " + path; return false; }
+  const size_t ncam = m.camera_body.size();
+  if (m.camera_mode.size() != ncam || m.camera_pos.size() != 3 * ncam || m.camera_quat.size() != 4 * ncam || m.camera_fovy.size() != ncam || m.names_camera.size() != ncam) {
+    err = "malformed camera entries in " + path; return false; }
+  for (int b : m.camera_body) if (b < 0 || b >= m.nbody) { err = "a camera refers to an unknown body in " + path; return false; }
   return true;
 }
 bool load_model_any(const std::string &path, HostModel &out, std::string &err) {

@@ -12,6 +12,7 @@ namespace cassie {
 enum JntType { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum GeomType { GEOM_PLANE = 0, GEOM_HFIELD = 1, GEOM_SPHERE = 2, GEOM_CAPSULE = 3, GEOM_BOX = 6, GEOM_MESH = 7 };
 // sensor kinds private to this table (the 29-number Cassie layout, model/cassie.xml:272-292)
+enum CameraMode { CAM_FIXED = 0, CAM_TRACK = 1, CAM_TRACKCOM = 2, CAM_TARGETBODY = 3, CAM_TARGETBODYCOM = 4 };
 enum SensorKind { SENS_ACTUATORPOS = 0, SENS_JOINTPOS = 1, SENS_FRAMEQUAT = 2, SENS_GYRO = 3, SENS_ACCEL = 4, SENS_MAG = 5 };
 
 struct HostModel {
@@ -49,15 +50,19 @@ struct HostModel {
   // rangefinders (<rangefinder site= cutoff=>): kept apart from the sensor table, whose 29 numbers the step kernel reads; optional table entries
   std::vector<int> rangefinder_site;
   std::vector<double> rangefinder_cutoff;
+  // cameras (<camera>): pose in the body frame, vertical field of view (degrees) and mode (CAM_FIXED ..); optional table entries (cassie_batch_set_camera)
+  std::vector<int> camera_body, camera_mode;
+  std::vector<double> camera_pos, camera_quat, camera_fovy;
   // height field (at most one)
   std::vector<int> hfield_nrow, hfield_ncol;
   std::vector<double> hfield_size;
   // names
-  std::vector<std::string> names_body, names_site, names_geom, names_joint;
+  std::vector<std::string> names_body, names_site, names_geom, names_joint, names_camera;
 
   int body_id(const std::string &n) const { for (int i = 0; i < (int)names_body.size(); i++) if (names_body[i] == n) return i; return -1; }
   int site_id(const std::string &n) const { for (int i = 0; i < (int)names_site.size(); i++) if (names_site[i] == n) return i; return -1; }
   int joint_id(const std::string &n) const { for (int i = 0; i < (int)names_joint.size(); i++) if (names_joint[i] == n) return i; return -1; }
+  int camera_id(const std::string &n) const { for (int i = 0; i < (int)names_camera.size(); i++) if (names_camera[i] == n) return i; return -1; }
   int geom_id(const std::string &n) const { for (int i = 0; i < (int)names_geom.size(); i++) if (names_geom[i] == n) return i; return -1; }
 };
 

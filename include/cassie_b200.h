@@ -210,6 +210,29 @@ int cassie_batch_set_rays(cassie_batch_t *b, const int *frame, const double *ori
 int cassie_batch_nrays(const cassie_batch_t *b);
 int cassie_batch_raycast(cassie_batch_t *b);
 int cassie_batch_get_rays(cassie_batch_t *b, double *out);
+/* Depth camera: one camera per batch, mounted on a body, rendered at the CURRENT qpos of every environment as a depth image -- the perception signal
+ * of the reference's CassieVis draw_depth (an offscreen OpenGL render, one environment at a time), here one kernel launch for the batch.
+ * The camera looks along its -z axis, +y is image up, fovy is the full vertical angle (degrees).  Pixel (r, c) of a width x height image is taken at
+ * its centre, row 0 at the TOP; its value is the z-depth (distance along the optical axis, metres) of the first hit in (0, zfar], and zfar where
+ * nothing is hit within zfar.  (The reference's mjr_readPixels buffer is bottom row first and holds OpenGL's non-linear depth; the values here are
+ * linear metres.)  What is seen: the static collision geoms with the ray rules (each environment's own placement and terrain), and the moving
+ * collision geoms -- the robot's spheres and capsules, boxes on moving bodies, the extra free body -- from outside only: a pixel whose ray starts
+ * inside a moving geom does not see that geom.  Visual meshes are not loaded, so the robot appears as its collision model.
+ * cassie_batch_set_camera: a <camera> of the model by name; only fixed-mode cameras (not the track cameras).  cassie_batch_set_camera_mount: a
+ * camera the caller mounts on a named body, pos / quat in the body frame (quat is normalised).  Either returns 0, or -1 with nothing changed
+ * (cassie_b200_last_error) for an unknown camera or body (the message lists the model's cameras), a camera that is not fixed, fovy outside
+ * (0, 180), width or height outside 1 .. CASSIE_CAM_MAXDIM, zfar <= 0 or not finite, a zero or non-finite quaternion.  width = 0 drops the
+ * camera.  Every successful set drops the rows: a device pointer taken before it is no longer valid.
+ * cassie_batch_render_depth: one launch on the batch stream (asynchronous); it writes nothing but the rows [n][height][width] in the batch precision
+ * (allocated by the first render after a set; snapshots, resets and cassie_sim_copy leave them alone).
+ * cassie_batch_get_depth: synchronous copy [n][height][width] doubles; -1 before the first render after a set.  Device rows:
+ * cassie_batch_device_ptr(b, "depth"), row width height x width. */
+#define CASSIE_CAM_MAXDIM 256
+int cassie_batch_set_camera(cassie_batch_t *b, const char *camera, int width, int height, double zfar);
+int cassie_batch_set_camera_mount(cassie_batch_t *b, const char *body, const double pos[3], const double quat[4], double fovy,
+                                  int width, int height, double zfar);
+int cassie_batch_render_depth(cassie_batch_t *b);
+int cassie_batch_get_depth(cassie_batch_t *b, double *out);
 /* include/cassiemujoco.h:61-73 (src/cassiemujoco.c:1072-1093): model (per-environment constants, height field, timestep) + full dynamic state */
 cassie_sim_t *cassie_sim_duplicate(const cassie_sim_t *src);
 void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *src);
