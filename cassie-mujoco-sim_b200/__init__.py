@@ -230,6 +230,15 @@ def lib():
     L.cassie_batch_get_env_geom_pose.restype = ci
     L.cassie_batch_clear_env_geom_poses.argtypes = [vp]
     L.cassie_batch_clear_env_geom_poses.restype = ci
+    L.cassie_batch_set_env_hfield.argtypes = [vp, C.POINTER(ci), cd, cd, C.c_void_p]
+    L.cassie_batch_get_env_hfield.argtypes = [vp, C.POINTER(ci), cd, cd]
+    L.cassie_batch_clear_env_hfield.argtypes = [vp]
+    L.cassie_batch_set_hfield_size.argtypes = L.cassie_batch_get_hfield_size.argtypes = [vp, cd]
+    for n in ('set_env_hfield', 'get_env_hfield', 'clear_env_hfield', 'set_hfield_size', 'get_hfield_size'):
+        getattr(L, 'cassie_batch_' + n).restype = ci
+    L.cassie_sim_get_hfield_size.argtypes = [vp]
+    L.cassie_sim_get_hfield_size.restype = cd
+    L.cassie_sim_set_hfield_size.argtypes = [vp, C.c_double * 4]
     L.cassie_sim_params.argtypes = [vp, C.POINTER(ci)]
     for n in ('cassie_sim_dof_damping', 'cassie_sim_body_mass', 'cassie_sim_body_ipos', 'cassie_sim_geom_friction'):
         getattr(L, n).argtypes = [vp]
@@ -473,6 +482,43 @@ class CassieBatch:
         """drop the per-environment placements: every environment follows the shared placement again"""
         if self.L.cassie_batch_clear_env_geom_poses(self.h) != 0:
             raise RuntimeError(_last_error())
+
+    # ---- per-environment terrain (terrain curricula: promote / demote environments between terrain types and difficulty levels at their resets)
+    def set_env_hfield(self, terrain=None, pos=None, size=None, mask=None):
+        """which bank entry each environment stands on and where and how large its height field is: terrain [n] (or one int) in [0, K) of
+        set_hfield_data, pos [3] or [n, 3] (in the height field's body frame; it stays axis-aligned), size [4] or [n, 4] (x half-extent, y half-extent,
+        elevation scale, base thickness); None leaves that part alone; mask [n]: only the selected environments change.  A bad value raises and
+        changes nothing.  Reset and snapshot restore leave these alone."""
+        t = None if terrain is None else np.ascontiguousarray(np.broadcast_to(np.asarray(terrain, dtype=np.int32), (self.n,)))
+        a = [None if v is None else np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (self.n, w))) for v, w in ((pos, 3), (size, 4))]
+        m = None if mask is None else np.ascontiguousarray(np.broadcast_to(np.asarray(mask, dtype=np.uint8), (self.n,)))
+        if self.L.cassie_batch_set_env_hfield(self.h, None if t is None else t.ctypes.data_as(C.POINTER(C.c_int)), *[None if v is None else self._dp(v) for v in a],
+                                              None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_hfield(self):
+        """(terrain [n] int32, pos [n, 3], size [n, 4]): the bank entry, height-field position and size each environment sees"""
+        t, pos, size = np.zeros(self.n, dtype=np.int32), np.zeros((self.n, 3)), np.zeros((self.n, 4))
+        if self.L.cassie_batch_get_env_hfield(self.h, t.ctypes.data_as(C.POINTER(C.c_int)), self._dp(pos), self._dp(size)) != 0:
+            raise RuntimeError(_last_error())
+        return t, pos, size
+
+    def clear_env_hfield(self):
+        """back to terrain e % K and the shared position and size"""
+        if self.L.cassie_batch_clear_env_hfield(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def set_hfield_size(self, size):
+        """the shared height-field size [4]; every environment's position and size go back to the shared ones, terrain selections stay"""
+        a = np.ascontiguousarray(np.asarray(size, dtype=np.float64).reshape(4))
+        if self.L.cassie_batch_set_hfield_size(self.h, self._dp(a)) != 0:
+            raise RuntimeError(_last_error())
+
+    def hfield_size(self):
+        out = np.zeros(4)
+        if self.L.cassie_batch_get_hfield_size(self.h, self._dp(out)) != 0:
+            raise RuntimeError(_last_error())
+        return out
 
     # ---- frames: named bodies / sites written by every step and forward (reference: xpos, xquat, get_site_xpos, get_site_quat, body_vel,
     # get_body_contact_force of example/cassiemujoco.py)
@@ -724,7 +770,8 @@ class CassieBatch:
 
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
-        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width]).  set_frames /
+        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width],
+        terrain [n] int32: each environment's bank entry, read mod K at the next launch; set_env_hfield first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -734,14 +781,18 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
+        if field == 'terrain':
+            ts = '<i4'
 
         class _Arr:
             pass
         a = _Arr()
         a.__cuda_array_interface__ = dict(shape=(self.n, width), typestr=ts, data=(ptr, False), version=2)
         t = torch.as_tensor(a, device='cuda')
+        if field == 'terrain':
+            return t.view(self.n)
         return t.view(self.n, *self._cam_hw) if field == 'depth' else t
 
 
@@ -1001,6 +1052,18 @@ class CassieSim:
 
     def set_const(self):
         self.L.cassie_sim_set_const(self.c)
+
+    def get_hfield_size(self):
+        """the height field's size [x half-extent, y half-extent, elevation scale, base thickness] (reference: example/cassiemujoco.py:741-746)"""
+        ptr = self.L.cassie_sim_get_hfield_size(self.c)
+        if not ptr:
+            raise RuntimeError(_last_error())
+        return np.array(ptr[:4])
+
+    def set_hfield_size(self, data):
+        """applied at the next step (reference: example/cassiemujoco.py:768-776)"""
+        assert len(data) == 4
+        self.L.cassie_sim_set_hfield_size(self.c, (C.c_double * 4)(*[float(x) for x in data]))
 
     def just_set_const(self):
         self.L.cassie_sim_just_set_const(self.c)

@@ -31,6 +31,7 @@ CASSIE_STEP_ENTRY(f20) CASSIE_STEP_ENTRY(f22) CASSIE_STEP_ENTRY(f24) CASSIE_STEP
 CASSIE_STEP_ENTRY(f0c) CASSIE_STEP_ENTRY(f1c) CASSIE_STEP_ENTRY(f2c) CASSIE_STEP_ENTRY(f0f) CASSIE_STEP_ENTRY(f1f) CASSIE_STEP_ENTRY(f2f)
 CASSIE_STEP_ENTRY(d0f) CASSIE_STEP_ENTRY(d1f) CASSIE_STEP_ENTRY(d2f)
 CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_STEP_ENTRY(f11c) CASSIE_STEP_ENTRY(f11f) CASSIE_STEP_ENTRY(d11f)
+CASSIE_STEP_ENTRY(f02f) CASSIE_STEP_ENTRY(f12f) CASSIE_STEP_ENTRY(f22f) CASSIE_STEP_ENTRY(d02f) CASSIE_STEP_ENTRY(d12f) CASSIE_STEP_ENTRY(d22f) CASSIE_STEP_ENTRY(f13f) CASSIE_STEP_ENTRY(d13f)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -40,6 +41,13 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_TR) {   // per-environment terrain (always with the per-environment static geoms): F_ALL | F_EG | F_TR, with or without frame rows
+    const bool dbl = std::is_same<real, double>::value, fr = (feat & F_FR) != 0;
+    if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | (fr ? F_FR : 0);
+    if (fr) { if (inst != 1) return nullptr; return dbl ? cassie_step_entry_d13f() : cassie_step_entry_f13f(); }
+    if (dbl) return inst == 1 ? cassie_step_entry_d12f() : (inst == 2 ? cassie_step_entry_d22f() : cassie_step_entry_d02f());
+    return inst == 1 ? cassie_step_entry_f12f() : (inst == 2 ? cassie_step_entry_f22f() : cassie_step_entry_f02f());
+  }
   if (feat & F_FR) {   // frame rows: extended instances only; F_BOX covers models with at most boxes, F_ALL the rest, each with or without F_EG
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value, eg = (feat & F_EG) != 0, box = !dbl && (feat & ~(F_BOX | F_EG | F_FR)) == 0;
@@ -278,6 +286,12 @@ struct BatchBase {
   virtual bool get_env_geom(int g, double *pos, double *quat, double *size) = 0;
   virtual bool clear_env_geoms() = 0;
   virtual bool shared_geom_changed(int g) = 0;          // after the shared placement of geom g was rebuilt: its slot in every row follows it
+  // per-environment terrain: bank entry [n], height-field position [n][3] (in its body frame) and size [n][4]; NULL parts unchanged, only masked
+  // environments change; checked as a whole before anything changes
+  virtual bool set_env_hfield(const int *terrain, const double *pos, const double *size, const unsigned char *mask) = 0;
+  virtual bool get_env_hfield(int *terrain, double *pos, double *size) = 0;
+  virtual bool clear_env_hfield() = 0;
+  virtual bool set_hfield_size(const double *size) = 0;   // the shared size; every environment's height-field position and size follow the shared ones
   virtual bool set_frames(const char *const *names, const int *kinds, int count) = 0;   // frame rows [n][count][FRAME_W]; count 0: none
   virtual bool frame_jacobian(int frame, double *jacp, double *jacr) = 0;                 // [n][3][nv] each at the current state (launch mode 4); jacr may be null
   virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
@@ -320,9 +334,11 @@ template <typename real> struct Batch : BatchBase {
   real *d_depth = nullptr;                     // depth rows of the last render
   real *d_genv = nullptr;                  // A.genv: [n][GEOM_ENV_W] per-environment static-geom placement, allocated by the first per-environment placement
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
+  int *d_terrain = nullptr;                // A.terrain: [n] per-environment bank entries, allocated by the first per-environment terrain (F_TR instances)
+  std::vector<double> hf_host;             // [n][7] height-field position (in its body frame) 3, size 4 per environment; empty: the shared ones
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -386,6 +402,9 @@ template <typename real> struct Batch : BatchBase {
         CUDA_OK(cudaFuncSetAttribute(entry, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
         CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, feat | F_EG), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // same scratch, same shape
         if (ext == 1) for (int fe : {feat | F_FR, feat | F_EG | F_FR}) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+        if (hm.nhfield == 1) {   // per-environment terrain: F_ALL | F_EG | F_TR (the scratch of F_ALL)
+          CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+          if (ext == 1) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR | F_FR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -737,9 +756,15 @@ template <typename real> struct Batch : BatchBase {
     if (!rebuild_model()) return false;
     if (src->A.cenv) { if (!ensure_cenv()) return false; CUDA_OK(cudaMemcpyAsync(A.cenv, src->A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToDevice, stream)); }
     else if (A.cenv) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; }
+    if (!src->d_terrain && !clear_env_hfield()) return false;
     if (src->d_genv) { if (!ensure_genv()) return false; CUDA_OK(cudaMemcpyAsync(d_genv, src->d_genv, sizeof(real) * n * GEOM_ENV_W, cudaMemcpyDeviceToDevice, stream)); }
     else if (!clear_env_geoms()) return false;
     for (int k = 0; k < MGS; k++) ge_host[k] = src->ge_host[k];
+    if (src->d_terrain) {   // the selection row and the height field's mirror (its slots came with the rows above)
+      if (!d_terrain) { CUDA_OK(cudaMalloc(&d_terrain, sizeof(int) * n)); A.terrain = d_terrain; }
+      CUDA_OK(cudaMemcpyAsync(d_terrain, src->d_terrain, sizeof(int) * n, cudaMemcpyDeviceToDevice, stream));
+      hf_host = src->hf_host;
+    }
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
       std::vector<float> tmp(cells); CUDA_OK(cudaMemcpy(tmp.data(), src->d_hfield, sizeof(float) * cells, cudaMemcpyDeviceToHost));
@@ -799,21 +824,96 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
-  bool clear_env_geoms() override {
+  bool clear_env_geoms() override {   // the height field's position and size go back to the shared ones too; a terrain selection stays
     for (int k = 0; k < MGS; k++) ge_host[k].clear();
+    hf_host.clear();
     if (!d_genv) return true;
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaFree(d_genv)); d_genv = nullptr; A.genv = nullptr;
-    return true;
+    return !d_terrain || (ensure_genv() && put_hf_slots());   // the F_TR instances read the height field's slot: fresh rows with the shared one
   }
   bool shared_geom_changed(int g) override {
     const int k = g >= 0 && g < hm.ngeom ? geom_dev[g] - MG : -1;
     if (k < 0 || k >= MGS) return true;
     ge_host[k].clear();
+    if (g == hfield_geom(hm)) { hf_host.clear(); if (d_terrain) return put_hf_slots(); }
     if (!d_genv) return true;
     std::vector<real> row(GEOM_ENV_W), slots((size_t)n * GE_SLOT); init_genv_row(h_model_copy, row.data());
     for (int e = 0; e < n; e++) memcpy(&slots[(size_t)e * GE_SLOT], &row[GE_SLOT * k], sizeof(real) * GE_SLOT);
     return put_genv_slot(k, slots);
+  }
+  // ---- per-environment terrain (terrain curricula): which bank entry each environment stands on, and where and how large its height field is
+  int hf_slot(const char *verb) {   // the height field's static slot, or -1 with an error
+    const int g = hfield_geom(hm), k = g >= 0 ? geom_dev[g] - MG : -1;
+    if (hm.nhfield != 1 || k < 0 || k >= MGS) { set_err(std::string(verb) + ": this model has no height field"); return -1; }
+    return k;
+  }
+  void hf_shared(double *r) { const int g = hfield_geom(hm); for (int c = 0; c < 3; c++) r[c] = hm.geom_pos[3 * g + c]; for (int c = 0; c < 4; c++) r[3 + c] = hm.hfield_size[c]; }
+  bool put_hf_slots() {   // the height field's slot of every row from the mirror (or the shared position and size)
+    const int g = hfield_geom(hm), k = geom_dev[g] - MG;
+    std::vector<real> slots((size_t)n * GE_SLOT); double sh[7]; hf_shared(sh);
+    for (int e = 0; e < n; e++) { const double *r = hf_host.empty() ? sh : &hf_host[(size_t)e * 7]; env_hfield_slot(hm, g, r, r + 3, &slots[(size_t)e * GE_SLOT]); }
+    return put_genv_slot(k, slots);
+  }
+  bool set_env_hfield(const int *terrain, const double *pos, const double *size, const unsigned char *mask) override {
+    const char *verb = "cassie_batch_set_env_hfield";
+    if (hf_slot(verb) < 0) return false;
+    for (int e = 0; e < n; e++) {   // every masked environment is checked before anything changes
+      if (mask && !mask[e]) continue;
+      const std::string at = std::string(verb) + ": environment " + std::to_string(e) + ": ";
+      if (terrain && (terrain[e] < 0 || terrain[e] >= A.n_terrain)) { set_err(at + "terrain " + std::to_string(terrain[e]) + " is outside [0, " + std::to_string(A.n_terrain) + ")"); return false; }
+      if (pos && !std::isfinite(pos[3 * e] + pos[3 * e + 1] + pos[3 * e + 2])) { set_err(at + "pos is not finite"); return false; }
+      if (size) { const std::string w = hfield_size_check(size + 4 * (size_t)e); if (!w.empty()) { set_err(at + w); return false; } }
+    }
+    CUDA_OK(cudaSetDevice(device));
+    if (!ensure_genv()) return false;
+    std::vector<int> t(n);
+    if (d_terrain) { CUDA_OK(cudaMemcpyAsync(t.data(), d_terrain, sizeof(int) * n, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }   // it may have been written on the device
+    else for (int e = 0; e < n; e++) t[e] = e % A.n_terrain;
+    if (hf_host.empty()) { double sh[7]; hf_shared(sh); hf_host.resize((size_t)n * 7); for (int e = 0; e < n; e++) memcpy(&hf_host[(size_t)e * 7], sh, sizeof sh); }
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      if (terrain) t[e] = terrain[e];
+      if (pos) for (int c = 0; c < 3; c++) hf_host[(size_t)e * 7 + c] = pos[3 * (size_t)e + c];
+      if (size) for (int c = 0; c < 4; c++) hf_host[(size_t)e * 7 + 3 + c] = size[4 * (size_t)e + c];
+    }
+    if (!d_terrain) CUDA_OK(cudaMalloc(&d_terrain, sizeof(int) * n));
+    CUDA_OK(cudaMemcpyAsync(d_terrain, t.data(), sizeof(int) * n, cudaMemcpyHostToDevice, stream));
+    A.terrain = d_terrain;
+    return put_hf_slots();
+  }
+  bool get_env_hfield(int *terrain, double *pos, double *size) override {
+    if (hf_slot("cassie_batch_get_env_hfield") < 0) return false;
+    CUDA_OK(cudaSetDevice(device));
+    if (terrain) {
+      if (d_terrain) { CUDA_OK(cudaMemcpyAsync(terrain, d_terrain, sizeof(int) * n, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
+      else for (int e = 0; e < n; e++) terrain[e] = e % A.n_terrain;
+    }
+    double sh[7]; hf_shared(sh);
+    for (int e = 0; e < n; e++) {
+      const double *r = hf_host.empty() ? sh : &hf_host[(size_t)e * 7];
+      if (pos) for (int c = 0; c < 3; c++) pos[3 * (size_t)e + c] = r[c];
+      if (size) for (int c = 0; c < 4; c++) size[4 * (size_t)e + c] = r[3 + c];
+    }
+    return true;
+  }
+  bool clear_env_hfield() override {   // back to terrain e % K and the shared placement and size: the slot as the model block has it
+    hf_host.clear();
+    if (d_terrain) { CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(d_terrain)); d_terrain = nullptr; A.terrain = nullptr; }
+    const int g = hfield_geom(hm);
+    return g < 0 || !d_genv || shared_geom_changed(g);
+  }
+  bool set_hfield_size(const double *size) override {
+    const char *verb = "cassie_batch_set_hfield_size";
+    if (hf_slot(verb) < 0) return false;
+    if (!size) { set_err(std::string(verb) + ": size is required"); return false; }
+    const std::string w = hfield_size_check(size);
+    if (!w.empty()) { set_err(std::string(verb) + ": " + w); return false; }
+    const int g = hfield_geom(hm);
+    for (int c = 0; c < 4; c++) hm.hfield_size[c] = size[c];
+    const double z = std::max(size[2], size[3]);
+    hm.geom_rbound[g] = std::sqrt(size[0] * size[0] + size[1] * size[1] + z * z);   // the model compiler's bound for the new size
+    return rebuild_model() && shared_geom_changed(g);   // every environment's height-field position and size follow the shared ones
   }
   // ---- frame rows: the table is checked as a whole before anything changes; the rows start at zero and are filled by the next step / forward launch
   bool set_frames(const char *const *names, const int *kinds, int count) override {
@@ -916,7 +1016,7 @@ template <typename real> struct Batch : BatchBase {
     if (!nray) { set_err("cassie_batch_raycast: no rays are set (cassie_batch_set_rays)"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (!d_rays) CUDA_OK(cudaMalloc(&d_rays, sizeof(real) * n * nray * RAY_SLOT));
-    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride;
+    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride; R.terrain = d_terrain;
     R.tab = d_rtab; R.k = nray; R.out = d_rays; R.n = n;
     CUDA_OK(launch_raycast<real>(R, device, stream));
     launches++; rays_done = true;
@@ -944,7 +1044,7 @@ template <typename real> struct Batch : BatchBase {
     if (!cam.width) { set_err("cassie_batch_render_depth: no camera is set (cassie_batch_set_camera)"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (!d_depth) CUDA_OK(cudaMalloc(&d_depth, sizeof(real) * n * cam.width * cam.height));
-    CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride;
+    CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain;
     C.body = cam.body; C.width = cam.width; C.height = cam.height; C.tan_half = (real)std::tan(cam.fovy * M_PI / 360); C.zfar = (real)cam.zfar;
     for (int i = 0; i < 3; i++) C.pos[i] = (real)cam.pos[i];
     for (int i = 0; i < 4; i++) C.quat[i] = (real)cam.quat[i];
@@ -986,7 +1086,7 @@ template <typename real> struct Batch : BatchBase {
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1054,7 +1154,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -1091,7 +1191,9 @@ struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[6
   // site_xpos[nsite][3], so that the borrowed pointers of cassie_sim_xpos / xquat / site_xpos index across bodies as &d->xpos[3 * id] does
   std::vector<double> frames, xpos, xquat, site_xpos;
   // the acceleration row of the simulator's batch (qacc, then the cacc of every body and site frame) and the nv-entry qacc mirror cassie_sim_qacc lends out
-  std::vector<double> acc, qacc; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
+  std::vector<double> acc, qacc;
+  // the height field's size (cassie_sim_get_hfield_size / set_hfield_size): a host mirror, uploaded before the next launch when it is valid
+  double hf_size[4] = {0, 0, 0, 0}, hf_size_dev[4] = {0, 0, 0, 0}; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
 
 // cassie_state_t (include/cassiemujoco.h:434-463): a device-resident snapshot of one simulator's rows plus the host mirrors the reference hands out as
 // borrowed pointers (time, qpos, qvel); the snapshot is allocated by the first cassie_get_state, which also fixes the owning simulator's sizes
@@ -1129,7 +1231,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
-  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height;
+  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -1223,6 +1325,8 @@ static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote thr
   if (c->time_dev != c->time) c->b->impl->set("time", &c->time);
   if (c->timestep != c->timestep_dev) { if (c->timestep > 0) { c->b->impl->hm.timestep = c->timestep; c->b->impl->rebuild_model(); } c->timestep_dev = c->timestep; }   // written through cassie_sim_timestep()
   if (!c->hfield.empty() && c->hfield != c->hfield_dev) { c->b->impl->set_hfield(c->hfield.data(), 1); c->hfield_dev = c->hfield; }
+  if (c->b->impl->hm.nhfield && memcmp(c->hf_size, c->hf_size_dev, sizeof c->hf_size)) {   // an invalid size is not uploaded: the error is recorded once, the last valid size stays
+    cassie_batch_set_hfield_size(c->b, c->hf_size); memcpy(c->hf_size_dev, c->hf_size, sizeof c->hf_size); }
   if (c->m_mass != c->m_mass_dev) { cassie_batch_set_body_mass(c->b, c->m_mass.data()); c->m_mass_dev = c->m_mass; }
   if (c->m_ipos != c->m_ipos_dev) { cassie_batch_set_body_ipos(c->b, c->m_ipos.data()); c->m_ipos_dev = c->m_ipos; }
   if (c->m_damp != c->m_damp_dev) { cassie_batch_set_dof_damping(c->b, c->m_damp.data()); c->m_damp_dev = c->m_damp; }
@@ -1251,7 +1355,8 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   { const HostModel &hm = b->impl->hm; c->m_mass = hm.body_mass; c->m_ipos = hm.body_ipos; c->m_damp = hm.dof_damping; c->m_fric = hm.geom_friction;
     c->m_mass_dev = c->m_mass; c->m_ipos_dev = c->m_ipos; c->m_damp_dev = c->m_damp; c->m_fric_dev = c->m_fric;
     c->m_gpos = hm.geom_pos; c->m_gquat = hm.geom_quat; c->m_gsize = hm.geom_size; c->m_gpos_dev = c->m_gpos; c->m_gquat_dev = c->m_gquat; c->m_gsize_dev = c->m_gsize; }
-  if (b->impl->hm.nhfield) { c->hfield.assign((size_t)b->impl->hm.hfield_nrow[0] * b->impl->hm.hfield_ncol[0], 0.0f); c->hfield_dev = c->hfield; }
+  if (b->impl->hm.nhfield) { c->hfield.assign((size_t)b->impl->hm.hfield_nrow[0] * b->impl->hm.hfield_ncol[0], 0.0f); c->hfield_dev = c->hfield;
+                             for (int k = 0; k < 4; k++) c->hf_size[k] = c->hf_size_dev[k] = b->impl->hm.hfield_size[k]; }
   return c;
 }
 void cassie_sim_free(cassie_sim_t *c) { if (!c) return; cassie_batch_free(c->b); delete c; }
@@ -1269,6 +1374,16 @@ int cassie_sim_get_hfield_ncol(cassie_sim_t *c) { return cassie_batch_hfield_nco
 int cassie_sim_get_nhfielddata(cassie_sim_t *c) { return (int)c->hfield.size(); }
 float *cassie_sim_hfielddata(cassie_sim_t *c) { return c->hfield.empty() ? nullptr : c->hfield.data(); }
 void cassie_sim_set_hfielddata(cassie_sim_t *c, float *data) { for (size_t i = 0; i < c->hfield.size(); i++) c->hfield[i] = data[i]; }
+// src/cassiemujoco.c:2062-2070: a borrowed pointer to the height field's size [x half-extent, y half-extent, elevation scale, base thickness], uploaded
+// before the next step or forward like the elevations
+double *cassie_sim_get_hfield_size(cassie_sim_t *c) {
+  if (!c->b->impl->hm.nhfield) { set_err("cassie_sim_get_hfield_size: this model has no height field"); return nullptr; }
+  return c->hf_size;
+}
+void cassie_sim_set_hfield_size(cassie_sim_t *c, double size[4]) {
+  if (!c->b->impl->hm.nhfield) { set_err("cassie_sim_set_hfield_size: this model has no height field"); return; }
+  if (size) for (int k = 0; k < 4; k++) c->hf_size[k] = size[k];
+}
 // ---- read-only derived quantities (include/cassiemujoco.h:200-240).  Contact forces, flags, foot positions / velocities are by-products of
 // the last step (the reference reads the same stale mjData arrays); the centre-of-mass group recomputes the kinematics of the CURRENT
 // state first, as the reference does with mj_fwdPosition, through a query launch that writes nothing else.
@@ -1483,6 +1598,17 @@ int cassie_batch_get_env_geom_pose(cassie_batch_t *b, const char *name, double *
   return b->impl->get_env_geom(b->impl->hm.geom_id(name ? name : ""), pos, quat, size) ? 0 : -1;
 }
 int cassie_batch_clear_env_geom_poses(cassie_batch_t *b) { return b->impl->clear_env_geoms() ? 0 : -1; }
+// per-environment terrain (bank entry, height-field position and size); see include/cassie_b200.h
+int cassie_batch_set_env_hfield(cassie_batch_t *b, const int *terrain, const double *pos, const double *size, const unsigned char *mask) { return b->impl->set_env_hfield(terrain, pos, size, mask) ? 0 : -1; }
+int cassie_batch_get_env_hfield(cassie_batch_t *b, int *terrain, double *pos, double *size) { return b->impl->get_env_hfield(terrain, pos, size) ? 0 : -1; }
+int cassie_batch_clear_env_hfield(cassie_batch_t *b) { return b->impl->clear_env_hfield() ? 0 : -1; }
+int cassie_batch_set_hfield_size(cassie_batch_t *b, const double size[4]) { return b->impl->set_hfield_size(size) ? 0 : -1; }
+int cassie_batch_get_hfield_size(const cassie_batch_t *b, double size[4]) {
+  const HostModel &hm = b->impl->hm;
+  if (hm.nhfield != 1) { set_err("cassie_batch_get_hfield_size: this model has no height field"); return -1; }
+  if (size) for (int c = 0; c < 4; c++) size[c] = hm.hfield_size[c];
+  return 0;
+}
 int cassie_batch_set_frames(cassie_batch_t *b, const char *const *names, const int *kinds, int count) { return b->impl->set_frames(names, kinds, count) ? 0 : -1; }
 int cassie_batch_nframes(const cassie_batch_t *b) { return (int)(b->impl->frame_list.size() / 2); }
 int cassie_batch_get_frames(cassie_batch_t *b, double *out) { return b->impl->get("frames", out) ? 0 : -1; }
@@ -1609,6 +1735,7 @@ void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *csrc) {
   dst->m_mass_dev = dst->m_mass; dst->m_ipos_dev = dst->m_ipos; dst->m_damp_dev = dst->m_damp; dst->m_fric_dev = dst->m_fric;
   dst->m_gpos = dst->m_gpos_dev = src->m_gpos; dst->m_gquat = dst->m_gquat_dev = src->m_gquat; dst->m_gsize = dst->m_gsize_dev = src->m_gsize;
   dst->hfield = src->hfield; dst->hfield_dev = src->hfield_dev; dst->timestep = dst->timestep_dev = src->timestep;
+  memcpy(dst->hf_size, src->hf_size, sizeof dst->hf_size); memcpy(dst->hf_size_dev, src->hf_size_dev, sizeof dst->hf_size_dev);
   for (int i = 0; i < 16; i++) dst->b->radio[i] = src->b->radio[i];
   cassie_state_t *s = cassie_state_alloc(); cassie_get_state(src, s); cassie_set_state(dst, s); cassie_state_free(s);
 }

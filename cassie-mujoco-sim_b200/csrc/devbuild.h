@@ -54,6 +54,22 @@ template <typename real> void init_genv_row(const DevModel<real> &d, real *row) 
     for (int c = 0; c < 3; c++) s[GE_SIZE + c] = d.geom_size[MG + k][c];
     s[GE_RBOUND] = d.geom_rbound[MG + k]; }
 }
+// the host geom of the model's height field (-1: none)
+inline int hfield_geom(const HostModel &m) { for (int g = 0; g < m.ngeom; g++) if (m.geom_type[g] == GEOM_HFIELD) return g; return -1; }
+// a height-field size [x half-extent, y half-extent, elevation scale, base thickness] the verbs accept: an empty reason, else what is wrong with it
+inline std::string hfield_size_check(const double *s) {
+  for (int c = 0; c < 4; c++) if (!std::isfinite(s[c])) return "size[" + std::to_string(c) + "] is not finite";
+  if (!(s[0] > 0) || !(s[1] > 0)) return "the half-extents size[0], size[1] must be > 0";
+  if (s[2] < 0 || s[3] < 0) return "the elevation scale size[2] and base thickness size[3] must be >= 0";
+  return std::string();
+}
+// the height field's slot of a per-environment row (F_TR instances): geom g at pos (in its body frame, the model's orientation) with size hs[4]: GE_SIZE
+// holds the half-extents and the elevation scale, GE_RBOUND the model compiler's bound |(x, y, max(elevation, base))|
+template <typename real> void env_hfield_slot(const HostModel &m, int g, const double *pos, const double *hs, real *slot) {
+  env_geom_slot(m, g, pos, &m.geom_quat[4 * g], hs, slot);
+  const double z = std::fmax(hs[2], hs[3]);
+  slot[GE_RBOUND] = (real)std::sqrt(hs[0] * hs[0] + hs[1] * hs[1] + z * z);
+}
 // the static collision slot (0 .. MGS-1) of host geom g, or a reason why it has none that a per-environment placement could move
 inline int env_geom_check(const HostModel &m, const int *geom_dev, int g, std::string &err) {
   if (g < 0 || g >= m.ngeom) { err = "unknown geom"; return -1; }

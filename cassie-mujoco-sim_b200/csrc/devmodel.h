@@ -33,6 +33,7 @@ constexpr int YSTRIDE_MAX = 39;   // with the 6 dofs of an extra free body (cass
 constexpr int F_XB = 1, F_HFIELD = 2, F_BOX = 4, F_ALL = 7;   // extra free body (cassie_tray_box.xml's cup), height field, box geoms
 constexpr int F_EG = 8;   // the static geoms' world poses, sizes and bounding radii come from per-environment rows (GEOM_ENV_W) instead of the model block
 constexpr int F_FR = 16;  // frame rows (FRAME_W per named body / site) are filled in the last sub-step of a launch (extended instances only)
+constexpr int F_TR = 32;  // per-environment terrain: the bank entry from a selection row, the height field's size from its F_EG slot (with F_ALL | F_EG only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -166,6 +167,9 @@ constexpr int CE_ROOT_MINV = 256, CE_TOT_MINV = 257, CE_PGS_SCALE = 258;   // 1 
 constexpr int GE_SLOT = 16;
 constexpr int GEOM_ENV_W = MGS * GE_SLOT;
 constexpr int GE_POSE = 0, GE_SIZE = 12, GE_RBOUND = 15;
+// per-environment terrain (optional, cassie_batch_set_env_hfield; F_TR instances): environment e stands on bank entry (unsigned)terrain[e] % K, and the
+// height field's slot of its F_EG row holds its position (GE_POSE, the model's axes) and its x / y half-extents and elevation scale (GE_SIZE); the base
+// thickness is kept on the host only.  Without a selection row the slot's size is not read and the model block's hf_size applies.
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

@@ -23,6 +23,7 @@ template <typename real> struct EnvArrays {
   real *jac; int jfr;                         // mode 4: Jacobian rows [n][FRAME_JAC_W] of frame jfr (F_FR instances)
   real *dyn;                                  // mode 5: dynamics rows [n][DYN_W] (F_FR instances)
   real *acc;                                  // modes 0 / 1: acceleration rows [n][acc_width(nfr)] or null (F_FR instances)
+  const int *terrain;                         // [n] bank entry of each environment, read mod n_terrain (F_TR instances)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -101,6 +102,7 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     EnvPtrs<real> E;   // (E.dbg: the stage dumps are compiled into the extended instance only; batches created with debug = 1 run that one)
     E.cst = A.cst + (size_t)env * CST_W; E.dfilt = A.dfilt + (size_t)env * DFILT_W; E.pd = A.pd + (size_t)env * PD_W; E.xfrc = A.xfrc + (size_t)env * XFRC_W; E.task = A.task ? A.task + (size_t)env * TASK_W : nullptr; E.gait = A.gait ? A.gait + (size_t)env * GAIT_W : nullptr;
     E.hfield = A.hfield ? A.hfield + (size_t)(env % A.n_terrain) * A.hfield_stride : nullptr;
+    if constexpr ((FEAT & F_TR) != 0) { if (A.hfield) E.hfield = A.hfield + (size_t)((unsigned)A.terrain[env] % (unsigned)A.n_terrain) * A.hfield_stride; }   // any value in the row stays inside the bank
     E.obs = A.obs + (size_t)env * OBS_W; E.qM = A.qM + (size_t)env * 2 * NM_MAX; E.dbg = (DBG_IN_ALL_INSTANCES || INST == 1) && A.dbg ? A.dbg + (size_t)env * D_SIZE : nullptr; E.counters = A.counters + (size_t)env * 8;
     E.aux = A.aux ? A.aux + (size_t)env * AUX_W : nullptr; E.cenv = A.cenv ? A.cenv + (size_t)env * CE_W : nullptr; E.cta_sync = sync_on; E.nsub = A.nsub;
     E.est = A.est ? A.est + (size_t)env * EST_W : nullptr; E.est_out = E.obs + OB_EST_OUT;

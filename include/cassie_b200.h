@@ -260,6 +260,11 @@ int cassie_sim_get_hfield_ncol(cassie_sim_t *sim);
 int cassie_sim_get_nhfielddata(cassie_sim_t *sim);
 float *cassie_sim_hfielddata(cassie_sim_t *sim);
 void cassie_sim_set_hfielddata(cassie_sim_t *sim, float *data);
+/* the height field's size [4] (src/cassiemujoco.c:2062-2070): get returns a borrowed read-write host mirror, set copies into it; it is uploaded before
+ * the next step or forward.  An invalid size is not uploaded: the error is recorded and the last valid size stays.  Without a height field: NULL / no
+ * change, and an error. */
+double *cassie_sim_get_hfield_size(cassie_sim_t *sim);
+void cassie_sim_set_hfield_size(cassie_sim_t *sim, double size[4]);
 /* read-only derived quantities (SURVEY.md 8f-2).  include/cassiemujoco.h:200-240 (src/cassiemujoco.c:1586-1699, 1812-1898, 1944-1961).
  * Like the reference, the contact / foot group reads what the LAST step left behind (contact list and forces of the state that step
  * started from); the centre-of-mass group first recomputes the kinematics of the current state (the reference calls mj_fwdPosition).
@@ -484,8 +489,27 @@ int cassie_batch_set_hfielddata(cassie_batch_t *b, const float *data, int n_terr
 int cassie_batch_hfield_nrow(const cassie_batch_t *b);
 int cassie_batch_hfield_ncol(const cassie_batch_t *b);
 
+/* Per-environment terrain (terrain curricula): which bank entry each environment stands on, and where and how large its height field is.  terrain [n]
+ * (bank entry in [0, K) of cassie_batch_set_hfielddata), pos [n][3] (the height field's position in its body frame, as MuJoCo's geom_pos; it stays
+ * axis-aligned), size [n][4] (x half-extent, y half-extent, elevation scale, base thickness, as hfield_size).  A NULL part leaves that part alone; mask
+ * [n] (or NULL: all) selects the environments that change.  The first call gives every environment terrain e % K and the shared position and size, and
+ * the batch then runs kernel instances that read them per environment.  Like the static-geom placement these are model inputs: reset and snapshot
+ * restore leave them alone, cassie_sim_copy copies them.  0, or -1 with nothing changed (cassie_b200_last_error names the environment and the field)
+ * when a terrain is outside [0, K), size[0] or size[1] is not > 0, size[2] or size[3] is < 0, a value is not finite, or the model has no height field.
+ * get: what each environment sees (any pointer may be NULL), with or without rows.  clear: back to terrain e % K and the shared position and size.
+ * The selection row is also cassie_batch_device_ptr(b, "terrain") (int32 [n], row width 1): a write there takes effect at the next launch, and
+ * every kernel reads (unsigned)t % K, so no value addresses outside the bank.  cassie_batch_set_hfielddata with another K keeps the selections, which
+ * are then read mod the new K.  cassie_batch_clear_env_geom_poses also returns the position and size to the shared ones and keeps the selections.
+ * cassie_batch_set_hfield_size sets the shared size (the same checks; the bounding radius follows the model compiler's rule) and returns every
+ * environment's position and size to the shared ones; the selections stay.  get: the shared size. */
+int cassie_batch_set_env_hfield(cassie_batch_t *b, const int *terrain, const double *pos, const double *size, const unsigned char *mask);
+int cassie_batch_get_env_hfield(cassie_batch_t *b, int *terrain, double *pos, double *size);
+int cassie_batch_clear_env_hfield(cassie_batch_t *b);
+int cassie_batch_set_hfield_size(cassie_batch_t *b, const double size[4]);
+int cassie_batch_get_hfield_size(const cassie_batch_t *b, double size[4]);
+
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count]) in the batch precision; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
