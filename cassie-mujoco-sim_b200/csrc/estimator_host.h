@@ -52,10 +52,11 @@ CASSIE_HD inline void estimator_leg_force_t(int side, const T ang[7], const T qu
   const M R3 = RZ_(5), RH = R3 * HF;
   const V hs0 = t0 + R3 * hsp, axh = RH.c2;
   T H = 0, gd = 1; V B{}, dB{};
-  for (int it = 0; it < 5; it++) {   // Newton on |B - A|^2 = L^2 (quadratic: 5 steps from 0 reach the last bit for |H| < 0.3)
+  for (int it = 0; it < 9; it++) {   // Newton on |B - A|^2 = L^2 from 0, 8 updates as the oracle: 4 reach the last bit only for |H| < 0.3, and a leg
+                                     // driven beyond its joint limits (tarsus ~2.4 rad) got forces off by up to 80 % from them
     B = hs0 + RH * (rotz(H) * Bl); dB = B - A;
     gd = 2 * dot(dB, crs(axh, B - hs0));
-    if (it < 4) H -= (dot(dB, dB) - T(0.5012) * T(0.5012)) / gd;
+    if (it < 8) H -= (dot(dB, dB) - T(0.5012) * T(0.5012)) / gd;
   }
   const T a = -2 * dot(dB, crs(ez, B - t0)) / gd, b = -2 * dot(dB, crs(ez, B - s0)) / gd;   // dH/dtarsus, dH/dshin
   // ---- serial chain pelvis -> hip roll -> hip yaw -> hip pitch: frame A2 of the hip-pitch link (exact quarter turns)

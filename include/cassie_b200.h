@@ -377,9 +377,13 @@ void cassie_batch_reset(cassie_batch_t *b, const unsigned char *mask);
  * Replaces n_env calls of src/cassiemujoco.c:1147-1157.  Synchronous.  state_out carries the stateless part of the reference's
  * state_output_step, decoded from the closed archive and checked equal to it to 1e-11: motor / joint position + velocity + torque,
  * pelvis.orientation (+-q, mat2quat's sign), rotationalVelocity, translationalAcceleration, both feet's position / orientation (pelvis frame) and
- * footRotationalVelocity / footTranslationalVelocity (foot frame), radio, battery; toeForce / heelForce when enabled (see
- * cassie_batch_enable_estimator_forces); pelvis.position / translationalVelocity / externalForce and terrain.height (the estimator's filters)
- * when enabled (see cassie_batch_enable_estimator_filter).  externalMoment and terrain.slope are zero, as they are in the reference's output. */
+ * footRotationalVelocity / footTranslationalVelocity (foot frame), radio, battery; toeForce / heelForce and pelvis.position /
+ * translationalVelocity / externalForce, terrain.height (the spring-force model and the filters) from the in-kernel estimator, which this call
+ * switches on by itself (see cassie_batch_enable_estimator_device; ..._forces / ..._filter select the host-side checker instead).
+ * externalMoment and terrain.slope are zero, as they are in the reference's output.
+ * Deviation: the reference runs state_output_step in every cassie_sim_step_pd call; here the estimator comes on at the first call that passes
+ * state_out, so a caller whose first k calls pass NULL gets filters that start k ticks late (as after cassie_batch_reset_estimator at that call).
+ * Calls with NULL state_out before that run the kernel without the estimator stage. */
 void cassie_sim_step_pd_batch(cassie_batch_t *envs, const pd_in_t *pd_in, state_out_t *state_out);
 
 /* throughput path: compact rows.  pd: host [n_env][CASSIE_PD_WIDTH] doubles, copied to the device (and converted to the batch
