@@ -246,10 +246,15 @@ def lib():
     for n in ('cassie_sim_set_dof_damping', 'cassie_sim_set_body_mass', 'cassie_sim_set_body_ipos', 'cassie_sim_set_geom_friction'):
         getattr(L, n).argtypes = [vp, cd]
         getattr(L, n).restype = None
-    for n in ('cassie_sim_set_dof_name_damping', 'cassie_sim_set_body_name_ipos', 'cassie_sim_set_geom_name_friction'):
+    L.cassie_batch_set_env_body_pos.argtypes = [vp, cd, C.c_void_p]
+    L.cassie_batch_get_env_body_pos.argtypes = [vp, cd]
+    L.cassie_batch_clear_env_body_pos.argtypes = [vp]
+    for n in ('set_env_body_pos', 'get_env_body_pos', 'clear_env_body_pos'):
+        getattr(L, 'cassie_batch_' + n).restype = ci
+    for n in ('cassie_sim_set_dof_name_damping', 'cassie_sim_set_body_name_ipos', 'cassie_sim_set_geom_name_friction', 'cassie_sim_set_body_name_pos'):
         getattr(L, n).argtypes = [vp, C.c_char_p, cd]
         getattr(L, n).restype = None
-    for n in ('cassie_sim_get_dof_name_damping', 'cassie_sim_get_body_name_ipos', 'cassie_sim_get_geom_name_friction'):
+    for n in ('cassie_sim_get_dof_name_damping', 'cassie_sim_get_body_name_ipos', 'cassie_sim_get_geom_name_friction', 'cassie_sim_get_body_name_pos'):
         getattr(L, n).argtypes = [vp, C.c_char_p]
         getattr(L, n).restype = cd
     L.cassie_sim_get_joint_num_dof.argtypes = [vp, C.c_char_p]
@@ -506,6 +511,30 @@ class CassieBatch:
     def clear_env_hfield(self):
         """back to terrain e % K and the shared position and size"""
         if self.L.cassie_batch_clear_env_hfield(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    # ---- per-environment body offsets (where a load or tray sits, link and mounting offsets: domain randomisation)
+    def set_env_body_pos(self, pos, mask=None):
+        """each environment's MuJoCo body_pos: pos [nbody, 3] (all environments) or [n, nbody, 3], in model body order; mask [n]: only the selected
+        environments change.  The world body, bodies welded to the world and the extra free body keep the model's offsets (a change raises, and nothing
+        changes).  The mj_setConst constants are not refreshed by this: call set_const, as with the reference.  Reset and snapshot restore leave the
+        offsets alone."""
+        nb = self.L.cassie_batch_nbody(self.h)
+        a = np.ascontiguousarray(np.broadcast_to(np.asarray(pos, dtype=np.float64), (self.n, nb, 3)))
+        m = None if mask is None else np.ascontiguousarray(np.broadcast_to(np.asarray(mask, dtype=np.uint8), (self.n,)))
+        if self.L.cassie_batch_set_env_body_pos(self.h, self._dp(a), None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_body_pos(self):
+        """[n, nbody, 3]: the body offsets each environment sees (the model's without rows)"""
+        out = np.zeros((self.n, self.L.cassie_batch_nbody(self.h), 3))
+        if self.L.cassie_batch_get_env_body_pos(self.h, self._dp(out)) != 0:
+            raise RuntimeError(_last_error())
+        return out
+
+    def clear_env_body_pos(self):
+        """back to the model's body offsets and the kernel instances that ran before"""
+        if self.L.cassie_batch_clear_env_body_pos(self.h) != 0:
             raise RuntimeError(_last_error())
 
     def set_hfield_size(self, size):
@@ -1009,6 +1038,13 @@ class CassieSim:
             return np.array(self.L.cassie_sim_get_body_name_ipos(self.c, name.encode())[:3])
         return self._marr(self.L.cassie_sim_body_ipos, 3 * self.params()[4])
 
+    def get_body_pos(self, name):
+        """the body's position in its parent frame (reference: example/cassiemujoco.py:437-442)"""
+        ptr = self.L.cassie_sim_get_body_name_pos(self.c, name.encode())
+        if not ptr:
+            raise RuntimeError(_last_error())
+        return np.array(ptr[:3])
+
     def get_geom_friction(self, name=None):
         if name:
             return np.array(self.L.cassie_sim_get_geom_name_friction(self.c, name.encode())[:3])
@@ -1033,6 +1069,12 @@ class CassieSim:
             self.L.cassie_sim_set_body_mass(self.c, self._carr(data))
         else:
             self.L.cassie_sim_set_body_name_mass(self.c, name.encode(), float(data))
+
+    def set_body_pos(self, name, data):
+        """moves the body in its parent frame from the next step on (reference: example/cassiemujoco.py:563-570); call set_const for the
+        mj_setConst constants, as with the reference"""
+        assert len(data) == 3
+        self.L.cassie_sim_set_body_name_pos(self.c, name.encode(), self._carr(data))
 
     def set_body_ipos(self, data, name=None):
         if name:

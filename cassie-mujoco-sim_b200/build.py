@@ -30,6 +30,10 @@ FRAME_INSTANCES = [('f114', 'float', 1, 20), ('f117', 'float', 1, 23), ('d117', 
 # height field's size come from per-environment rows; in each instance kind, and the extended kernel with frame rows; tag = precision, kind, features in hex
 TERRAIN_INSTANCES = [('f02f', 'float', 0, 47), ('f12f', 'float', 1, 47), ('f22f', 'float', 2, 47), ('d02f', 'double', 0, 47), ('d12f', 'double', 1, 47), ('d22f', 'double', 2, 47),
                      ('f13f', 'float', 1, 63), ('d13f', 'double', 1, 63)]
+# the extended kernel with per-environment body offsets (feature 64 = F_BP; cassie_batch_set_env_body_pos): each differs from its counterpart (f14, f117 /
+# d117, f11f / d11f, f13f / d13f) by F_BP only; tag = precision, kind, features in hex
+BODY_POS_INSTANCES = [('f144', 'float', 1, 68), ('f157', 'float', 1, 87), ('d157', 'double', 1, 87), ('f15f', 'float', 1, 95), ('d15f', 'double', 1, 95),
+                      ('f17f', 'float', 1, 127), ('d17f', 'double', 1, 127)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -63,7 +67,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

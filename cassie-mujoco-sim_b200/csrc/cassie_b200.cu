@@ -32,6 +32,7 @@ CASSIE_STEP_ENTRY(f0c) CASSIE_STEP_ENTRY(f1c) CASSIE_STEP_ENTRY(f2c) CASSIE_STEP
 CASSIE_STEP_ENTRY(d0f) CASSIE_STEP_ENTRY(d1f) CASSIE_STEP_ENTRY(d2f)
 CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_STEP_ENTRY(f11c) CASSIE_STEP_ENTRY(f11f) CASSIE_STEP_ENTRY(d11f)
 CASSIE_STEP_ENTRY(f02f) CASSIE_STEP_ENTRY(f12f) CASSIE_STEP_ENTRY(f22f) CASSIE_STEP_ENTRY(d02f) CASSIE_STEP_ENTRY(d12f) CASSIE_STEP_ENTRY(d22f) CASSIE_STEP_ENTRY(f13f) CASSIE_STEP_ENTRY(d13f)
+CASSIE_STEP_ENTRY(f144) CASSIE_STEP_ENTRY(f157) CASSIE_STEP_ENTRY(d157) CASSIE_STEP_ENTRY(f15f) CASSIE_STEP_ENTRY(d15f) CASSIE_STEP_ENTRY(f17f) CASSIE_STEP_ENTRY(d17f)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -41,6 +42,15 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_BP) {   // per-environment body offsets: extended instances only (a batch with offset rows always has constant rows)
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP; return dbl ? cassie_step_entry_d17f() : cassie_step_entry_f17f(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP; return dbl ? cassie_step_entry_d15f() : cassie_step_entry_f15f(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP; return cassie_step_entry_f144(); }   // no frame / acceleration / dynamics / Jacobian launch
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP;
+    return dbl ? cassie_step_entry_d157() : cassie_step_entry_f157();
+  }
   if (feat & F_TR) {   // per-environment terrain (always with the per-environment static geoms): F_ALL | F_EG | F_TR, with or without frame rows
     const bool dbl = std::is_same<real, double>::value, fr = (feat & F_FR) != 0;
     if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | (fr ? F_FR : 0);
@@ -292,6 +302,10 @@ struct BatchBase {
   virtual bool get_env_hfield(int *terrain, double *pos, double *size) = 0;
   virtual bool clear_env_hfield() = 0;
   virtual bool set_hfield_size(const double *size) = 0;   // the shared size; every environment's height-field position and size follow the shared ones
+  // per-environment body offsets [n][nbody][3] (F_BP instances): only masked environments change; checked as a whole before anything changes
+  virtual bool set_env_body_pos(const double *pos, const unsigned char *mask) = 0;
+  virtual bool get_env_body_pos(double *pos) = 0;
+  virtual bool clear_env_body_pos() = 0;
   virtual bool set_frames(const char *const *names, const int *kinds, int count) = 0;   // frame rows [n][count][FRAME_W]; count 0: none
   virtual bool frame_jacobian(int frame, double *jacp, double *jacr) = 0;                 // [n][3][nv] each at the current state (launch mode 4); jacr may be null
   virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
@@ -336,9 +350,12 @@ template <typename real> struct Batch : BatchBase {
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   int *d_terrain = nullptr;                // A.terrain: [n] per-environment bank entries, allocated by the first per-environment terrain (F_TR instances)
   std::vector<double> hf_host;             // [n][7] height-field position (in its body frame) 3, size 4 per environment; empty: the shared ones
+  real *d_bpos = nullptr;                  // A.bpos: [n][BP_W] per-environment body offsets, allocated by the first cassie_batch_set_env_body_pos (F_BP instances)
+  std::vector<double> bp_host;             // [n][nbody][3] the offsets every environment sees while d_bpos exists (in double: what get returns)
+  bool bp_cenv = false;                    // the constant rows were allocated by the body-offset setter, and no model-row setter has written them since
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -405,6 +422,8 @@ template <typename real> struct Batch : BatchBase {
         if (hm.nhfield == 1) {   // per-environment terrain: F_ALL | F_EG | F_TR (the scratch of F_ALL)
           CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
           if (ext == 1) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR | F_FR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }
+        if (ext == 1)   // per-environment body offsets: every instance step_entry routes F_BP launches to (the extended scratch)
+          for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -458,6 +477,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(what, "body_ipos") && h_model_copy.xb >= 0) for (int e = 0; e < n; e++) for (int k = 0; k < 3; k++)
       if (rows[(size_t)e * w + 3 * h_model_copy.xb + k] != hm.body_ipos[3 * h_model_copy.xb + k]) { set_err("body_ipos of the extra free body cannot be changed (its inertial frame must stay its body frame)"); return false; }
     if (!ensure_cenv()) return false;
+    bp_cenv = false;
     std::vector<real> all((size_t)n * CE_W);
     CUDA_OK(cudaMemcpyAsync(all.data(), A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
     for (int e = 0; e < n; e++) for (int i = 0; i < w; i++) { int ww; const int sl = cenv_slot(what, i, ww); if (sl >= 0) all[(size_t)e * CE_W + sl] = (real)rows[(size_t)e * w + i]; }
@@ -743,6 +763,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     DevModel<real> *hmodel = (DevModel<real> *)calloc(1, model_bytes<real>()); std::string err; BuildInfo info;
     if (!build_dev_model(hm, *hmodel, err, &info)) { free(hmodel); set_err(err); return false; }
+    if (d_bpos) hmodel->robot_reach = rows_reach(*hmodel);   // per-environment body offsets: the broad phase's bound covers every row
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaMemcpy(d_model, hmodel, model_bytes<real>(), cudaMemcpyHostToDevice));
     h_model_copy = *hmodel; free(hmodel);
@@ -754,6 +775,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     hm = src->hm;
     if (!rebuild_model()) return false;
+    if (!src->d_bpos && !clear_env_body_pos()) return false;   // before the constant rows are copied: clearing drops rows the offset setter allocated
     if (src->A.cenv) { if (!ensure_cenv()) return false; CUDA_OK(cudaMemcpyAsync(A.cenv, src->A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToDevice, stream)); }
     else if (A.cenv) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; }
     if (!src->d_terrain && !clear_env_hfield()) return false;
@@ -765,6 +787,7 @@ template <typename real> struct Batch : BatchBase {
       CUDA_OK(cudaMemcpyAsync(d_terrain, src->d_terrain, sizeof(int) * n, cudaMemcpyDeviceToDevice, stream));
       hf_host = src->hf_host;
     }
+    if (src->d_bpos) { bp_host = src->bp_host; bp_cenv = src->bp_cenv; if (!put_bpos()) return false; }   // the source's constant rows came above
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
       std::vector<float> tmp(cells); CUDA_OK(cudaMemcpy(tmp.data(), src->d_hfield, sizeof(float) * cells, cudaMemcpyDeviceToHost));
@@ -915,6 +938,63 @@ template <typename real> struct Batch : BatchBase {
     hm.geom_rbound[g] = std::sqrt(size[0] * size[0] + size[1] * size[1] + z * z);   // the model compiler's bound for the new size
     return rebuild_model() && shared_geom_changed(g);   // every environment's height-field position and size follow the shared ones
   }
+  // ---- per-environment body offsets (loads, trays, link offsets): MuJoCo's body_pos per environment, read by the F_BP instances' kinematics and by the
+  // ray and camera kernels
+  real rows_reach(const DevModel<real> &d) const {   // the block's robot_reach for the rows: build_dev_model's bound, the largest over the environments
+    const int nb3 = 3 * hm.nbody; double r = 0;
+    for (int e = 0; e < n; e++) r = std::max(r, robot_reach_of(hm, &bp_host[(size_t)e * nb3], d.root_body, d.xb, geom_dev));
+    return (real)(r * 1.05 + 0.05);
+  }
+  bool put_bpos() {   // the device rows and the block's robot_reach from the mirror
+    const int nb3 = 3 * hm.nbody;
+    std::vector<real> all((size_t)n * BP_W, real(0));
+    for (int e = 0; e < n; e++) for (int i = 0; i < nb3; i++) all[(size_t)e * BP_W + i] = (real)bp_host[(size_t)e * nb3 + i];
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows and the block
+    if (!d_bpos) CUDA_OK(cudaMalloc(&d_bpos, sizeof(real) * n * BP_W));
+    CUDA_OK(cudaMemcpy(d_bpos, all.data(), sizeof(real) * n * BP_W, cudaMemcpyHostToDevice));
+    h_model_copy.robot_reach = rows_reach(h_model_copy);
+    CUDA_OK(cudaMemcpy(&d_model->robot_reach, &h_model_copy.robot_reach, sizeof(real), cudaMemcpyHostToDevice));
+    A.bpos = d_bpos;
+    return true;
+  }
+  bool set_env_body_pos(const double *pos, const unsigned char *mask) override {
+    const std::string verb = "cassie_batch_set_env_body_pos";
+    if (!pos) { set_err(verb + ": pos is required"); return false; }
+    const int nb = hm.nbody, nb3 = 3 * nb;
+    for (int e = 0; e < n; e++) {   // every masked environment is checked before anything changes
+      if (mask && !mask[e]) continue;
+      const double *now = bp_host.empty() ? hm.body_pos.data() : &bp_host[(size_t)e * nb3];
+      for (int b = 0; b < nb; b++) {
+        const double *p = pos + (size_t)e * nb3 + 3 * b;
+        const std::string at = verb + ": environment " + std::to_string(e) + ", body " + hm.names_body[b] + ": ";
+        if (!std::isfinite(p[0]) || !std::isfinite(p[1]) || !std::isfinite(p[2])) { set_err(at + "pos is not finite"); return false; }
+        if (p[0] == now[3 * b] && p[1] == now[3 * b + 1] && p[2] == now[3 * b + 2]) continue;
+        const std::string w = env_body_pos_check(hm, b, h_model_copy.xb);
+        if (!w.empty()) { set_err(at + "the offset of " + w + " cannot change"); return false; }
+      }
+    }
+    if (!A.cenv) bp_cenv = true;
+    if (!ensure_cenv()) return false;   // mode 3 (set_const) writes the environment's invweights into its constant row
+    if (bp_host.empty()) { bp_host.resize((size_t)n * nb3); for (int e = 0; e < n; e++) memcpy(&bp_host[(size_t)e * nb3], hm.body_pos.data(), sizeof(double) * nb3); }
+    for (int e = 0; e < n; e++) if (!mask || mask[e]) memcpy(&bp_host[(size_t)e * nb3], pos + (size_t)e * nb3, sizeof(double) * nb3);
+    return put_bpos();
+  }
+  bool get_env_body_pos(double *pos) override {
+    if (!pos) { set_err("cassie_batch_get_env_body_pos: pos is required"); return false; }
+    const int nb3 = 3 * hm.nbody;
+    for (int e = 0; e < n; e++) memcpy(pos + (size_t)e * nb3, bp_host.empty() ? hm.body_pos.data() : &bp_host[(size_t)e * nb3], sizeof(double) * nb3);
+    return true;
+  }
+  // back to the model's offsets and the instances that ran before: the block's robot_reach is the model's again, and constant rows the setter
+  // allocated (and no model-row setter wrote since) are dropped
+  bool clear_env_body_pos() override {
+    bp_host.clear();
+    if (!d_bpos) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_bpos)); d_bpos = nullptr; A.bpos = nullptr;
+    if (bp_cenv) { CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; bp_cenv = false; }
+    return rebuild_model();
+  }
   // ---- frame rows: the table is checked as a whole before anything changes; the rows start at zero and are filled by the next step / forward launch
   bool set_frames(const char *const *names, const int *kinds, int count) override {
     if (count < 0 || count > FRAME_MAX || (count > 0 && (!names || !kinds))) { set_err("cassie_batch_set_frames: between 0 and " + std::to_string(FRAME_MAX) + " frames, with names and kinds"); return false; }
@@ -1016,7 +1096,7 @@ template <typename real> struct Batch : BatchBase {
     if (!nray) { set_err("cassie_batch_raycast: no rays are set (cassie_batch_set_rays)"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (!d_rays) CUDA_OK(cudaMalloc(&d_rays, sizeof(real) * n * nray * RAY_SLOT));
-    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride; R.terrain = d_terrain;
+    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride; R.terrain = d_terrain; R.bpos = d_bpos;
     R.tab = d_rtab; R.k = nray; R.out = d_rays; R.n = n;
     CUDA_OK(launch_raycast<real>(R, device, stream));
     launches++; rays_done = true;
@@ -1044,7 +1124,7 @@ template <typename real> struct Batch : BatchBase {
     if (!cam.width) { set_err("cassie_batch_render_depth: no camera is set (cassie_batch_set_camera)"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (!d_depth) CUDA_OK(cudaMalloc(&d_depth, sizeof(real) * n * cam.width * cam.height));
-    CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain;
+    CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = d_bpos;
     C.body = cam.body; C.width = cam.width; C.height = cam.height; C.tan_half = (real)std::tan(cam.fovy * M_PI / 360); C.zfar = (real)cam.zfar;
     for (int i = 0; i < 3; i++) C.pos[i] = (real)cam.pos[i];
     for (int i = 0; i < 4; i++) C.quat[i] = (real)cam.quat[i];
@@ -1086,7 +1166,7 @@ template <typename real> struct Batch : BatchBase {
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1193,7 +1273,9 @@ struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[6
   // the acceleration row of the simulator's batch (qacc, then the cacc of every body and site frame) and the nv-entry qacc mirror cassie_sim_qacc lends out
   std::vector<double> acc, qacc;
   // the height field's size (cassie_sim_get_hfield_size / set_hfield_size): a host mirror, uploaded before the next launch when it is valid
-  double hf_size[4] = {0, 0, 0, 0}, hf_size_dev[4] = {0, 0, 0, 0}; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
+  double hf_size[4] = {0, 0, 0, 0}, hf_size_dev[4] = {0, 0, 0, 0};
+  // body offsets (cassie_sim_get_body_name_pos / set_body_name_pos): [nbody][3] host mirror; the constant block is rebuilt from it when it changes
+  std::vector<double> m_bpos, m_bpos_dev; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
 
 // cassie_state_t (include/cassiemujoco.h:434-463): a device-resident snapshot of one simulator's rows plus the host mirrors the reference hands out as
 // borrowed pointers (time, qpos, qvel); the snapshot is allocated by the first cassie_get_state, which also fixes the owning simulator's sizes
@@ -1334,6 +1416,8 @@ static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote thr
   if (c->m_gpos != c->m_gpos_dev || c->m_gquat != c->m_gquat_dev || c->m_gsize != c->m_gsize_dev) {   // a geom was moved / turned / resized (src/cassiemujoco.c:1438-1541)
     HostModel &hm = c->b->impl->hm; hm.geom_pos = c->m_gpos; hm.geom_quat = c->m_gquat; hm.geom_size = c->m_gsize;
     c->b->impl->rebuild_model(); c->m_gpos_dev = c->m_gpos; c->m_gquat_dev = c->m_gquat; c->m_gsize_dev = c->m_gsize; }
+  if (c->m_bpos != c->m_bpos_dev) {   // a body was moved (src/cassiemujoco.c:1408-1418): kinematics, static geoms' world poses and the broad phase's bound follow
+    c->b->impl->hm.body_pos = c->m_bpos; c->b->impl->rebuild_model(); c->m_bpos_dev = c->m_bpos; }
 }
 cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   std::string path;
@@ -1354,7 +1438,8 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   sim_pull(c);
   { const HostModel &hm = b->impl->hm; c->m_mass = hm.body_mass; c->m_ipos = hm.body_ipos; c->m_damp = hm.dof_damping; c->m_fric = hm.geom_friction;
     c->m_mass_dev = c->m_mass; c->m_ipos_dev = c->m_ipos; c->m_damp_dev = c->m_damp; c->m_fric_dev = c->m_fric;
-    c->m_gpos = hm.geom_pos; c->m_gquat = hm.geom_quat; c->m_gsize = hm.geom_size; c->m_gpos_dev = c->m_gpos; c->m_gquat_dev = c->m_gquat; c->m_gsize_dev = c->m_gsize; }
+    c->m_gpos = hm.geom_pos; c->m_gquat = hm.geom_quat; c->m_gsize = hm.geom_size; c->m_gpos_dev = c->m_gpos; c->m_gquat_dev = c->m_gquat; c->m_gsize_dev = c->m_gsize;
+    c->m_bpos = c->m_bpos_dev = hm.body_pos; }
   if (b->impl->hm.nhfield) { c->hfield.assign((size_t)b->impl->hm.hfield_nrow[0] * b->impl->hm.hfield_ncol[0], 0.0f); c->hfield_dev = c->hfield;
                              for (int k = 0; k < 4; k++) c->hf_size[k] = c->hf_size_dev[k] = b->impl->hm.hfield_size[k]; }
   return c;
@@ -1532,6 +1617,17 @@ void cassie_sim_set_body_name_mass(cassie_sim_t *c, const char *name, double mas
 double cassie_sim_get_body_name_mass(cassie_sim_t *c, const char *name) { const int id = c->b->impl->hm.body_id(name ? name : ""); return id >= 0 ? c->m_mass[id] : 0.0; }
 void cassie_sim_set_body_name_ipos(cassie_sim_t *c, const char *name, double *ipos) { const int id = c->b->impl->hm.body_id(name ? name : ""); if (id >= 0) for (int k = 0; k < 3; k++) c->m_ipos[3 * id + k] = ipos[k]; }
 double *cassie_sim_get_body_name_ipos(cassie_sim_t *c, const char *name) { const int id = c->b->impl->hm.body_id(name ? name : ""); return id >= 0 ? &c->m_ipos[3 * id] : nullptr; }
+// src/cassiemujoco.c:1408-1418: a body's position in its parent frame through the host mirror (uploaded before the next launch); any body is accepted,
+// the world body's and the extra free body's entries have no effect, as in MuJoCo.  An unknown name: NULL / no change, and an error (the reference indexes -1)
+double *cassie_sim_get_body_name_pos(cassie_sim_t *c, const char *name) {
+  const int id = c->b->impl->hm.body_id(name ? name : "");
+  if (id < 0) { set_err(std::string("cassie_sim_get_body_name_pos: unknown body ") + (name ? name : "(null)")); return nullptr; }
+  return &c->m_bpos[3 * id];
+}
+void cassie_sim_set_body_name_pos(cassie_sim_t *c, const char *name, double *data) {
+  double *p = cassie_sim_get_body_name_pos(c, name);
+  if (p && data) for (int k = 0; k < 3; k++) p[k] = data[k];
+}
 int cassie_sim_get_joint_num_dof(cassie_sim_t *c, const char *name) { const HostModel &hm = c->b->impl->hm; const int j = hm.joint_id(name ? name : ""); if (j < 0) return 0; return hm.jnt_type[j] == JNT_FREE ? 6 : (hm.jnt_type[j] == JNT_BALL ? 3 : 1); }
 void cassie_sim_set_dof_name_damping(cassie_sim_t *c, const char *name, double *damp) { const HostModel &hm = c->b->impl->hm; const int j = hm.joint_id(name ? name : ""); if (j < 0) return; const int nd = cassie_sim_get_joint_num_dof(c, name); for (int i = 0; i < nd; i++) c->m_damp[hm.jnt_dofadr[j] + i] = damp[i]; }
 double *cassie_sim_get_dof_name_damping(cassie_sim_t *c, const char *name) { const HostModel &hm = c->b->impl->hm; const int j = hm.joint_id(name ? name : ""); return j >= 0 ? &c->m_damp[hm.jnt_dofadr[j]] : nullptr; }
@@ -1602,6 +1698,10 @@ int cassie_batch_clear_env_geom_poses(cassie_batch_t *b) { return b->impl->clear
 int cassie_batch_set_env_hfield(cassie_batch_t *b, const int *terrain, const double *pos, const double *size, const unsigned char *mask) { return b->impl->set_env_hfield(terrain, pos, size, mask) ? 0 : -1; }
 int cassie_batch_get_env_hfield(cassie_batch_t *b, int *terrain, double *pos, double *size) { return b->impl->get_env_hfield(terrain, pos, size) ? 0 : -1; }
 int cassie_batch_clear_env_hfield(cassie_batch_t *b) { return b->impl->clear_env_hfield() ? 0 : -1; }
+// per-environment body offsets; see include/cassie_b200.h
+int cassie_batch_set_env_body_pos(cassie_batch_t *b, const double *pos, const unsigned char *mask) { return b->impl->set_env_body_pos(pos, mask) ? 0 : -1; }
+int cassie_batch_get_env_body_pos(cassie_batch_t *b, double *pos) { return b->impl->get_env_body_pos(pos) ? 0 : -1; }
+int cassie_batch_clear_env_body_pos(cassie_batch_t *b) { return b->impl->clear_env_body_pos() ? 0 : -1; }
 int cassie_batch_set_hfield_size(cassie_batch_t *b, const double size[4]) { return b->impl->set_hfield_size(size) ? 0 : -1; }
 int cassie_batch_get_hfield_size(const cassie_batch_t *b, double size[4]) {
   const HostModel &hm = b->impl->hm;
@@ -1736,6 +1836,7 @@ void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *csrc) {
   dst->m_gpos = dst->m_gpos_dev = src->m_gpos; dst->m_gquat = dst->m_gquat_dev = src->m_gquat; dst->m_gsize = dst->m_gsize_dev = src->m_gsize;
   dst->hfield = src->hfield; dst->hfield_dev = src->hfield_dev; dst->timestep = dst->timestep_dev = src->timestep;
   memcpy(dst->hf_size, src->hf_size, sizeof dst->hf_size); memcpy(dst->hf_size_dev, src->hf_size_dev, sizeof dst->hf_size_dev);
+  dst->m_bpos = src->m_bpos; dst->m_bpos_dev = src->m_bpos_dev;
   for (int i = 0; i < 16; i++) dst->b->radio[i] = src->b->radio[i];
   cassie_state_t *s = cassie_state_alloc(); cassie_get_state(src, s); cassie_set_state(dst, s); cassie_state_free(s);
 }

@@ -80,6 +80,29 @@ inline int env_geom_check(const HostModel &m, const int *geom_dev, int g, std::s
   return geom_dev[g] - MG;
 }
 
+// the obstacle broad phase's robot bound (DevModel::robot_reach, before its slack) for body offsets bp [nbody][3]: build_dev_model's rule -- the
+// farthest any collision geom of the robot reaches from the root body's origin along the offset chain -- over the geoms that have a moving slot
+inline double robot_reach_of(const HostModel &m, const double *bp, int root, int xb, const int *geom_dev) {
+  std::vector<double> reach(m.nbody, 0.0);
+  for (int b = 1; b < m.nbody; b++) if (m.body_weldid[b] != 0 && b != root && b != xb) {
+    const double *p = bp + 3 * b; reach[b] = reach[m.body_parentid[b]] + std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]); }
+  double r = 0;
+  for (int g = 0; g < m.ngeom && g < 256; g++) {
+    const int b = m.geom_bodyid[g];
+    if (geom_dev[g] < 0 || geom_dev[g] >= MG || b == xb) continue;
+    const double *gp = &m.geom_pos[3 * g]; r = std::max(r, reach[b] + std::sqrt(gp[0] * gp[0] + gp[1] * gp[1] + gp[2] * gp[2]) + m.geom_rbound[g]);
+  }
+  return r;
+}
+// a body offset the per-environment verb may change: an empty reason, else why not (the world body, a body welded to the world -- its geoms are static
+// and placed per environment by the static-geom verbs -- and the extra free body, whose pose is qpos)
+inline std::string env_body_pos_check(const HostModel &m, int b, int xb) {
+  if (b == 0) return "the world body";
+  if (m.body_weldid[b] == 0) return "a body welded to the world (place its geoms with cassie_batch_set_env_geom_pose / set_env_hfield)";
+  if (b == xb) return "the extra free body (its pose is qpos)";
+  return std::string();
+}
+
 // one row of a batch's frame table (FT_W) for body (kind 0) or site (kind 1) `name`; its id, or -1 with a reason for an unknown name or kind
 template <typename real> int frame_table_row(const HostModel &m, const char *name, int kind, real *row, std::string &err) {
   for (int c = 0; c < FT_W; c++) row[c] = 0;

@@ -34,6 +34,7 @@ constexpr int F_XB = 1, F_HFIELD = 2, F_BOX = 4, F_ALL = 7;   // extra free body
 constexpr int F_EG = 8;   // the static geoms' world poses, sizes and bounding radii come from per-environment rows (GEOM_ENV_W) instead of the model block
 constexpr int F_FR = 16;  // frame rows (FRAME_W per named body / site) are filled in the last sub-step of a launch (extended instances only)
 constexpr int F_TR = 32;  // per-environment terrain: the bank entry from a selection row, the height field's size from its F_EG slot (with F_ALL | F_EG only)
+constexpr int F_BP = 64;  // per-environment body offsets: each body's position in its parent frame comes from a BP_W row instead of the model block (extended instances only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -170,6 +171,9 @@ constexpr int GE_POSE = 0, GE_SIZE = 12, GE_RBOUND = 15;
 // per-environment terrain (optional, cassie_batch_set_env_hfield; F_TR instances): environment e stands on bank entry (unsigned)terrain[e] % K, and the
 // height field's slot of its F_EG row holds its position (GE_POSE, the model's axes) and its x / y half-extents and elevation scale (GE_SIZE); the base
 // thickness is kept on the host only.  Without a selection row the slot's size is not read and the model block's hf_size applies.
+// per-environment body offsets (optional, cassie_batch_set_env_body_pos; F_BP instances): MuJoCo's body_pos of every body [MB][3] in model body order,
+// the rest of the row zero.  The kinematics, the ray and the camera kernels read it instead of DevModel::body_pos.  A model input like the CE rows.
+constexpr int BP_W = MB * 3;
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

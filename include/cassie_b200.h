@@ -335,6 +335,13 @@ double cassie_sim_get_body_name_mass(cassie_sim_t *c, const char *name);        
 void cassie_sim_set_body_ipos(cassie_sim_t *c, double *ipos);          /* :1385 (reads ipos[i + j], as the reference does) */
 void cassie_sim_set_body_name_ipos(cassie_sim_t *c, const char *name, double *ipos);     /* :1394 */
 double *cassie_sim_get_body_name_ipos(cassie_sim_t *c, const char *name);                /* :1402 */
+/* src/cassiemujoco.c:1408-1418: a body's position in its parent frame (MuJoCo's body_pos).  get returns a borrowed read-write pointer into an
+ * [nbody][3] host mirror, set copies 3 values into it; when the mirror changed, the constant block is rebuilt from it before the next launch (the
+ * static geoms' world poses and the broad phase's robot bound follow, so moving "floor" moves the height field).  Any body is accepted; the world
+ * body's and the extra free body's entries have no effect, as in MuJoCo.  The constants of mj_setConst are not refreshed: call cassie_sim_set_const.
+ * An unknown name: NULL / no change, and an error (the reference indexes -1). */
+void cassie_sim_set_body_name_pos(cassie_sim_t *c, const char *name, double *data);
+double *cassie_sim_get_body_name_pos(cassie_sim_t *c, const char *name);
 void cassie_sim_set_geom_friction(cassie_sim_t *c, double *fric);      /* :1420 */
 void cassie_sim_set_geom_name_friction(cassie_sim_t *c, const char *name, double *fric); /* :1427 (addresses the geom's own triple) */
 double *cassie_sim_get_geom_name_friction(cassie_sim_t *c, const char *name);            /* :1433 */
@@ -511,6 +518,22 @@ int cassie_batch_get_env_hfield(cassie_batch_t *b, int *terrain, double *pos, do
 int cassie_batch_clear_env_hfield(cassie_batch_t *b);
 int cassie_batch_set_hfield_size(cassie_batch_t *b, const double size[4]);
 int cassie_batch_get_hfield_size(const cassie_batch_t *b, double size[4]);
+
+/* Per-environment body offsets (domain randomisation of where a load or tray sits, and of link and mounting offsets): pos [n][nbody][3] is each
+ * environment's MuJoCo body_pos (a body's position in its parent frame; body_quat stays the model's), mask [n] (or NULL: all) selects the environments
+ * that change.  The first call gives every environment the model's offsets; the batch then also carries constant rows (cassie_batch_set_body_mass &
+ * co.) and runs kernel instances that read the offsets per environment in the kinematics: everything that follows from the body poses (contacts,
+ * sensors, connect rows, frames, Jacobians, dynamics and acceleration rows, rays, depth images) follows.  As in MuJoCo, offsets inside a leg's closed
+ * loop open it at qpos0 and the connect rows pull it shut; the mj_setConst constants are not refreshed by themselves (cassie_batch_set_const); the
+ * in-kernel estimator keeps the model's leg geometry.  The broad phase's robot bound is recomputed over all rows.  0, or -1 with nothing changed
+ * (cassie_b200_last_error names the environment and the body) for a non-finite value, or a change of the world body, of a body welded to the world
+ * (its geoms are static: cassie_batch_set_env_geom_pose / set_env_hfield place them per environment) or of the extra free body (its pose is qpos).
+ * The rows are model inputs: reset and snapshot restore leave them alone, cassie_sim_copy copies them.  get: what every environment sees (the model's
+ * offsets without rows).  clear: back to the model's offsets and the instances that ran before (constant rows the setter allocated are dropped unless
+ * a model-row setter wrote them since). */
+int cassie_batch_set_env_body_pos(cassie_batch_t *b, const double *pos, const unsigned char *mask);
+int cassie_batch_get_env_body_pos(cassie_batch_t *b, double *pos);
+int cassie_batch_clear_env_body_pos(cassie_batch_t *b);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
  * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
