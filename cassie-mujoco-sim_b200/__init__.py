@@ -14,6 +14,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libcassie_b200.so')
 MODEL_DIR = os.path.join(_HERE, 'models')
 FP32, FP64 = 0, 1
+LINE_MAX = 6   # the longest torque delay in control ticks (the delay line's length, csrc/devmodel.h AC_MAXDELAY)
+NU = 10   # motors: every supported model has Cassie's ten (csrc/devmodel.h MU), in the model's actuator order
 PD_WIDTH, OBS_WIDTH, AUX_WIDTH, EST_WIDTH = 52, 112, 64, 16
 # one frame's slot of a frame row (CASSIE_FRAME_* in include/cassie_b200.h) and the frame kinds of set_frames
 FRAME_WIDTH, FRAME_BODY, FRAME_SITE, FRAME_MAX = 20, 0, 1, 64
@@ -537,6 +539,79 @@ class CassieBatch:
         if self.L.cassie_batch_clear_env_body_pos(self.h) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- per-environment actuators (actuator latency and torque saturation: sim-to-real randomisation) and the controller-stage state
+    def _act_lib(self):
+        L = self.L
+        if not getattr(L, '_act_bound', False):
+            vp, dp, ip = C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int)
+            L.cassie_batch_set_env_actuators.argtypes = [vp, dp, dp, ip, vp]
+            L.cassie_batch_get_env_actuators.argtypes = [vp, dp, dp, ip]
+            L.cassie_batch_clear_env_actuators.argtypes = [vp]
+            L.cassie_batch_get_actuator_state.argtypes = [vp, dp, ip, dp, dp]
+            L.cassie_batch_set_actuator_state.argtypes = [vp, dp, ip, dp, dp, vp]
+            for n in ('set_env_actuators', 'get_env_actuators', 'clear_env_actuators', 'get_actuator_state', 'set_actuator_state'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._act_bound = True
+        return L
+
+    @staticmethod
+    def _arr(a, dtype, shape):
+        return None if a is None else np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=dtype), shape))
+
+    def set_env_actuators(self, ctrlrange=None, rpm=None, delay=None, mask=None):
+        """each environment's actuators, per motor (10, in the model's actuator order): ctrlrange [nu, 2] or [n, nu, 2] -- MuJoCo's actuator_ctrlrange
+        (lo, hi): the clamp of ctrl and motor()'s peak torque --, rpm [nu] or [n, nu] -- the no-load speed (actuator_user) --, delay [nu] or [n, nu] --
+        the torque delay in control ticks, 0..6 (6: the reference's).  A part left None is kept; mask [n]: only the selected environments change.  A
+        non-finite value, lo >= hi, rpm <= 0 or a delay outside 0..6 raises, and nothing changes.  Reset and snapshot restore leave the rows alone."""
+        L, nu = self._act_lib(), NU
+        cr = self._arr(ctrlrange, np.float64, (self.n, nu, 2))
+        rp = self._arr(rpm, np.float64, (self.n, nu))
+        m = self._arr(mask, np.uint8, (self.n,))
+        dl = None
+        if delay is not None:   # checked before the conversion to int32, which would wrap a large value into the range
+            d = np.broadcast_to(np.asarray(delay, dtype=np.float64), (self.n, nu))
+            dm = d if m is None else d[m != 0]
+            if not np.all(np.isfinite(dm)) or np.any(dm != np.round(dm)) or np.any((dm < 0) | (dm > LINE_MAX)):
+                raise RuntimeError('set_env_actuators: delay must be whole ticks in 0..%d' % LINE_MAX)
+            dl = np.ascontiguousarray(np.where(np.isfinite(d) & (d >= 0) & (d <= LINE_MAX), d, 0).astype(np.int32))   # unmasked rows are not read
+        ptr = lambda a, t: None if a is None else a.ctypes.data_as(C.POINTER(t))
+        if L.cassie_batch_set_env_actuators(self.h, ptr(cr, C.c_double), ptr(rp, C.c_double), ptr(dl, C.c_int), None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_actuators(self):
+        """(ctrlrange [n, nu, 2], rpm [n, nu], delay [n, nu] int): the actuators each environment sees (the model's without rows)"""
+        L, nu = self._act_lib(), NU
+        cr, rp, dl = np.zeros((self.n, nu, 2)), np.zeros((self.n, nu)), np.zeros((self.n, nu), dtype=np.int32)
+        if L.cassie_batch_get_env_actuators(self.h, self._dp(cr), self._dp(rp), dl.ctypes.data_as(C.POINTER(C.c_int))) != 0:
+            raise RuntimeError(_last_error())
+        return cr, rp, dl
+
+    def clear_env_actuators(self):
+        """back to the model's actuators and the kernel instances that ran before"""
+        if self._act_lib().cassie_batch_clear_env_actuators(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def actuator_state(self):
+        """dict of the controller-stage state: torque_delay [n, 10, 6] (slot 0 newest), drive_filter [n, 10, 9] int32, joint_x [n, 6, 4], joint_y [n, 6, 3]"""
+        L = self._act_lib()
+        td, df, jx, jy = np.zeros((self.n, 10, 6)), np.zeros((self.n, 10, 9), dtype=np.int32), np.zeros((self.n, 6, 4)), np.zeros((self.n, 6, 3))
+        if L.cassie_batch_get_actuator_state(self.h, self._dp(td), df.ctypes.data_as(C.POINTER(C.c_int)), self._dp(jx), self._dp(jy)) != 0:
+            raise RuntimeError(_last_error())
+        return dict(torque_delay=td, drive_filter=df, joint_x=jx, joint_y=jy)
+
+    def set_actuator_state(self, torque_delay=None, drive_filter=None, joint_x=None, joint_y=None, mask=None):
+        """writes the parts given (shapes as actuator_state(), or one environment's broadcast to all); mask [n]: only the selected environments change"""
+        L = self._act_lib()
+        td = self._arr(torque_delay, np.float64, (self.n, 10, 6))
+        df = self._arr(drive_filter, np.int32, (self.n, 10, 9))
+        jx = self._arr(joint_x, np.float64, (self.n, 6, 4))
+        jy = self._arr(joint_y, np.float64, (self.n, 6, 3))
+        m = self._arr(mask, np.uint8, (self.n,))
+        ptr = lambda a, t: None if a is None else a.ctypes.data_as(C.POINTER(t))
+        if L.cassie_batch_set_actuator_state(self.h, ptr(td, C.c_double), ptr(df, C.c_int), ptr(jx, C.c_double), ptr(jy, C.c_double),
+                                             None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
     def set_hfield_size(self, size):
         """the shared height-field size [4]; every environment's position and size go back to the shared ones, terrain selections stay"""
         a = np.ascontiguousarray(np.asarray(size, dtype=np.float64).reshape(4))
@@ -800,7 +875,8 @@ class CassieBatch:
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
         frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width],
-        terrain [n] int32: each environment's bank entry, read mod K at the next launch; set_env_hfield first).  set_frames /
+        terrain [n] int32: each environment's bank entry, read mod K at the next launch; set_env_hfield first; actuators [n, 40]: lo[10], hi[10], wmax[10]
+        in rad/s, delay[10], read at the next launch; set_env_actuators first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -810,7 +886,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field == 'terrain':
             ts = '<i4'
@@ -823,6 +899,16 @@ class CassieBatch:
         if field == 'terrain':
             return t.view(self.n)
         return t.view(self.n, *self._cam_hw) if field == 'depth' else t
+
+
+class joint_filter_t(C.Structure):
+    """the joint encoders' IIR filter state, as the C struct"""
+    _fields_ = [('x', C.c_double * 4), ('y', C.c_double * 3)]
+
+
+class drive_filter_t(C.Structure):
+    """the drive encoders' FIR taps: int x[9] as in the C struct (the reference's ctypes file declares doubles here)"""
+    _fields_ = [('x', C.c_int * 9)]
 
 
 class cassie_user_in_t(C.Structure):
@@ -1069,6 +1155,60 @@ class CassieSim:
             self.L.cassie_sim_set_body_mass(self.c, self._carr(data))
         else:
             self.L.cassie_sim_set_body_name_mass(self.c, name.encode(), float(data))
+
+    # ---- the controller-stage state (reference: example/cassiemujoco.py:132-161, 780-813)
+    def _act_lib(self):
+        L = self.L
+        if not getattr(L, '_sim_act_bound', False):
+            vp, dp, ip = C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int)
+            for n, a in (('cassie_sim_torque_delay', [vp, dp]), ('cassie_sim_set_torque_delay', [vp, dp]), ('cassie_sim_get_joint_filter', [vp, dp, dp]),
+                         ('cassie_sim_set_joint_filter', [vp, dp, dp]), ('cassie_sim_get_drive_filter', [vp, ip]), ('cassie_sim_set_drive_filter', [vp, ip])):
+                getattr(L, n).argtypes = a
+                getattr(L, n).restype = None
+            L.cassie_sim_joint_filter.argtypes = L.cassie_sim_drive_filter.argtypes = L.cassie_sim_ctrl.argtypes = [vp]
+            L.cassie_sim_joint_filter.restype = C.POINTER(joint_filter_t)
+            L.cassie_sim_drive_filter.restype = C.POINTER(drive_filter_t)
+            L.cassie_sim_ctrl.restype = dp
+            L._sim_act_bound = True
+        return L
+
+    def ctrl(self):
+        """the ctrl [nu] the last physics step applied"""
+        return self._act_lib().cassie_sim_ctrl(self.c)[:NU]
+
+    def set_ctrl(self, ctrl):
+        """writes through cassie_sim_ctrl, as the reference does; the next step overwrites it (the delay line's output is what is applied)"""
+        p = self._act_lib().cassie_sim_ctrl(self.c)
+        for i in range(NU):
+            p[i] = ctrl[i]
+
+    def get_joint_filter(self):
+        """a pointer to the joint_filter_t[6] mirror, indexable as an array of filters (writes are uploaded before the next step)"""
+        return self._act_lib().cassie_sim_joint_filter(self.c)
+
+    def set_joint_filter(self, x, y):
+        """x [6 * 4], y [6 * 3]"""
+        x_arr, y_arr = (C.c_double * 24)(*x), (C.c_double * 18)(*y)
+        self._act_lib().cassie_sim_set_joint_filter(self.c, C.cast(x_arr, C.POINTER(C.c_double)), C.cast(y_arr, C.POINTER(C.c_double)))
+
+    def get_drive_filter(self):
+        """a pointer to the drive_filter_t[10] mirror (int x[9] each), indexable as an array of filters"""
+        return self._act_lib().cassie_sim_drive_filter(self.c)
+
+    def set_drive_filter(self, x):
+        """x [10 * 9] integers"""
+        x_arr = (C.c_int * 90)(*[int(v) for v in x])
+        self._act_lib().cassie_sim_set_drive_filter(self.c, C.cast(x_arr, C.POINTER(C.c_int)))
+
+    def get_torque_delay(self):
+        """the torque delay line [10, 6] (motor by delay slot, slot 0 newest)"""
+        t = (C.c_double * 60)()
+        self._act_lib().cassie_sim_torque_delay(self.c, t)
+        return np.array(t[:]).reshape((10, 6))
+
+    def set_torque_delay(self, data):
+        t = (C.c_double * 60)(*np.asarray(data, dtype=np.float64).flatten())
+        self._act_lib().cassie_sim_set_torque_delay(self.c, C.cast(t, C.POINTER(C.c_double)))
 
     def set_body_pos(self, name, data):
         """moves the body in its parent frame from the next step on (reference: example/cassiemujoco.py:563-570); call set_const for the

@@ -34,6 +34,11 @@ TERRAIN_INSTANCES = [('f02f', 'float', 0, 47), ('f12f', 'float', 1, 47), ('f22f'
 # d117, f11f / d11f, f13f / d13f) by F_BP only; tag = precision, kind, features in hex
 BODY_POS_INSTANCES = [('f144', 'float', 1, 68), ('f157', 'float', 1, 87), ('d157', 'double', 1, 87), ('f15f', 'float', 1, 95), ('d15f', 'double', 1, 95),
                       ('f17f', 'float', 1, 127), ('d17f', 'double', 1, 127)]
+# the extended kernel with per-environment actuators (feature 128 = F_AC; cassie_batch_set_env_actuators), always with body-offset rows (a batch with
+# actuator rows carries offset rows holding the model's values when it has no others): each is the F_AC twin of one BODY_POS_INSTANCES entry (f144,
+# f157 / d157, f15f / d15f, f17f / d17f); tag = precision, kind, features in hex
+ACTUATOR_INSTANCES = [('f1c4', 'float', 1, 196), ('f1d7', 'float', 1, 215), ('d1d7', 'double', 1, 215), ('f1df', 'float', 1, 223), ('d1df', 'double', 1, 223),
+                      ('f1ff', 'float', 1, 255), ('d1ff', 'double', 1, 255)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -67,7 +72,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

@@ -33,6 +33,7 @@ CASSIE_STEP_ENTRY(d0f) CASSIE_STEP_ENTRY(d1f) CASSIE_STEP_ENTRY(d2f)
 CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_STEP_ENTRY(f11c) CASSIE_STEP_ENTRY(f11f) CASSIE_STEP_ENTRY(d11f)
 CASSIE_STEP_ENTRY(f02f) CASSIE_STEP_ENTRY(f12f) CASSIE_STEP_ENTRY(f22f) CASSIE_STEP_ENTRY(d02f) CASSIE_STEP_ENTRY(d12f) CASSIE_STEP_ENTRY(d22f) CASSIE_STEP_ENTRY(f13f) CASSIE_STEP_ENTRY(d13f)
 CASSIE_STEP_ENTRY(f144) CASSIE_STEP_ENTRY(f157) CASSIE_STEP_ENTRY(d157) CASSIE_STEP_ENTRY(f15f) CASSIE_STEP_ENTRY(d15f) CASSIE_STEP_ENTRY(f17f) CASSIE_STEP_ENTRY(d17f)
+CASSIE_STEP_ENTRY(f1c4) CASSIE_STEP_ENTRY(f1d7) CASSIE_STEP_ENTRY(d1d7) CASSIE_STEP_ENTRY(f1df) CASSIE_STEP_ENTRY(d1df) CASSIE_STEP_ENTRY(f1ff) CASSIE_STEP_ENTRY(d1ff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -42,6 +43,15 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_AC) {   // per-environment actuators: the F_AC twins of the F_BP instances, by the same rule (a batch with actuator rows always has offset rows)
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC; return dbl ? cassie_step_entry_d1ff() : cassie_step_entry_f1ff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC; return dbl ? cassie_step_entry_d1df() : cassie_step_entry_f1df(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC; return cassie_step_entry_f1c4(); }   // no frame / acceleration / dynamics / Jacobian launch
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC;
+    return dbl ? cassie_step_entry_d1d7() : cassie_step_entry_f1d7();
+  }
   if (feat & F_BP) {   // per-environment body offsets: extended instances only (a batch with offset rows always has constant rows)
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value;
@@ -306,6 +316,15 @@ struct BatchBase {
   virtual bool set_env_body_pos(const double *pos, const unsigned char *mask) = 0;
   virtual bool get_env_body_pos(double *pos) = 0;
   virtual bool clear_env_body_pos() = 0;
+  // per-environment actuators (F_AC instances): ctrlrange [n][nu][2], rpm [n][nu], delay [n][nu], each may be null (kept); only masked environments
+  // change; checked as a whole before anything changes
+  virtual bool set_env_actuators(const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) = 0;
+  virtual bool get_env_actuators(double *ctrlrange, double *rpm, int *delay) = 0;
+  virtual bool clear_env_actuators() = 0;
+  // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
+  // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
+  virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
+  virtual bool set_actuator_state(const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) = 0;
   virtual bool set_frames(const char *const *names, const int *kinds, int count) = 0;   // frame rows [n][count][FRAME_W]; count 0: none
   virtual bool frame_jacobian(int frame, double *jacp, double *jacr) = 0;                 // [n][3][nv] each at the current state (launch mode 4); jacr may be null
   virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
@@ -353,9 +372,12 @@ template <typename real> struct Batch : BatchBase {
   real *d_bpos = nullptr;                  // A.bpos: [n][BP_W] per-environment body offsets, allocated by the first cassie_batch_set_env_body_pos (F_BP instances)
   std::vector<double> bp_host;             // [n][nbody][3] the offsets every environment sees while d_bpos exists (in double: what get returns)
   bool bp_cenv = false;                    // the constant rows were allocated by the body-offset setter, and no model-row setter has written them since
+  real *d_act = nullptr;                   // A.act: [n][ACT_W] per-environment actuators, allocated by the first cassie_batch_set_env_actuators (F_AC instances)
+  std::vector<double> ac_host;             // [n][nu][4] lo, hi, rpm, delay every environment sees while d_act exists (in double: what get returns)
+  bool ac_bpos = false;                    // the offset rows were allocated by the actuator setter (model values), and no body-offset call has written them since
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -423,7 +445,9 @@ template <typename real> struct Batch : BatchBase {
           CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
           if (ext == 1) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR | F_FR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }
         if (ext == 1)   // per-environment body offsets: every instance step_entry routes F_BP launches to (the extended scratch)
-          for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+          for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) {   // and their F_AC twins (per-environment actuators)
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -775,6 +799,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     hm = src->hm;
     if (!rebuild_model()) return false;
+    if (!src->d_act && !clear_env_actuators()) return false;   // likewise the actuator rows and the offset rows their setter allocated
     if (!src->d_bpos && !clear_env_body_pos()) return false;   // before the constant rows are copied: clearing drops rows the offset setter allocated
     if (src->A.cenv) { if (!ensure_cenv()) return false; CUDA_OK(cudaMemcpyAsync(A.cenv, src->A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToDevice, stream)); }
     else if (A.cenv) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; }
@@ -788,6 +813,13 @@ template <typename real> struct Batch : BatchBase {
       hf_host = src->hf_host;
     }
     if (src->d_bpos) { bp_host = src->bp_host; bp_cenv = src->bp_cenv; if (!put_bpos()) return false; }   // the source's constant rows came above
+    if (src->d_act) {   // the rows as the source's environments run with them (its offset rows came just now)
+      ac_host = src->ac_host; ac_bpos = src->ac_bpos;
+      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
+      if (!d_act) CUDA_OK(cudaMalloc(&d_act, sizeof(real) * n * ACT_W));
+      CUDA_OK(cudaMemcpy(d_act, src->d_act, sizeof(real) * n * ACT_W, cudaMemcpyDeviceToDevice));
+      A.act = d_act;
+    }
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
       std::vector<float> tmp(cells); CUDA_OK(cudaMemcpy(tmp.data(), src->d_hfield, sizeof(float) * cells, cudaMemcpyDeviceToHost));
@@ -977,6 +1009,7 @@ template <typename real> struct Batch : BatchBase {
     if (!ensure_cenv()) return false;   // mode 3 (set_const) writes the environment's invweights into its constant row
     if (bp_host.empty()) { bp_host.resize((size_t)n * nb3); for (int e = 0; e < n; e++) memcpy(&bp_host[(size_t)e * nb3], hm.body_pos.data(), sizeof(double) * nb3); }
     for (int e = 0; e < n; e++) if (!mask || mask[e]) memcpy(&bp_host[(size_t)e * nb3], pos + (size_t)e * nb3, sizeof(double) * nb3);
+    ac_bpos = false;   // the rows are the caller's now, also when the actuator setter allocated them
     return put_bpos();
   }
   bool get_env_body_pos(double *pos) override {
@@ -986,14 +1019,143 @@ template <typename real> struct Batch : BatchBase {
     return true;
   }
   // back to the model's offsets and the instances that ran before: the block's robot_reach is the model's again, and constant rows the setter
-  // allocated (and no model-row setter wrote since) are dropped
+  // allocated (and no model-row setter wrote since) are dropped.  A batch with actuator rows keeps offset rows, holding the model's values again.
   bool clear_env_body_pos() override {
+    if (d_act) { model_bpos_rows(); ac_bpos = true; return put_bpos(); }
     bp_host.clear();
     if (!d_bpos) return true;
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaFree(d_bpos)); d_bpos = nullptr; A.bpos = nullptr;
     if (bp_cenv) { CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; bp_cenv = false; }
     return rebuild_model();
+  }
+  void model_bpos_rows() {   // the mirror of offset rows holding the model's offsets in every environment
+    const int nb3 = 3 * hm.nbody;
+    bp_host.resize((size_t)n * nb3); for (int e = 0; e < n; e++) memcpy(&bp_host[(size_t)e * nb3], hm.body_pos.data(), sizeof(double) * nb3);
+  }
+  // ---- per-environment actuators (actuator latency and torque saturation: sim-to-real randomisation): ctrlrange, no-load speed and torque delay per
+  // motor, read by the F_AC instances' motor stage and actuation.  Those instances are the F_AC twins of the F_BP ones, so a batch with actuator rows
+  // carries offset rows too: when it has none, the actuator setter allocates them holding the model's values (and constant rows with them, as the
+  // offset setter does); clear drops them again unless a body-offset call has written them since.
+  // The device rows are what the environments run with: a caller may have written them through the "actuators" device pointer.  The mirror keeps
+  // the doubles the verb was last given, so that get reports them exactly (rpm included) wherever the device still holds what they stored.
+  static real act_row_value(const double *a, int f) { return f == 2 ? (real)(a[2] * 2 * M_PI / 60) : (real)a[f]; }   // wmax: build_dev_model's expression
+  static int act_delay_host(real v) { return (int)(v > real(0) ? (v < real(AC_MAXDELAY) ? v : real(AC_MAXDELAY)) : real(0)); }   // the kernel's act_delay_index
+  static constexpr int AC_FIELD[4] = {AC_LO, AC_HI, AC_WMAX, AC_DELAY};
+  bool pull_act(std::vector<real> &all) {   // the device rows (zero without rows)
+    all.assign((size_t)n * ACT_W, real(0));
+    if (!d_act) return true;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemcpyAsync(all.data(), d_act, sizeof(real) * n * ACT_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  bool push_act(const std::vector<real> &all) {
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    if (!d_act) CUDA_OK(cudaMalloc(&d_act, sizeof(real) * n * ACT_W));
+    CUDA_OK(cudaMemcpy(d_act, all.data(), sizeof(real) * n * ACT_W, cudaMemcpyHostToDevice));
+    A.act = d_act;
+    return true;
+  }
+  void model_act(int i, double *a) const {   // motor i as the model has it: lo, hi (the clamp the block holds), rpm, the reference's delay
+    a[0] = (double)h_model_copy.act_ctrl_lo[i]; a[1] = (double)h_model_copy.act_ctrl_hi[i]; a[2] = hm.actuator_user[i]; a[3] = AC_MAXDELAY;
+  }
+  bool set_env_actuators(const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) override {
+    const std::string verb = "cassie_batch_set_env_actuators";
+    const int nu = hm.nu;
+    if (nu > MU) { set_err(verb + ": the model has more than " + std::to_string(MU) + " actuators"); return false; }
+    const std::string why = env_actuators_check(n, nu, ctrlrange, rpm, delay, mask);   // every masked value is checked before anything changes
+    if (!why.empty()) { set_err(verb + ": " + why); return false; }
+    if (!d_bpos) {   // the F_AC instances read offset rows: the model's values, dropped again by clear unless a body-offset call writes them
+      if (!A.cenv) bp_cenv = true;
+      if (!ensure_cenv()) return false;
+      model_bpos_rows();
+      if (!put_bpos()) return false;
+      ac_bpos = true;
+    }
+    std::vector<real> all;
+    if (!d_act) {   // the first call: every environment starts from the model's actuators
+      ac_host.resize((size_t)n * nu * 4); all.assign((size_t)n * ACT_W, real(0));
+      for (int e = 0; e < n; e++) for (int i = 0; i < nu; i++) {
+        double *a = &ac_host[((size_t)e * nu + i) * 4]; model_act(i, a);
+        for (int f = 0; f < 4; f++) all[(size_t)e * ACT_W + AC_FIELD[f] + i] = act_row_value(a, f);
+      }
+    } else if (!pull_act(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      for (int i = 0; i < nu; i++) {
+        const size_t k = (size_t)e * nu + i; double *a = &ac_host[k * 4]; real *r = &all[(size_t)e * ACT_W];
+        if (ctrlrange) { a[0] = ctrlrange[2 * k]; a[1] = ctrlrange[2 * k + 1]; r[AC_LO + i] = act_row_value(a, 0); r[AC_HI + i] = act_row_value(a, 1); }
+        if (rpm) { a[2] = rpm[k]; r[AC_WMAX + i] = act_row_value(a, 2); }
+        if (delay) { a[3] = delay[k]; r[AC_DELAY + i] = act_row_value(a, 3); }
+      }
+    }
+    return push_act(all);
+  }
+  // what every environment runs with: a value the device row still holds as the verb stored it is reported as the verb was given it; one written on the
+  // device is reported from the row (rpm = wmax * 60 / 2 pi, the delay as the kernel reads it)
+  bool get_env_actuators(double *ctrlrange, double *rpm, int *delay) override {
+    const int nu = hm.nu;
+    std::vector<real> all;
+    if (!pull_act(all)) return false;
+    for (int e = 0; e < n; e++) for (int i = 0; i < nu; i++) {
+      const size_t k = (size_t)e * nu + i;
+      double m[4]; model_act(i, m);
+      double v[4] = {m[0], m[1], m[2], m[3]};
+      if (d_act) {
+        const double *a = &ac_host[k * 4];
+        for (int f = 0; f < 4; f++) {
+          const real dv = all[(size_t)e * ACT_W + AC_FIELD[f] + i];
+          if (dv == act_row_value(a, f)) v[f] = a[f];
+          else v[f] = f == 2 ? (double)dv * 60 / (2 * M_PI) : (f == 3 ? (double)act_delay_host(dv) : (double)dv);
+        }
+      }
+      if (ctrlrange) { ctrlrange[2 * k] = v[0]; ctrlrange[2 * k + 1] = v[1]; }
+      if (rpm) rpm[k] = v[2];
+      if (delay) delay[k] = (int)v[3];
+    }
+    return true;
+  }
+  bool clear_env_actuators() override {
+    ac_host.clear();
+    if (!d_act) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_act)); d_act = nullptr; A.act = nullptr;
+    if (ac_bpos) { ac_bpos = false; return clear_env_body_pos(); }   // (which drops the constant rows too when the offset rows brought them)
+    return true;
+  }
+  // ---- the controller-stage state: the delay line, the encoders' filters (views of the cst / dfilt rows; snapshots carry them)
+  bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) override {
+    CUDA_OK(cudaSetDevice(device));
+    std::vector<real> cst; std::vector<int> df;   // only the rows asked for are downloaded
+    if (torque_delay || joint_x || joint_y) { cst.resize((size_t)n * CST_W); CUDA_OK(cudaMemcpyAsync(cst.data(), A.cst, sizeof(real) * n * CST_W, cudaMemcpyDeviceToHost, stream)); }
+    if (drive_filter) { df.resize((size_t)n * DFILT_W); CUDA_OK(cudaMemcpyAsync(df.data(), A.dfilt, sizeof(int) * n * DFILT_W, cudaMemcpyDeviceToHost, stream)); }
+    CUDA_OK(cudaStreamSynchronize(stream));
+    for (int e = 0; e < n; e++) {
+      const real *c = cst.empty() ? nullptr : &cst[(size_t)e * CST_W];
+      if (torque_delay) for (int i = 0; i < 60; i++) torque_delay[(size_t)e * 60 + i] = (double)c[CS_DELAY + i];
+      if (joint_x) for (int i = 0; i < 24; i++) joint_x[(size_t)e * 24 + i] = (double)c[CS_JFX + i];
+      if (joint_y) for (int i = 0; i < 18; i++) joint_y[(size_t)e * 18 + i] = (double)c[CS_JFY + i];
+      if (drive_filter) memcpy(drive_filter + (size_t)e * 90, &df[(size_t)e * DFILT_W], sizeof(int) * 90);
+    }
+    return true;
+  }
+  bool set_actuator_state(const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) override {
+    CUDA_OK(cudaSetDevice(device));
+    std::vector<real> cst((size_t)n * CST_W); std::vector<int> df((size_t)n * DFILT_W);
+    CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaMemcpy(cst.data(), A.cst, sizeof(real) * n * CST_W, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(df.data(), A.dfilt, sizeof(int) * n * DFILT_W, cudaMemcpyDeviceToHost));
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      real *c = &cst[(size_t)e * CST_W];
+      if (torque_delay) for (int i = 0; i < 60; i++) c[CS_DELAY + i] = (real)torque_delay[(size_t)e * 60 + i];
+      if (joint_x) for (int i = 0; i < 24; i++) c[CS_JFX + i] = (real)joint_x[(size_t)e * 24 + i];
+      if (joint_y) for (int i = 0; i < 18; i++) c[CS_JFY + i] = (real)joint_y[(size_t)e * 18 + i];
+      if (drive_filter) memcpy(&df[(size_t)e * DFILT_W], drive_filter + (size_t)e * 90, sizeof(int) * 90);
+    }
+    if (torque_delay || joint_x || joint_y) CUDA_OK(cudaMemcpy(A.cst, cst.data(), sizeof(real) * n * CST_W, cudaMemcpyHostToDevice));
+    if (drive_filter) CUDA_OK(cudaMemcpy(A.dfilt, df.data(), sizeof(int) * n * DFILT_W, cudaMemcpyHostToDevice));
+    return true;
   }
   // ---- frame rows: the table is checked as a whole before anything changes; the rows start at zero and are filled by the next step / forward launch
   bool set_frames(const char *const *names, const int *kinds, int count) override {
@@ -1166,7 +1328,7 @@ template <typename real> struct Batch : BatchBase {
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1234,7 +1396,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -1275,11 +1437,16 @@ struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[6
   // the height field's size (cassie_sim_get_hfield_size / set_hfield_size): a host mirror, uploaded before the next launch when it is valid
   double hf_size[4] = {0, 0, 0, 0}, hf_size_dev[4] = {0, 0, 0, 0};
   // body offsets (cassie_sim_get_body_name_pos / set_body_name_pos): [nbody][3] host mirror; the constant block is rebuilt from it when it changes
-  std::vector<double> m_bpos, m_bpos_dev; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
+  std::vector<double> m_bpos, m_bpos_dev;
+  // the controller-stage state lent out by cassie_sim_joint_filter / drive_filter / ctrl: host mirrors laid out as joint_filter_t[6] (x[4], y[3]),
+  // drive_filter_t[10] (int x[9]) and mjData's ctrl[nu].  Refreshed after every launch once one was lent; the filter mirrors are uploaded before the
+  // next launch when they were written, ctrl is read-only in effect (the next step overwrites it, as cassie_motor_data does in the reference)
+  double jfilt[6][7], jfilt_dev[6][7], ctrl[MU]; int dfilt[10][9], dfilt_dev[10][9]; bool act_lent = false, ctrl_zero = false; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
 
 // cassie_state_t (include/cassiemujoco.h:434-463): a device-resident snapshot of one simulator's rows plus the host mirrors the reference hands out as
 // borrowed pointers (time, qpos, qvel); the snapshot is allocated by the first cassie_get_state, which also fixes the owning simulator's sizes
-struct cassie_state { cassie::Snap *snap = nullptr; double qpos[64], qvel[64], time = 0, qpos_snap[64], qvel_snap[64], time_snap = 0; };
+struct cassie_state { cassie::Snap *snap = nullptr; double qpos[64], qvel[64], time = 0, qpos_snap[64], qvel_snap[64], time_snap = 0;
+  bool ctrl_zero = false; };   // the simulator's ctrl read zeros when the snapshot was taken (after cassie_sim_full_reset, before a step)
 
 static std::mutex g_model_mutex;
 static std::string g_model_path;   // what cassie_mujoco_init cached (the reference caches the parsed model, src/cassiemujoco.c:48-59)
@@ -1313,7 +1480,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
-  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1;
+  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -1391,6 +1558,16 @@ bool cassie_mujoco_init(const char *modelfile) {
   g_model_path = modelfile; return true;
 }
 void cassie_cleanup(void) { std::lock_guard<std::mutex> g(g_model_mutex); g_model_path.clear(); }
+static void sim_pull_act(cassie_sim_t *c) {   // the controller-stage mirrors, once lent out; a filter mirror written and not yet uploaded is kept
+  double cst[CST_W]; int df[90];   // one download of the controller row (joint filters, drive torques) and one of the FIR taps
+  if (!c->b->impl->get("cst", cst) || !c->b->impl->get_actuator_state(nullptr, df, nullptr, nullptr)) return;
+  if (!memcmp(c->jfilt, c->jfilt_dev, sizeof c->jfilt)) {
+    for (int j = 0; j < 6; j++) { for (int k = 0; k < 4; k++) c->jfilt[j][k] = cst[CS_JFX + 4 * j + k]; for (int k = 0; k < 3; k++) c->jfilt[j][4 + k] = cst[CS_JFY + 3 * j + k]; }
+    memcpy(c->jfilt_dev, c->jfilt, sizeof c->jfilt); }
+  if (!memcmp(c->dfilt, c->dfilt_dev, sizeof c->dfilt)) { memcpy(c->dfilt, df, sizeof c->dfilt); memcpy(c->dfilt_dev, c->dfilt, sizeof c->dfilt); }
+  const HostModel &hm = c->b->impl->hm;   // the ctrl the last physics step applied: the drive torque over the gear (src/cassiemujoco.c:660-662)
+  for (int i = 0; i < hm.nu && i < MU; i++) c->ctrl[i] = c->ctrl_zero ? 0.0 : cst[CS_DTORQUE + i] / hm.actuator_gear[i];
+}
 static void sim_pull(cassie_sim_t *c) {
   c->b->impl->get("qpos", c->qpos); c->b->impl->get("qvel", c->qvel); c->b->impl->get("time", &c->time); if (c->b->impl->has_aux()) c->b->impl->get("aux", c->aux);
   if (!c->frames.empty() && c->b->impl->get("frames", c->frames.data())) {   // the sizes were fixed at init: the borrowed pointers stay valid
@@ -1400,7 +1577,9 @@ static void sim_pull(cassie_sim_t *c) {
   }
   if (!c->acc.empty() && c->b->impl->get("acc", c->acc.data())) for (int i = 0; i < c->b->impl->hm.nv; i++) c->qacc[i] = c->acc[AC_QACC + i];
   memcpy(c->qpos_dev, c->qpos, sizeof c->qpos); memcpy(c->qvel_dev, c->qvel, sizeof c->qvel); c->time_dev = c->time;
+  if (c->act_lent) sim_pull_act(c);
 }
+static void sim_lend_act(cassie_sim_t *c) { if (!c->act_lent) { c->act_lent = true; sim_pull_act(c); } }   // the first lend fills the mirrors
 static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote through the borrowed pointers
   if (memcmp(c->qpos_dev, c->qpos, sizeof c->qpos)) c->b->impl->set("qpos", c->qpos);
   if (memcmp(c->qvel_dev, c->qvel, sizeof c->qvel)) c->b->impl->set("qvel", c->qvel);
@@ -1418,6 +1597,12 @@ static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote thr
     c->b->impl->rebuild_model(); c->m_gpos_dev = c->m_gpos; c->m_gquat_dev = c->m_gquat; c->m_gsize_dev = c->m_gsize; }
   if (c->m_bpos != c->m_bpos_dev) {   // a body was moved (src/cassiemujoco.c:1408-1418): kinematics, static geoms' world poses and the broad phase's bound follow
     c->b->impl->hm.body_pos = c->m_bpos; c->b->impl->rebuild_model(); c->m_bpos_dev = c->m_bpos; }
+  if (c->act_lent && memcmp(c->jfilt, c->jfilt_dev, sizeof c->jfilt)) {   // written through cassie_sim_joint_filter (src/cassiemujoco.c:2119-2121)
+    double jx[24], jy[18];
+    for (int j = 0; j < 6; j++) { for (int k = 0; k < 4; k++) jx[4 * j + k] = c->jfilt[j][k]; for (int k = 0; k < 3; k++) jy[3 * j + k] = c->jfilt[j][4 + k]; }
+    c->b->impl->set_actuator_state(nullptr, nullptr, jx, jy, nullptr); memcpy(c->jfilt_dev, c->jfilt, sizeof c->jfilt); }
+  if (c->act_lent && memcmp(c->dfilt, c->dfilt_dev, sizeof c->dfilt)) {   // written through cassie_sim_drive_filter (:2151-2153)
+    c->b->impl->set_actuator_state(nullptr, &c->dfilt[0][0], nullptr, nullptr, nullptr); memcpy(c->dfilt_dev, c->dfilt, sizeof c->dfilt); }
 }
 cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   std::string path;
@@ -1444,8 +1629,10 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
                              for (int k = 0; k < 4; k++) c->hf_size[k] = c->hf_size_dev[k] = b->impl->hm.hfield_size[k]; }
   return c;
 }
+// the one-environment batch a simulator steps: batch verbs (per-environment rows, device pointers) apply to it; owned by the simulator
+cassie_batch_t *cassie_sim_batch(cassie_sim_t *c) { return c ? c->b : nullptr; }
 void cassie_sim_free(cassie_sim_t *c) { if (!c) return; cassie_batch_free(c->b); delete c; }
-void cassie_sim_step_pd(cassie_sim_t *c, state_out_t *y, const pd_in_t *u) { sim_push(c); cassie_sim_step_pd_batch(c->b, u, y); sim_pull(c); }
+void cassie_sim_step_pd(cassie_sim_t *c, state_out_t *y, const pd_in_t *u) { sim_push(c); cassie_sim_step_pd_batch(c->b, u, y); c->ctrl_zero = false; sim_pull(c); }
 double *cassie_sim_time(cassie_sim_t *c) { return &c->time; }
 double *cassie_sim_qpos(cassie_sim_t *c) { return c->qpos; }
 double *cassie_sim_qvel(cassie_sim_t *c) { return c->qvel; }
@@ -1628,6 +1815,19 @@ void cassie_sim_set_body_name_pos(cassie_sim_t *c, const char *name, double *dat
   double *p = cassie_sim_get_body_name_pos(c, name);
   if (p && data) for (int k = 0; k < 3; k++) p[k] = data[k];
 }
+// src/cassiemujoco.c:2114-2192: the delay line and the encoders' filters, read and written through the simulator's batch (pending writes through
+// the borrowed mirrors go first)
+void cassie_sim_torque_delay(cassie_sim_t *c, double *t) { sim_push(c); c->b->impl->get_actuator_state(t, nullptr, nullptr, nullptr); }
+void cassie_sim_set_torque_delay(cassie_sim_t *c, double *t) { sim_push(c); c->b->impl->set_actuator_state(t, nullptr, nullptr, nullptr, nullptr); }
+void cassie_sim_get_joint_filter(cassie_sim_t *c, double *x, double *y) { sim_push(c); c->b->impl->get_actuator_state(nullptr, nullptr, x, y); }
+void cassie_sim_set_joint_filter(cassie_sim_t *c, double *x, double *y) { sim_push(c); c->b->impl->set_actuator_state(nullptr, nullptr, x, y, nullptr); if (c->act_lent) sim_pull_act(c); }
+void cassie_sim_get_drive_filter(cassie_sim_t *c, int *x) { sim_push(c); c->b->impl->get_actuator_state(nullptr, x, nullptr, nullptr); }
+void cassie_sim_set_drive_filter(cassie_sim_t *c, int *x) { sim_push(c); c->b->impl->set_actuator_state(nullptr, x, nullptr, nullptr, nullptr); if (c->act_lent) sim_pull_act(c); }
+void *cassie_sim_joint_filter(cassie_sim_t *c) { sim_lend_act(c); return &c->jfilt[0][0]; }   // joint_filter_t[6]
+void *cassie_sim_drive_filter(cassie_sim_t *c) { sim_lend_act(c); return &c->dfilt[0][0]; }   // drive_filter_t[10]
+// :1237: mjData's ctrl as the last physics step applied it; writes through the pointer have no effect (cassie_motor_data overwrites d->ctrl before
+// mj_step in the reference); zeros after cassie_sim_full_reset until the next step
+double *cassie_sim_ctrl(cassie_sim_t *c) { sim_lend_act(c); return c->ctrl; }
 int cassie_sim_get_joint_num_dof(cassie_sim_t *c, const char *name) { const HostModel &hm = c->b->impl->hm; const int j = hm.joint_id(name ? name : ""); if (j < 0) return 0; return hm.jnt_type[j] == JNT_FREE ? 6 : (hm.jnt_type[j] == JNT_BALL ? 3 : 1); }
 void cassie_sim_set_dof_name_damping(cassie_sim_t *c, const char *name, double *damp) { const HostModel &hm = c->b->impl->hm; const int j = hm.joint_id(name ? name : ""); if (j < 0) return; const int nd = cassie_sim_get_joint_num_dof(c, name); for (int i = 0; i < nd; i++) c->m_damp[hm.jnt_dofadr[j] + i] = damp[i]; }
 double *cassie_sim_get_dof_name_damping(cassie_sim_t *c, const char *name) { const HostModel &hm = c->b->impl->hm; const int j = hm.joint_id(name ? name : ""); return j >= 0 ? &c->m_damp[hm.jnt_dofadr[j]] : nullptr; }
@@ -1652,6 +1852,7 @@ void cassie_sim_full_reset(cassie_sim_t *c) {
     c->b->impl->set("acc", row.data());
   }
   c->b->impl->reset_estimator(nullptr); c->b->impl->reset_estimator_device(nullptr);   // state_output_setup (src/cassiemujoco.c:2032) restarts the estimator's filters
+  c->ctrl_zero = true;   // ctrl <- 0 (:2024) until the next step applies one
   sim_pull(c);
 }
 // sizes the reference's Python wrapper asks for (src/cassiemujoco.c:1038-1060)
@@ -1702,6 +1903,13 @@ int cassie_batch_clear_env_hfield(cassie_batch_t *b) { return b->impl->clear_env
 int cassie_batch_set_env_body_pos(cassie_batch_t *b, const double *pos, const unsigned char *mask) { return b->impl->set_env_body_pos(pos, mask) ? 0 : -1; }
 int cassie_batch_get_env_body_pos(cassie_batch_t *b, double *pos) { return b->impl->get_env_body_pos(pos) ? 0 : -1; }
 int cassie_batch_clear_env_body_pos(cassie_batch_t *b) { return b->impl->clear_env_body_pos() ? 0 : -1; }
+// per-environment actuators and the controller-stage state; see include/cassie_b200.h
+int cassie_batch_set_env_actuators(cassie_batch_t *b, const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) { return b->impl->set_env_actuators(ctrlrange, rpm, delay, mask) ? 0 : -1; }
+int cassie_batch_get_env_actuators(cassie_batch_t *b, double *ctrlrange, double *rpm, int *delay) { return b->impl->get_env_actuators(ctrlrange, rpm, delay) ? 0 : -1; }
+int cassie_batch_clear_env_actuators(cassie_batch_t *b) { return b->impl->clear_env_actuators() ? 0 : -1; }
+int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) { return b->impl->get_actuator_state(torque_delay, drive_filter, joint_x, joint_y) ? 0 : -1; }
+int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) {
+  return b->impl->set_actuator_state(torque_delay, drive_filter, joint_x, joint_y, mask) ? 0 : -1; }
 int cassie_batch_set_hfield_size(cassie_batch_t *b, const double size[4]) { return b->impl->set_hfield_size(size) ? 0 : -1; }
 int cassie_batch_get_hfield_size(const cassie_batch_t *b, double size[4]) {
   const HostModel &hm = b->impl->hm;
@@ -1774,11 +1982,11 @@ cassie_out_t cassie_sim_get_cassie_out(cassie_sim_t *c) { double o[OBS_W]; cassi
 void cassie_sim_step(cassie_sim_t *c, cassie_out_t *y, const cassie_user_in_t *u) {
   pd_in_t pd; memset(&pd, 0, sizeof pd);
   for (int i = 0; i < 5; i++) { pd.leftLeg.motorPd.torque[i] = u->torque[i]; pd.rightLeg.motorPd.torque[i] = u->torque[5 + i]; }
-  state_out_t so; sim_push(c); cassie_sim_step_pd_batch(c->b, &pd, &so); sim_pull(c);
+  state_out_t so; sim_push(c); cassie_sim_step_pd_batch(c->b, &pd, &so); c->ctrl_zero = false; sim_pull(c);
   if (y) *y = cassie_sim_get_cassie_out(c);
 }
 // :1159-1181: the same tick with ONE physics step whatever the model's timestep is
-void cassie_sim_step_pd_no2khz(cassie_sim_t *c, state_out_t *y, const pd_in_t *u) { sim_push(c); c->b->impl->nsub_override = 1; cassie_sim_step_pd_batch(c->b, u, y); c->b->impl->nsub_override = 0; sim_pull(c); }
+void cassie_sim_step_pd_no2khz(cassie_sim_t *c, state_out_t *y, const pd_in_t *u) { sim_push(c); c->b->impl->nsub_override = 1; cassie_sim_step_pd_batch(c->b, u, y); c->b->impl->nsub_override = 0; c->ctrl_zero = false; sim_pull(c); }
 // :1196-1204: the borrowed pointer is a host mirror, uploaded (constant block rebuilt) before the next launch
 double *cassie_sim_timestep(cassie_sim_t *c) { return &c->timestep; }
 void cassie_sim_set_timestep(cassie_sim_t *c, double dt) { c->timestep = dt; }
@@ -1806,11 +2014,13 @@ void cassie_get_state(const cassie_sim_t *cc, cassie_state_t *s) {
   if (!s->snap) { s->snap = impl->snap_alloc(); if (!s->snap) return; }
   impl->snap_get(s->snap);
   memcpy(s->qpos, c->qpos, sizeof s->qpos); memcpy(s->qvel, c->qvel, sizeof s->qvel); s->time = c->time;
-  memcpy(s->qpos_snap, s->qpos, sizeof s->qpos); memcpy(s->qvel_snap, s->qvel, sizeof s->qvel); s->time_snap = s->time;
+  memcpy(s->qpos_snap, s->qpos, sizeof s->qpos); memcpy(s->qvel_snap, s->qvel, sizeof s->qvel); s->time_snap = s->time; s->ctrl_zero = c->ctrl_zero;
 }
 void cassie_set_state(cassie_sim_t *c, const cassie_state_t *s) {
   if (!s->snap) { set_err("cassie_set_state: the state object holds no snapshot (cassie_get_state first)"); return; }
   if (!c->b->impl->snap_set(s->snap, nullptr)) return;   // any simulator of the same model accepts it
+  c->ctrl_zero = s->ctrl_zero;   // mjData's ctrl is part of the reference's state
+  memcpy(c->jfilt_dev, c->jfilt, sizeof c->jfilt); memcpy(c->dfilt_dev, c->dfilt, sizeof c->dfilt);   // the restored filters replace writes not yet uploaded
   sim_pull(c);
   // what the caller wrote through cassie_state_qpos / qvel / time after the snapshot was taken
   if (memcmp(s->qpos, s->qpos_snap, sizeof s->qpos)) memcpy(c->qpos, s->qpos, sizeof s->qpos);
@@ -1825,6 +2035,7 @@ void cassie_state_copy(cassie_state_t *dst, const cassie_state_t *src) {
   if (!snap_clone_into(dst->snap, src->snap)) { set_err("cassie_state_copy failed"); return; }
   memcpy(dst->qpos, src->qpos, sizeof dst->qpos); memcpy(dst->qvel, src->qvel, sizeof dst->qvel); dst->time = src->time;
   memcpy(dst->qpos_snap, src->qpos_snap, sizeof dst->qpos_snap); memcpy(dst->qvel_snap, src->qvel_snap, sizeof dst->qvel_snap); dst->time_snap = src->time_snap;
+  dst->ctrl_zero = src->ctrl_zero;
 }
 cassie_state_t *cassie_state_duplicate(const cassie_state_t *src) { cassie_state_t *s = cassie_state_alloc(); cassie_state_copy(s, src); return s; }
 // :1072-1093: model (per-environment constants, height field, timestep) and full dynamic state

@@ -103,6 +103,27 @@ inline std::string env_body_pos_check(const HostModel &m, int b, int xb) {
   return std::string();
 }
 
+// cassie_batch_set_env_actuators' check of every masked value, before anything changes: an empty reason, else the first refusal (a non-finite value,
+// lo >= hi, rpm <= 0, a delay outside 0..AC_MAXDELAY), naming the environment and the actuator.  ctrlrange [n][nu][2], rpm [n][nu], delay [n][nu]; null
+// parts are not checked (kept)
+inline std::string env_actuators_check(int n, int nu, const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) {
+  for (int e = 0; e < n; e++) {
+    if (mask && !mask[e]) continue;
+    for (int i = 0; i < nu; i++) {
+      const std::string at = "environment " + std::to_string(e) + ", actuator " + std::to_string(i) + ": ";
+      const size_t k = (size_t)e * nu + i;
+      if (ctrlrange) {
+        const double lo = ctrlrange[2 * k], hi = ctrlrange[2 * k + 1];
+        if (!std::isfinite(lo) || !std::isfinite(hi)) return at + "ctrlrange is not finite";
+        if (!(lo < hi)) return at + "ctrlrange needs lo < hi";
+      }
+      if (rpm && !(std::isfinite(rpm[k]) && rpm[k] > 0)) return at + "rpm must be finite and positive";
+      if (delay && (delay[k] < 0 || delay[k] > AC_MAXDELAY)) return at + "delay must be in 0.." + std::to_string(AC_MAXDELAY);
+    }
+  }
+  return std::string();
+}
+
 // one row of a batch's frame table (FT_W) for body (kind 0) or site (kind 1) `name`; its id, or -1 with a reason for an unknown name or kind
 template <typename real> int frame_table_row(const HostModel &m, const char *name, int kind, real *row, std::string &err) {
   for (int c = 0; c < FT_W; c++) row[c] = 0;

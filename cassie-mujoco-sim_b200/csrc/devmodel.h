@@ -35,6 +35,7 @@ constexpr int F_EG = 8;   // the static geoms' world poses, sizes and bounding r
 constexpr int F_FR = 16;  // frame rows (FRAME_W per named body / site) are filled in the last sub-step of a launch (extended instances only)
 constexpr int F_TR = 32;  // per-environment terrain: the bank entry from a selection row, the height field's size from its F_EG slot (with F_ALL | F_EG only)
 constexpr int F_BP = 64;  // per-environment body offsets: each body's position in its parent frame comes from a BP_W row instead of the model block (extended instances only)
+constexpr int F_AC = 128; // per-environment actuators: ctrlrange, no-load speed and torque delay of every motor come from an ACT_W row (with F_BP, extended instances only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -174,6 +175,12 @@ constexpr int GE_POSE = 0, GE_SIZE = 12, GE_RBOUND = 15;
 // per-environment body offsets (optional, cassie_batch_set_env_body_pos; F_BP instances): MuJoCo's body_pos of every body [MB][3] in model body order,
 // the rest of the row zero.  The kinematics, the ray and the camera kernels read it instead of DevModel::body_pos.  A model input like the CE rows.
 constexpr int BP_W = MB * 3;
+// per-environment actuators (optional, cassie_batch_set_env_actuators; F_AC instances): per motor i MuJoCo's actuator_ctrlrange (lo, hi) -- the
+// ctrllimited clamp of the actuation and motor()'s tmax --, the no-load speed wmax = actuator_user * 2 pi / 60 (rad/s) and the torque delay in control
+// ticks, stored as a real; the kernel reads it clamped to [0, 6] (NaN: 0) and truncated.  A model input like the CE rows.
+constexpr int ACT_W = 40;
+constexpr int AC_LO = 0, AC_HI = 10, AC_WMAX = 20, AC_DELAY = 30;
+constexpr int AC_MAXDELAY = 6;   // the length of the delay line (cst CS_DELAY [10][6]): the reference's TORQUE_DELAY_CYCLES
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

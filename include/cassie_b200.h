@@ -31,6 +31,9 @@ void cassie_cleanup(void);
 cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit);
 /* include/cassiemujoco.h:77  (src/cassiemujoco.c:1102-1113): NULL is a no-op */
 void cassie_sim_free(cassie_sim_t *sim);
+/* new: the one-environment batch a simulator steps, owned by it (not to be freed), so that the batch verbs -- per-environment rows such as
+ * cassie_batch_set_env_actuators, device pointers -- apply to a legacy simulator; cassie_sim_copy copies what they set. */
+cassie_batch_t *cassie_sim_batch(cassie_sim_t *c);
 /* include/cassiemujoco.h:95  (src/cassiemujoco.c:1147-1157): THE hot path, one environment, one 0.5 ms tick */
 void cassie_sim_step_pd(cassie_sim_t *sim, state_out_t *y, const pd_in_t *u);
 /* include/cassiemujoco.h:104,147,183 (src/cassiemujoco.c:1191-1214): borrowed read-write pointers (35 / 32 / 1 doubles) into a
@@ -342,6 +345,22 @@ double *cassie_sim_get_body_name_ipos(cassie_sim_t *c, const char *name);       
  * An unknown name: NULL / no change, and an error (the reference indexes -1). */
 void cassie_sim_set_body_name_pos(cassie_sim_t *c, const char *name, double *data);
 double *cassie_sim_get_body_name_pos(cassie_sim_t *c, const char *name);
+/* src/cassiemujoco.c:2114-2192: the torque delay line [10][6], the joint filters x [6][4] / y [6][3] and the drive filters [10][9], read and written
+ * through the simulator's batch.  cassie_sim_joint_filter / cassie_sim_drive_filter lend host mirrors laid out as joint_filter_t[6] {double x[4], y[3]}
+ * and drive_filter_t[10] {int x[9]} (the C structs; the reference's ctypes file declares double x[9] for the latter); a write through them is
+ * uploaded before the next launch, like the other borrowed pointers. */
+void cassie_sim_torque_delay(cassie_sim_t *c, double *t);
+void cassie_sim_set_torque_delay(cassie_sim_t *c, double *t);
+void cassie_sim_get_joint_filter(cassie_sim_t *c, double *x, double *y);
+void cassie_sim_set_joint_filter(cassie_sim_t *c, double *x, double *y);
+void cassie_sim_get_drive_filter(cassie_sim_t *c, int *x);
+void cassie_sim_set_drive_filter(cassie_sim_t *c, int *x);
+void *cassie_sim_joint_filter(cassie_sim_t *c);
+void *cassie_sim_drive_filter(cassie_sim_t *c);
+/* :1237: mjData's ctrl [nu] as the last physics step applied it (the drive torque over the gear: exact to 1 ulp).  Writes through the pointer have
+ * no effect on the next step, as in the reference, where cassie_motor_data overwrites d->ctrl before mj_step; zeros after cassie_sim_full_reset
+ * (:2024) until the next step. */
+double *cassie_sim_ctrl(cassie_sim_t *c);
 void cassie_sim_set_geom_friction(cassie_sim_t *c, double *fric);      /* :1420 */
 void cassie_sim_set_geom_name_friction(cassie_sim_t *c, const char *name, double *fric); /* :1427 (addresses the geom's own triple) */
 double *cassie_sim_get_geom_name_friction(cassie_sim_t *c, const char *name);            /* :1433 */
@@ -535,8 +554,37 @@ int cassie_batch_set_env_body_pos(cassie_batch_t *b, const double *pos, const un
 int cassie_batch_get_env_body_pos(cassie_batch_t *b, double *pos);
 int cassie_batch_clear_env_body_pos(cassie_batch_t *b);
 
+/* Per-environment actuators (domain randomisation of actuator latency and torque saturation): for motor i of each environment
+ *   ctrlrange [n][nu][2]: MuJoCo's actuator_ctrlrange (lo, hi), in both places the reference reads it -- the ctrllimited clamp of ctrl in the
+ *                         actuation and motor()'s tmax, the top of the torque-speed curve and the saturation (src/cassiemujoco.c:638-664);
+ *   rpm [n][nu]:          MuJoCo's actuator_user, the no-load speed in rpm (motor()'s wmax = rpm * 2 pi / 60);
+ *   delay [n][nu]:        the torque delay in control ticks, 0..6: the control applied at tick k is the motor's torque of tick k - delay (6 is the
+ *                         reference's TORQUE_DELAY_CYCLES, 0 applies this tick's torque).  All six slots of the delay line keep shifting whatever the
+ *                         delay, so a change takes effect at once with the history in place; a variable delay is this project's extension.
+ * Any of the three may be NULL (kept); mask [n] (or NULL: all) selects the environments that change.  The first call gives every environment the
+ * model's values (delay 6).  0, or -1 with nothing changed (cassie_b200_last_error names the environment and the motor) for a non-finite value,
+ * lo >= hi, rpm <= 0 or a delay outside 0..6.  A batch with actuator rows runs the kernel instances that read them, which also read body-offset rows:
+ * without rows of its own the batch gets offset rows holding the model's values (and constant rows, as cassie_batch_set_env_body_pos does) --
+ * cassie_batch_get_env_body_pos reports the model's values, cassie_batch_clear_env_body_pos puts them back instead of dropping the rows, and
+ * cassie_batch_clear_env_actuators drops them unless a body-offset call has written them since.  The rows are model inputs: reset and snapshot
+ * restore leave them alone, cassie_sim_copy copies them (as the rows hold them), cassie_sim_step_pd_batch honours them.  The gear, the safety layer's torque limits and the
+ * encoders stay the model's.  get: what every environment sees (the model's values without rows).  clear: back to the model's actuators and the
+ * kernel instances that ran before.  Device rows: cassie_batch_device_ptr(b, "actuators"), [n][ACT_W = 40] in the batch precision: lo[10], hi[10],
+ * wmax[10] (rad/s), delay[10] (a real; the kernel reads it clamped to 0..6, NaN as 0, truncated) -- a write takes effect at the next launch, and the
+ * rows are what the verbs work on: a masked set changes the masked environments' rows only, get reports what the rows hold (a value written on the
+ * device as rpm = wmax * 60 / 2 pi and the delay as the kernel reads it). */
+int cassie_batch_set_env_actuators(cassie_batch_t *b, const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask);
+int cassie_batch_get_env_actuators(cassie_batch_t *b, double *ctrlrange, double *rpm, int *delay);
+int cassie_batch_clear_env_actuators(cassie_batch_t *b);
+/* The controller-stage state of every environment, as the reference's cassie_sim_t holds it: the torque delay line torque_delay [n][10][6] (slot 0
+ * newest), the drive encoders' integer FIR taps drive_filter [n][10][9], the joint encoders' IIR filters joint_x [n][6][4] and joint_y [n][6][3].
+ * NULL parts are skipped; set changes masked environments only (mask NULL: all).  They are state: reset, snapshots and cassie_sim_copy carry them. */
+int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y);
+int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y,
+                                    const unsigned char *mask);
+
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
