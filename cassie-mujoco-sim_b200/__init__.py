@@ -591,6 +591,50 @@ class CassieBatch:
         if self._act_lib().cassie_batch_clear_env_actuators(self.h) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- per-environment mechanics (link inertia, rotor armature, leaf springs: sim-to-real randomisation)
+    def _mech_lib(self):
+        L = self.L
+        if not getattr(L, '_mech_bound', False):
+            vp, dp = C.c_void_p, C.POINTER(C.c_double)
+            L.cassie_batch_set_env_mechanics.argtypes = [vp, dp, dp, dp, dp, vp]
+            L.cassie_batch_get_env_mechanics.argtypes = [vp, dp, dp, dp, dp]
+            L.cassie_batch_clear_env_mechanics.argtypes = [vp]
+            L.cassie_batch_njnt.argtypes = [vp]
+            for n in ('set_env_mechanics', 'get_env_mechanics', 'clear_env_mechanics', 'njnt'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._mech_bound = True
+        return L
+
+    def _mech_shapes(self):
+        L = self._mech_lib()
+        return (L.cassie_batch_nbody(self.h), 3), (self.nv,), (L.cassie_batch_njnt(self.h),), (L.cassie_batch_njnt(self.h),)
+
+    def set_env_mechanics(self, inertia=None, armature=None, stiffness=None, springref=None, mask=None):
+        """each environment's mechanics: inertia [nbody, 3] or [n, nbody, 3] -- MuJoCo's body_inertia, the principal moments, in model body order --,
+        armature [nv] or [n, nv] -- dof_armature --, stiffness and springref [njnt] or [n, njnt] -- jnt_stiffness and qpos_spring of every hinge (slide,
+        ball and free joints must keep what env_mechanics() reports).  A part left None is kept; mask [n]: only the selected environments change.  A
+        non-finite value, a negative moment / armature / stiffness, moments with A + B < C, or a change to the world body, a body welded to the world or
+        the extra free body raises, and nothing changes.  As in MuJoCo the mj_setConst constants are not refreshed: call set_const.  Reset and snapshot
+        restore leave the rows alone."""
+        L = self._mech_lib()
+        a = [self._arr(v, np.float64, (self.n,) + sh) for v, sh in zip((inertia, armature, stiffness, springref), self._mech_shapes())]
+        m = self._arr(mask, np.uint8, (self.n,))
+        if L.cassie_batch_set_env_mechanics(self.h, *[None if v is None else self._dp(v) for v in a], None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_mechanics(self):
+        """dict of inertia [n, nbody, 3], armature [n, nv], stiffness [n, njnt], springref [n, njnt]: what each environment sees (the model's without rows)"""
+        L = self._mech_lib()
+        out = [np.zeros((self.n,) + sh) for sh in self._mech_shapes()]
+        if L.cassie_batch_get_env_mechanics(self.h, *[self._dp(v) for v in out]) != 0:
+            raise RuntimeError(_last_error())
+        return dict(zip(('inertia', 'armature', 'stiffness', 'springref'), out))
+
+    def clear_env_mechanics(self):
+        """back to the model's inertias, armatures and springs and the kernel instances that ran before"""
+        if self._mech_lib().cassie_batch_clear_env_mechanics(self.h) != 0:
+            raise RuntimeError(_last_error())
+
     def actuator_state(self):
         """dict of the controller-stage state: torque_delay [n, 10, 6] (slot 0 newest), drive_filter [n, 10, 9] int32, joint_x [n, 6, 4], joint_y [n, 6, 3]"""
         L = self._act_lib()
@@ -876,7 +920,8 @@ class CassieBatch:
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
         frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width],
         terrain [n] int32: each environment's bank entry, read mod K at the next launch; set_env_hfield first; actuators [n, 40]: lo[10], hi[10], wmax[10]
-        in rad/s, delay[10], read at the next launch; set_env_actuators first).  set_frames /
+        in rad/s, delay[10], read at the next launch; set_env_actuators first; mechanics [n, 192]: body_inertia[32][3], armature[32], stiffness[32],
+        qpos_spring[32] per main-tree dof (the springs of hinge dofs only are read), read at the next launch; set_env_mechanics first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -886,7 +931,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field == 'terrain':
             ts = '<i4'

@@ -34,6 +34,7 @@ CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_S
 CASSIE_STEP_ENTRY(f02f) CASSIE_STEP_ENTRY(f12f) CASSIE_STEP_ENTRY(f22f) CASSIE_STEP_ENTRY(d02f) CASSIE_STEP_ENTRY(d12f) CASSIE_STEP_ENTRY(d22f) CASSIE_STEP_ENTRY(f13f) CASSIE_STEP_ENTRY(d13f)
 CASSIE_STEP_ENTRY(f144) CASSIE_STEP_ENTRY(f157) CASSIE_STEP_ENTRY(d157) CASSIE_STEP_ENTRY(f15f) CASSIE_STEP_ENTRY(d15f) CASSIE_STEP_ENTRY(f17f) CASSIE_STEP_ENTRY(d17f)
 CASSIE_STEP_ENTRY(f1c4) CASSIE_STEP_ENTRY(f1d7) CASSIE_STEP_ENTRY(d1d7) CASSIE_STEP_ENTRY(f1df) CASSIE_STEP_ENTRY(d1df) CASSIE_STEP_ENTRY(f1ff) CASSIE_STEP_ENTRY(d1ff)
+CASSIE_STEP_ENTRY(f11c4) CASSIE_STEP_ENTRY(f11d7) CASSIE_STEP_ENTRY(d11d7) CASSIE_STEP_ENTRY(f11df) CASSIE_STEP_ENTRY(d11df) CASSIE_STEP_ENTRY(f11ff) CASSIE_STEP_ENTRY(d11ff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -43,6 +44,15 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_MC) {   // per-environment mechanics: the F_MC twins of the F_AC instances, by the same rule (a batch with mechanics rows always has actuator rows)
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC; return dbl ? cassie_step_entry_d11ff() : cassie_step_entry_f11ff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC; return dbl ? cassie_step_entry_d11df() : cassie_step_entry_f11df(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC; return cassie_step_entry_f11c4(); }   // no frame / acceleration / dynamics / Jacobian launch
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC;
+    return dbl ? cassie_step_entry_d11d7() : cassie_step_entry_f11d7();
+  }
   if (feat & F_AC) {   // per-environment actuators: the F_AC twins of the F_BP instances, by the same rule (a batch with actuator rows always has offset rows)
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value;
@@ -321,6 +331,11 @@ struct BatchBase {
   virtual bool set_env_actuators(const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) = 0;
   virtual bool get_env_actuators(double *ctrlrange, double *rpm, int *delay) = 0;
   virtual bool clear_env_actuators() = 0;
+  // per-environment mechanics (F_MC instances): inertia [n][nbody][3], armature [n][nv], stiffness and springref [n][njnt], each may be null (kept); only
+  // masked environments change; checked as a whole before anything changes
+  virtual bool set_env_mechanics(const double *inertia, const double *armature, const double *stiffness, const double *springref, const unsigned char *mask) = 0;
+  virtual bool get_env_mechanics(double *inertia, double *armature, double *stiffness, double *springref) = 0;
+  virtual bool clear_env_mechanics() = 0;
   // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
   // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
   virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
@@ -375,9 +390,12 @@ template <typename real> struct Batch : BatchBase {
   real *d_act = nullptr;                   // A.act: [n][ACT_W] per-environment actuators, allocated by the first cassie_batch_set_env_actuators (F_AC instances)
   std::vector<double> ac_host;             // [n][nu][4] lo, hi, rpm, delay every environment sees while d_act exists (in double: what get returns)
   bool ac_bpos = false;                    // the offset rows were allocated by the actuator setter (model values), and no body-offset call has written them since
+  real *d_mech = nullptr;                  // A.mech: [n][MECH_W] per-environment mechanics, allocated by the first cassie_batch_set_env_mechanics (F_MC instances)
+  std::vector<double> mc_host;             // [n][mech_host_w()] inertia, armature, stiffness, springref every environment sees while d_mech exists (in double)
+  bool mc_act = false;                     // the actuator rows were allocated by the mechanics setter (model values), and no actuator call has written them since
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -447,7 +465,8 @@ template <typename real> struct Batch : BatchBase {
         if (ext == 1)   // per-environment body offsets: every instance step_entry routes F_BP launches to (the extended scratch)
           for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) {   // and their F_AC twins (per-environment actuators)
             CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }   // and their F_MC twins
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -799,6 +818,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     hm = src->hm;
     if (!rebuild_model()) return false;
+    if (!src->d_mech && !clear_env_mechanics()) return false;   // likewise the mechanics rows and the actuator rows their setter allocated
     if (!src->d_act && !clear_env_actuators()) return false;   // likewise the actuator rows and the offset rows their setter allocated
     if (!src->d_bpos && !clear_env_body_pos()) return false;   // before the constant rows are copied: clearing drops rows the offset setter allocated
     if (src->A.cenv) { if (!ensure_cenv()) return false; CUDA_OK(cudaMemcpyAsync(A.cenv, src->A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToDevice, stream)); }
@@ -819,6 +839,13 @@ template <typename real> struct Batch : BatchBase {
       if (!d_act) CUDA_OK(cudaMalloc(&d_act, sizeof(real) * n * ACT_W));
       CUDA_OK(cudaMemcpy(d_act, src->d_act, sizeof(real) * n * ACT_W, cudaMemcpyDeviceToDevice));
       A.act = d_act;
+    }
+    if (src->d_mech) {   // likewise the mechanics rows (the actuator rows came just now)
+      mc_host = src->mc_host; mc_act = src->mc_act;
+      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
+      if (!d_mech) CUDA_OK(cudaMalloc(&d_mech, sizeof(real) * n * MECH_W));
+      CUDA_OK(cudaMemcpy(d_mech, src->d_mech, sizeof(real) * n * MECH_W, cudaMemcpyDeviceToDevice));
+      A.mech = d_mech;
     }
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
@@ -1059,6 +1086,14 @@ template <typename real> struct Batch : BatchBase {
   void model_act(int i, double *a) const {   // motor i as the model has it: lo, hi (the clamp the block holds), rpm, the reference's delay
     a[0] = (double)h_model_copy.act_ctrl_lo[i]; a[1] = (double)h_model_copy.act_ctrl_hi[i]; a[2] = hm.actuator_user[i]; a[3] = AC_MAXDELAY;
   }
+  void model_act_rows(std::vector<real> &all) {   // the mirror and the rows holding the model's actuators in every environment
+    const int nu = hm.nu;
+    ac_host.resize((size_t)n * nu * 4); all.assign((size_t)n * ACT_W, real(0));
+    for (int e = 0; e < n; e++) for (int i = 0; i < nu; i++) {
+      double *a = &ac_host[((size_t)e * nu + i) * 4]; model_act(i, a);
+      for (int f = 0; f < 4; f++) all[(size_t)e * ACT_W + AC_FIELD[f] + i] = act_row_value(a, f);
+    }
+  }
   bool set_env_actuators(const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) override {
     const std::string verb = "cassie_batch_set_env_actuators";
     const int nu = hm.nu;
@@ -1072,14 +1107,10 @@ template <typename real> struct Batch : BatchBase {
       if (!put_bpos()) return false;
       ac_bpos = true;
     }
+    mc_act = false;   // the rows are the caller's now, also when the mechanics setter allocated them
     std::vector<real> all;
-    if (!d_act) {   // the first call: every environment starts from the model's actuators
-      ac_host.resize((size_t)n * nu * 4); all.assign((size_t)n * ACT_W, real(0));
-      for (int e = 0; e < n; e++) for (int i = 0; i < nu; i++) {
-        double *a = &ac_host[((size_t)e * nu + i) * 4]; model_act(i, a);
-        for (int f = 0; f < 4; f++) all[(size_t)e * ACT_W + AC_FIELD[f] + i] = act_row_value(a, f);
-      }
-    } else if (!pull_act(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    if (!d_act) model_act_rows(all);   // the first call: every environment starts from the model's actuators
+    else if (!pull_act(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
     for (int e = 0; e < n; e++) {
       if (mask && !mask[e]) continue;
       for (int i = 0; i < nu; i++) {
@@ -1115,12 +1146,110 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
+  // back to the model's actuators and the instances that ran before.  A batch with mechanics rows keeps actuator rows, holding the model's values again.
   bool clear_env_actuators() override {
+    if (d_mech) { std::vector<real> all; model_act_rows(all); mc_act = true; return push_act(all); }
     ac_host.clear();
     if (!d_act) return true;
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaFree(d_act)); d_act = nullptr; A.act = nullptr;
     if (ac_bpos) { ac_bpos = false; return clear_env_body_pos(); }   // (which drops the constant rows too when the offset rows brought them)
+    return true;
+  }
+  // ---- per-environment mechanics (link inertia, rotor armature, leaf springs: sim-to-real randomisation): MuJoCo's body_inertia, dof_armature and the
+  // jnt_stiffness / qpos_spring of the hinges per environment, read by the F_MC instances' cinert, CRB and passive phases.  Those instances are the F_MC
+  // twins of the F_AC ones, so a batch with mechanics rows carries actuator rows too: when it has none, the setter allocates them holding the model's
+  // values (and offset and constant rows with them, as the actuator setter does); clear drops them again unless an actuator call has written them since.
+  // As with the actuator rows, the device rows are what the environments run with, and the mirror keeps the doubles the verb was last given.
+  int mech_host_w() const { return 3 * hm.nbody + hm.nv + 2 * hm.njnt; }   // the mirror per environment: inertia [nbody][3], armature [nv], stiffness [njnt], springref [njnt]
+  int mech_slot(int k) const {   // the row slot of mirror entry k, or -1 where the kernel reads the block (the extra free body's dofs, non-hinge springs)
+    const int nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
+    if (k < nb3) return MC_INERTIA + k;
+    if ((k -= nb3) < nv) return k < h_model_copy.nv ? MC_ARMATURE + k : -1;
+    const int base = (k -= nv) < nj ? MC_STIFF : MC_SPRING, j = k % nj;
+    return hm.jnt_type[j] == JNT_HINGE ? base + hm.jnt_dofadr[j] : -1;
+  }
+  double block_mech(int k) const {   // mirror entry k as the shared block has it (what get reports where the kernel reads the block)
+    const int nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
+    if (k < nb3) return hm.body_inertia[k];
+    if ((k -= nb3) < nv) return hm.dof_armature[k];
+    return (k -= nv) < nj ? hm.jnt_stiffness[k] : hm.qpos_spring[hm.jnt_qposadr[k - nj]];
+  }
+  bool pull_mech(std::vector<real> &all) {
+    all.assign((size_t)n * MECH_W, real(0));
+    if (!d_mech) return true;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemcpyAsync(all.data(), d_mech, sizeof(real) * n * MECH_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  bool push_mech(const std::vector<real> &all) {
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    if (!d_mech) CUDA_OK(cudaMalloc(&d_mech, sizeof(real) * n * MECH_W));
+    CUDA_OK(cudaMemcpy(d_mech, all.data(), sizeof(real) * n * MECH_W, cudaMemcpyHostToDevice));
+    A.mech = d_mech;
+    return true;
+  }
+  bool set_env_mechanics(const double *inertia, const double *armature, const double *stiffness, const double *springref, const unsigned char *mask) override {
+    const std::string verb = "cassie_batch_set_env_mechanics";
+    const std::string why = env_mechanics_check(hm, n, h_model_copy.xb, h_model_copy.nv, inertia, armature, stiffness, springref, mask);   // every masked value first
+    if (!why.empty()) { set_err(verb + ": " + why); return false; }
+    if (!d_act) {   // the F_MC instances read actuator rows: the model's values, dropped again by clear unless an actuator call writes them
+      if (!set_env_actuators(nullptr, nullptr, nullptr, nullptr)) return false;
+      mc_act = true;
+    }
+    const int w = mech_host_w(), nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
+    std::vector<real> all;
+    if (!d_mech) {   // the first call: every environment starts from the model's values (a non-hinge dof's slots too, though the kernel reads the block there)
+      mc_host.resize((size_t)n * w); all.assign((size_t)n * MECH_W, real(0));
+      for (int e = 0; e < n; e++) {
+        real *r = &all[(size_t)e * MECH_W];
+        for (int k = 0; k < w; k++) { mc_host[(size_t)e * w + k] = block_mech(k); const int sl = mech_slot(k); if (sl >= 0) r[sl] = (real)block_mech(k); }
+        for (int i = 0; i < h_model_copy.nv; i++) { const int j = hm.dof_jntid[i]; r[MC_STIFF + i] = (real)hm.jnt_stiffness[j]; r[MC_SPRING + i] = (real)hm.qpos_spring[hm.jnt_qposadr[j]]; }
+      }
+    } else if (!pull_mech(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    const double *part[4] = {inertia, armature, stiffness, springref};
+    const int off[5] = {0, nb3, nb3 + nv, nb3 + nv + nj, w};
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      for (int p = 0; p < 4; p++) {
+        if (!part[p]) continue;
+        const int cnt = off[p + 1] - off[p];
+        for (int i = 0; i < cnt; i++) {
+          const double v = part[p][(size_t)e * cnt + i]; const int k = off[p] + i, sl = mech_slot(k);
+          mc_host[(size_t)e * w + k] = v;
+          if (sl >= 0) all[(size_t)e * MECH_W + sl] = (real)v;
+        }
+      }
+    }
+    return push_mech(all);
+  }
+  // what every environment runs with: a value the device row still holds as the verb stored it is reported as the verb was given it, one written on the
+  // device from the row; where the kernel reads the block (the extra free body's armature, non-hinge springs), the block's current value
+  bool get_env_mechanics(double *inertia, double *armature, double *stiffness, double *springref) override {
+    const int w = mech_host_w(), nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
+    std::vector<real> all;
+    if (!pull_mech(all)) return false;
+    double *part[4] = {inertia, armature, stiffness, springref};
+    const int off[5] = {0, nb3, nb3 + nv, nb3 + nv + nj, w};
+    for (int e = 0; e < n; e++) for (int p = 0; p < 4; p++) {
+      if (!part[p]) continue;
+      const int cnt = off[p + 1] - off[p];
+      for (int i = 0; i < cnt; i++) {
+        const int k = off[p] + i, sl = mech_slot(k);
+        double v = block_mech(k);
+        if (d_mech && sl >= 0) { const real dv = all[(size_t)e * MECH_W + sl]; const double a = mc_host[(size_t)e * w + k]; v = dv == (real)a ? a : (double)dv; }
+        part[p][(size_t)e * cnt + i] = v;
+      }
+    }
+    return true;
+  }
+  // back to the model's values and the instances that ran before (which drops the actuator rows too when this setter brought them)
+  bool clear_env_mechanics() override {
+    mc_host.clear();
+    if (!d_mech) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_mech)); d_mech = nullptr; A.mech = nullptr;
+    if (mc_act) { mc_act = false; return clear_env_actuators(); }
     return true;
   }
   // ---- the controller-stage state: the delay line, the encoders' filters (views of the cst / dfilt rows; snapshots carry them)
@@ -1328,7 +1457,7 @@ template <typename real> struct Batch : BatchBase {
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1396,7 +1525,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -1480,7 +1609,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
-  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W;
+  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -1497,6 +1626,7 @@ void cassie_batch_get_time(cassie_batch_t *b, double *out) { b->impl->get("time"
 void cassie_batch_get_obs(cassie_batch_t *b, double *out) { b->impl->get("obs", out); }
 int cassie_batch_nbody(const cassie_batch_t *b) { return b->impl->hm.nbody; }
 int cassie_batch_ngeom(const cassie_batch_t *b) { return b->impl->hm.ngeom; }
+int cassie_batch_njnt(const cassie_batch_t *b) { return b->impl->hm.njnt; }
 int cassie_batch_set_body_mass(cassie_batch_t *b, const double *mass) { return b->impl->set_model_rows("body_mass", mass, b->impl->hm.nbody) ? 0 : -1; }
 int cassie_batch_set_body_ipos(cassie_batch_t *b, const double *ipos) { return b->impl->set_model_rows("body_ipos", ipos, 3 * b->impl->hm.nbody) ? 0 : -1; }
 int cassie_batch_set_dof_damping(cassie_batch_t *b, const double *damp) { return b->impl->set_model_rows("dof_damping", damp, b->impl->hm.nv) ? 0 : -1; }
@@ -1907,6 +2037,11 @@ int cassie_batch_clear_env_body_pos(cassie_batch_t *b) { return b->impl->clear_e
 int cassie_batch_set_env_actuators(cassie_batch_t *b, const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask) { return b->impl->set_env_actuators(ctrlrange, rpm, delay, mask) ? 0 : -1; }
 int cassie_batch_get_env_actuators(cassie_batch_t *b, double *ctrlrange, double *rpm, int *delay) { return b->impl->get_env_actuators(ctrlrange, rpm, delay) ? 0 : -1; }
 int cassie_batch_clear_env_actuators(cassie_batch_t *b) { return b->impl->clear_env_actuators() ? 0 : -1; }
+// per-environment mechanics (link inertia, rotor armature, hinge springs); see include/cassie_b200.h
+int cassie_batch_set_env_mechanics(cassie_batch_t *b, const double *inertia, const double *armature, const double *stiffness, const double *springref, const unsigned char *mask) {
+  return b->impl->set_env_mechanics(inertia, armature, stiffness, springref, mask) ? 0 : -1; }
+int cassie_batch_get_env_mechanics(cassie_batch_t *b, double *inertia, double *armature, double *stiffness, double *springref) { return b->impl->get_env_mechanics(inertia, armature, stiffness, springref) ? 0 : -1; }
+int cassie_batch_clear_env_mechanics(cassie_batch_t *b) { return b->impl->clear_env_mechanics() ? 0 : -1; }
 int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) { return b->impl->get_actuator_state(torque_delay, drive_filter, joint_x, joint_y) ? 0 : -1; }
 int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) {
   return b->impl->set_actuator_state(torque_delay, drive_filter, joint_x, joint_y, mask) ? 0 : -1; }

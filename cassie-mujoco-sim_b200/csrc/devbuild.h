@@ -124,6 +124,56 @@ inline std::string env_actuators_check(int n, int nu, const double *ctrlrange, c
   return std::string();
 }
 
+// cassie_batch_set_env_mechanics' check of every masked value, before anything changes: an empty reason, else the first refusal, naming the environment,
+// the body / dof / joint and the field.  Refused: a non-finite value; a negative inertia moment, armature or stiffness; moments that break MuJoCo's
+// compiler rule A + B >= C for some order; a change (against the shared block m, which is what get reports there) to the inertia of the world body, a
+// body welded to the world or the extra free body xb, to the armature of the extra free body's dofs (>= nv_main), or to the stiffness or qpos_spring of a
+// slide, ball or free joint.  inertia [n][nbody][3], armature [n][nv], stiffness and springref [n][njnt]; null parts are not checked (kept)
+inline std::string env_mechanics_check(const HostModel &m, int n, int xb, int nv_main, const double *inertia, const double *armature, const double *stiffness,
+                                       const double *springref, const unsigned char *mask) {
+  const int nb = m.nbody, nv = m.nv, nj = m.njnt;
+  auto joint = [&](int j) { return (size_t)j < m.names_joint.size() && !m.names_joint[j].empty() ? m.names_joint[j] : std::to_string(j); };   // unnamed: the index
+  for (int e = 0; e < n; e++) {
+    if (mask && !mask[e]) continue;
+    const std::string env = "environment " + std::to_string(e) + ", ";
+    if (inertia) for (int b = 0; b < nb; b++) {
+      const double *I = inertia + ((size_t)e * nb + b) * 3, *I0 = &m.body_inertia[3 * b];
+      const std::string at = env + "body " + m.names_body[b] + ": body_inertia ";
+      for (int k = 0; k < 3; k++) {
+        if (!std::isfinite(I[k])) return at + "is not finite";
+        if (I[k] < 0) return at + "must be >= 0";
+      }
+      if (I[0] + I[1] < I[2] || I[1] + I[2] < I[0] || I[2] + I[0] < I[1]) return at + "must satisfy A + B >= C for every order of the three moments";
+      if (I[0] == I0[0] && I[1] == I0[1] && I[2] == I0[2]) continue;
+      const std::string w = env_body_pos_check(m, b, xb);
+      if (!w.empty()) return at + "of " + w + " cannot change";
+    }
+    if (armature) for (int i = 0; i < nv; i++) {
+      const double a = armature[(size_t)e * nv + i];
+      const std::string at = env + "dof " + std::to_string(i) + " (joint " + joint(m.dof_jntid[i]) + "): dof_armature ";
+      if (!std::isfinite(a)) return at + "is not finite";
+      if (a < 0) return at + "must be >= 0";
+      if (i >= nv_main && a != m.dof_armature[i]) return at + "of the extra free body cannot change";
+    }
+    for (int j = 0; j < nj; j++) {
+      const std::string at = env + "joint " + joint(j) + ": ";
+      const bool hinge = m.jnt_type[j] == JNT_HINGE;
+      if (stiffness) {
+        const double k = stiffness[(size_t)e * nj + j];
+        if (!std::isfinite(k)) return at + "jnt_stiffness is not finite";
+        if (k < 0) return at + "jnt_stiffness must be >= 0";
+        if (!hinge && k != m.jnt_stiffness[j]) return at + "jnt_stiffness of a slide, ball or free joint cannot change";
+      }
+      if (springref) {
+        const double q = springref[(size_t)e * nj + j];
+        if (!std::isfinite(q)) return at + "qpos_spring is not finite";
+        if (!hinge && q != m.qpos_spring[m.jnt_qposadr[j]]) return at + "qpos_spring of a slide, ball or free joint cannot change";
+      }
+    }
+  }
+  return std::string();
+}
+
 // one row of a batch's frame table (FT_W) for body (kind 0) or site (kind 1) `name`; its id, or -1 with a reason for an unknown name or kind
 template <typename real> int frame_table_row(const HostModel &m, const char *name, int kind, real *row, std::string &err) {
   for (int c = 0; c < FT_W; c++) row[c] = 0;

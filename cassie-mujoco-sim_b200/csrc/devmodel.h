@@ -36,6 +36,7 @@ constexpr int F_FR = 16;  // frame rows (FRAME_W per named body / site) are fill
 constexpr int F_TR = 32;  // per-environment terrain: the bank entry from a selection row, the height field's size from its F_EG slot (with F_ALL | F_EG only)
 constexpr int F_BP = 64;  // per-environment body offsets: each body's position in its parent frame comes from a BP_W row instead of the model block (extended instances only)
 constexpr int F_AC = 128; // per-environment actuators: ctrlrange, no-load speed and torque delay of every motor come from an ACT_W row (with F_BP, extended instances only)
+constexpr int F_MC = 256; // per-environment mechanics: link inertia, rotor armature and hinge springs come from a MECH_W row (with F_BP | F_AC, extended instances only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -181,6 +182,12 @@ constexpr int BP_W = MB * 3;
 constexpr int ACT_W = 40;
 constexpr int AC_LO = 0, AC_HI = 10, AC_WMAX = 20, AC_DELAY = 30;
 constexpr int AC_MAXDELAY = 6;   // the length of the delay line (cst CS_DELAY [10][6]): the reference's TORQUE_DELAY_CYCLES
+// per-environment mechanics (optional, cassie_batch_set_env_mechanics; F_MC instances): MuJoCo's body_inertia (principal moments) of every body [MB][3] in
+// model body order, and per main-tree dof its dof_armature and the jnt_stiffness / qpos_spring of its joint; entries past nbody / nv zero.  The cinert
+// phase reads the inertia, the CRB phase the armature (the diagonal of M and of M + hB), the passive force the spring of a hinge dof only: slide, ball
+// and free joints keep the model block's (the pelvis slides carry cassie_sim_hold's spring).  A model input like the CE rows.
+constexpr int MECH_W = 192;
+constexpr int MC_INERTIA = 0, MC_ARMATURE = 96, MC_STIFF = 128, MC_SPRING = 160;
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

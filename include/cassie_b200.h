@@ -32,7 +32,7 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit);
 /* include/cassiemujoco.h:77  (src/cassiemujoco.c:1102-1113): NULL is a no-op */
 void cassie_sim_free(cassie_sim_t *sim);
 /* new: the one-environment batch a simulator steps, owned by it (not to be freed), so that the batch verbs -- per-environment rows such as
- * cassie_batch_set_env_actuators, device pointers -- apply to a legacy simulator; cassie_sim_copy copies what they set. */
+ * cassie_batch_set_env_actuators or cassie_batch_set_env_mechanics, device pointers -- apply to a legacy simulator; cassie_sim_copy copies what they set. */
 cassie_batch_t *cassie_sim_batch(cassie_sim_t *c);
 /* include/cassiemujoco.h:95  (src/cassiemujoco.c:1147-1157): THE hot path, one environment, one 0.5 ms tick */
 void cassie_sim_step_pd(cassie_sim_t *sim, state_out_t *y, const pd_in_t *u);
@@ -454,6 +454,7 @@ int cassie_batch_query(cassie_batch_t *b);
  * masses, mean inertia -- and, with reset_state != 0, the state reset of cassie_sim_set_const (src/cassiemujoco.c:955-971).  0 / -1. */
 int cassie_batch_nbody(const cassie_batch_t *b);
 int cassie_batch_ngeom(const cassie_batch_t *b);
+int cassie_batch_njnt(const cassie_batch_t *b);   /* joints of the model (the stiffness / springref width of cassie_batch_set_env_mechanics) */
 int cassie_batch_set_body_mass(cassie_batch_t *b, const double *mass);
 int cassie_batch_set_body_ipos(cassie_batch_t *b, const double *ipos);
 int cassie_batch_set_dof_damping(cassie_batch_t *b, const double *damp);
@@ -576,6 +577,31 @@ int cassie_batch_clear_env_body_pos(cassie_batch_t *b);
 int cassie_batch_set_env_actuators(cassie_batch_t *b, const double *ctrlrange, const double *rpm, const int *delay, const unsigned char *mask);
 int cassie_batch_get_env_actuators(cassie_batch_t *b, double *ctrlrange, double *rpm, int *delay);
 int cassie_batch_clear_env_actuators(cassie_batch_t *b);
+/* Per-environment mechanics (domain randomisation of the rigid-body model's inertias and the leaf springs): for each environment
+ *   inertia [n][nbody][3]: MuJoCo's body_inertia, the principal moments of every body in model body order (the principal axes, body_iquat, stay the
+ *                          model's);
+ *   armature [n][nv]:      MuJoCo's dof_armature, the reflected rotor inertia on the diagonal of the mass matrix;
+ *   stiffness [n][njnt]:   MuJoCo's jnt_stiffness, and springref [n][njnt]: its qpos_spring (the rest angle), of every hinge -- cassie.xml's shin and
+ *                          heel springs.  Slide, ball and free joints keep the model's: the pelvis slides carry cassie_sim_hold's spring.
+ * Any of the four may be NULL (kept); mask [n] (or NULL: all) selects the environments that change.  The first call gives every environment the model's
+ * values.  0, or -1 with nothing changed (cassie_b200_last_error names the environment, the body / dof / joint and the field) for a non-finite value, a
+ * negative moment, armature or stiffness, moments that break MuJoCo's rule A + B >= C for some order of the three, or a change to the world body, a body
+ * welded to the world or the extra free body (its inertia and dofs), or to the stiffness or springref of a slide, ball or free joint: there the entries
+ * must equal what get reports, the shared model's current values.  As in MuJoCo, the mj_setConst constants (dof_invweight0, body_invweight0, the PGS
+ * scale) are not refreshed: cassie_batch_set_const computes them with each environment's inertia and armature.  A batch with mechanics rows runs the
+ * kernel instances that read them, which also read actuator rows: without rows of its own the batch gets actuator rows holding the model's values (and
+ * offset and constant rows through them, as cassie_batch_set_env_actuators does) -- cassie_batch_clear_env_actuators puts the model's values back
+ * instead of dropping the rows, and cassie_batch_clear_env_mechanics drops them unless an actuator call has written them since.  The rows are model
+ * inputs: reset and snapshot restore leave them alone, cassie_sim_copy copies them, cassie_sim_step_pd_batch honours them.  The in-kernel estimator's
+ * spring model keeps the model's constants, as the robot's own estimator does.  get: what every environment sees (the model's values without rows).
+ * clear: back to the model's values and the kernel instances that ran before.  Device rows: cassie_batch_device_ptr(b, "mechanics"), [n][MECH_W = 192]
+ * in the batch precision: body_inertia [32][3] (model body order), then per main-tree dof armature [32], its joint's stiffness [32] and qpos_spring
+ * [32], zero past nbody / nv; the kernel reads the stiffness and qpos_spring slots of hinge dofs only.  A write takes effect at the next launch, and the
+ * rows are what the verbs work on: a masked set changes the masked environments' rows only, get reports what the rows hold. */
+int cassie_batch_set_env_mechanics(cassie_batch_t *b, const double *inertia, const double *armature, const double *stiffness, const double *springref,
+                                   const unsigned char *mask);
+int cassie_batch_get_env_mechanics(cassie_batch_t *b, double *inertia, double *armature, double *stiffness, double *springref);
+int cassie_batch_clear_env_mechanics(cassie_batch_t *b);
 /* The controller-stage state of every environment, as the reference's cassie_sim_t holds it: the torque delay line torque_delay [n][10][6] (slot 0
  * newest), the drive encoders' integer FIR taps drive_filter [n][10][9], the joint encoders' IIR filters joint_x [n][6][4] and joint_y [n][6][3].
  * NULL parts are skipped; set changes masked environments only (mask NULL: all).  They are state: reset, snapshots and cassie_sim_copy carry them. */
@@ -584,7 +610,7 @@ int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_dela
                                     const unsigned char *mask);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
