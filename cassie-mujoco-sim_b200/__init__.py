@@ -635,6 +635,49 @@ class CassieBatch:
         if self._mech_lib().cassie_batch_clear_env_mechanics(self.h) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- per-environment contact softness (ground stiffness, damping and impedance: sim-to-real randomisation)
+    def _contact_lib(self):
+        L = self.L
+        if not getattr(L, '_contact_bound', False):
+            vp, dp = C.c_void_p, C.POINTER(C.c_double)
+            L.cassie_batch_set_env_contact.argtypes = [vp, dp, dp, dp, vp]
+            L.cassie_batch_get_env_contact.argtypes = [vp, dp, dp, dp]
+            L.cassie_batch_clear_env_contact.argtypes = [vp]
+            for n in ('set_env_contact', 'get_env_contact', 'clear_env_contact'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._contact_bound = True
+        return L
+
+    def _contact_shapes(self):
+        ng = self.L.cassie_batch_ngeom(self.h)
+        return (ng, 2), (ng, 5), (ng,)
+
+    def set_env_contact(self, solref=None, solimp=None, solmix=None, mask=None):
+        """each environment's contact softness, per geom (model geom order): solref [ngeom, 2] or [n, ngeom, 2] -- MuJoCo's geom_solref, (timeconst,
+        dampratio) or direct (-stiffness, -damping) --, solimp [ngeom, 5] or [n, ngeom, 5] -- geom_solimp (dmin, dmax, width, midpoint, power) --, solmix
+        [ngeom] or [n, ngeom] -- geom_solmix.  Each contact mixes its two geoms' values as MuJoCo's mj_contactParam does.  A part left None is kept; mask
+        [n]: only the selected environments change.  A non-finite value, a solref with mixed signs, a solimp outside 0 < dmin, dmax, midpoint < 1,
+        width >= 0, power >= 1, or a negative solmix raises, and nothing changes.  Entries of geoms that never collide are ignored.  Reset and snapshot
+        restore leave the rows alone."""
+        L = self._contact_lib()
+        a = [self._arr(v, np.float64, (self.n,) + sh) for v, sh in zip((solref, solimp, solmix), self._contact_shapes())]
+        m = self._arr(mask, np.uint8, (self.n,))
+        if L.cassie_batch_set_env_contact(self.h, *[None if v is None else self._dp(v) for v in a], None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_contact(self):
+        """dict of solref [n, ngeom, 2], solimp [n, ngeom, 5], solmix [n, ngeom]: what each environment sees (the model's without rows)"""
+        L = self._contact_lib()
+        out = [np.zeros((self.n,) + sh) for sh in self._contact_shapes()]
+        if L.cassie_batch_get_env_contact(self.h, *[self._dp(v) for v in out]) != 0:
+            raise RuntimeError(_last_error())
+        return dict(zip(('solref', 'solimp', 'solmix'), out))
+
+    def clear_env_contact(self):
+        """back to the model's contact softness and the kernel instances that ran before"""
+        if self._contact_lib().cassie_batch_clear_env_contact(self.h) != 0:
+            raise RuntimeError(_last_error())
+
     def actuator_state(self):
         """dict of the controller-stage state: torque_delay [n, 10, 6] (slot 0 newest), drive_filter [n, 10, 9] int32, joint_x [n, 6, 4], joint_y [n, 6, 3]"""
         L = self._act_lib()
@@ -921,7 +964,9 @@ class CassieBatch:
         frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width],
         terrain [n] int32: each environment's bank entry, read mod K at the next launch; set_env_hfield first; actuators [n, 40]: lo[10], hi[10], wmax[10]
         in rad/s, delay[10], read at the next launch; set_env_actuators first; mechanics [n, 192]: body_inertia[32][3], armature[32], stiffness[32],
-        qpos_spring[32] per main-tree dof (the springs of hinge dofs only are read), read at the next launch; set_env_mechanics first).  set_frames /
+        qpos_spring[32] per main-tree dof (the springs of hinge dofs only are read), read at the next launch; set_env_mechanics first; contact [n, 256]:
+        32 slots of 8 -- solref[2], solimp[5], solmix -- one per device collision geom (moving 0..15, static 16..31; unused slots zero), read at the next
+        launch; set_env_contact first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -931,7 +976,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field == 'terrain':
             ts = '<i4'

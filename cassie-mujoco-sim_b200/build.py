@@ -44,6 +44,12 @@ ACTUATOR_INSTANCES = [('f1c4', 'float', 1, 196), ('f1d7', 'float', 1, 215), ('d1
 # each is the F_MC twin of one ACTUATOR_INSTANCES entry (f1c4, f1d7 / d1d7, f1df / d1df, f1ff / d1ff); tag = precision, kind, features in hex
 MECHANICS_INSTANCES = [('f11c4', 'float', 1, 452), ('f11d7', 'float', 1, 471), ('d11d7', 'double', 1, 471), ('f11df', 'float', 1, 479), ('d11df', 'double', 1, 479),
                        ('f11ff', 'float', 1, 511), ('d11ff', 'double', 1, 511)]
+# the extended kernel with per-environment contact softness (feature 512 = F_CT; cassie_batch_set_env_contact: solref, solimp, solmix per collision geom),
+# always with mechanics rows (a batch with contact rows carries mechanics rows holding the model's values when it has no others, and actuator and offset
+# rows through them): each is the F_CT twin of one MECHANICS_INSTANCES entry (f11c4, f11d7 / d11d7, f11df / d11df, f11ff / d11ff); tag = precision,
+# kind, features in hex
+CONTACT_INSTANCES = [('f13c4', 'float', 1, 964), ('f13d7', 'float', 1, 983), ('d13d7', 'double', 1, 983), ('f13df', 'float', 1, 991), ('d13df', 'double', 1, 991),
+                     ('f13ff', 'float', 1, 1023), ('d13ff', 'double', 1, 1023)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -77,7 +83,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

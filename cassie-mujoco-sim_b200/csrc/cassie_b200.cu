@@ -35,6 +35,7 @@ CASSIE_STEP_ENTRY(f02f) CASSIE_STEP_ENTRY(f12f) CASSIE_STEP_ENTRY(f22f) CASSIE_S
 CASSIE_STEP_ENTRY(f144) CASSIE_STEP_ENTRY(f157) CASSIE_STEP_ENTRY(d157) CASSIE_STEP_ENTRY(f15f) CASSIE_STEP_ENTRY(d15f) CASSIE_STEP_ENTRY(f17f) CASSIE_STEP_ENTRY(d17f)
 CASSIE_STEP_ENTRY(f1c4) CASSIE_STEP_ENTRY(f1d7) CASSIE_STEP_ENTRY(d1d7) CASSIE_STEP_ENTRY(f1df) CASSIE_STEP_ENTRY(d1df) CASSIE_STEP_ENTRY(f1ff) CASSIE_STEP_ENTRY(d1ff)
 CASSIE_STEP_ENTRY(f11c4) CASSIE_STEP_ENTRY(f11d7) CASSIE_STEP_ENTRY(d11d7) CASSIE_STEP_ENTRY(f11df) CASSIE_STEP_ENTRY(d11df) CASSIE_STEP_ENTRY(f11ff) CASSIE_STEP_ENTRY(d11ff)
+CASSIE_STEP_ENTRY(f13c4) CASSIE_STEP_ENTRY(f13d7) CASSIE_STEP_ENTRY(d13d7) CASSIE_STEP_ENTRY(f13df) CASSIE_STEP_ENTRY(d13df) CASSIE_STEP_ENTRY(f13ff) CASSIE_STEP_ENTRY(d13ff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -44,6 +45,15 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_CT) {   // per-environment contact softness: the F_CT twins of the F_MC instances, by the same rule (a batch with contact rows always has mechanics rows)
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT; return dbl ? cassie_step_entry_d13ff() : cassie_step_entry_f13ff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT; return dbl ? cassie_step_entry_d13df() : cassie_step_entry_f13df(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT; return cassie_step_entry_f13c4(); }   // no frame / acceleration / dynamics / Jacobian launch
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT;
+    return dbl ? cassie_step_entry_d13d7() : cassie_step_entry_f13d7();
+  }
   if (feat & F_MC) {   // per-environment mechanics: the F_MC twins of the F_AC instances, by the same rule (a batch with mechanics rows always has actuator rows)
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value;
@@ -336,6 +346,11 @@ struct BatchBase {
   virtual bool set_env_mechanics(const double *inertia, const double *armature, const double *stiffness, const double *springref, const unsigned char *mask) = 0;
   virtual bool get_env_mechanics(double *inertia, double *armature, double *stiffness, double *springref) = 0;
   virtual bool clear_env_mechanics() = 0;
+  // per-environment contact softness (F_CT instances): solref [n][ngeom][2], solimp [n][ngeom][5], solmix [n][ngeom], each may be null (kept); only
+  // masked environments change; checked as a whole before anything changes
+  virtual bool set_env_contact(const double *solref, const double *solimp, const double *solmix, const unsigned char *mask) = 0;
+  virtual bool get_env_contact(double *solref, double *solimp, double *solmix) = 0;
+  virtual bool clear_env_contact() = 0;
   // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
   // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
   virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
@@ -393,9 +408,12 @@ template <typename real> struct Batch : BatchBase {
   real *d_mech = nullptr;                  // A.mech: [n][MECH_W] per-environment mechanics, allocated by the first cassie_batch_set_env_mechanics (F_MC instances)
   std::vector<double> mc_host;             // [n][mech_host_w()] inertia, armature, stiffness, springref every environment sees while d_mech exists (in double)
   bool mc_act = false;                     // the actuator rows were allocated by the mechanics setter (model values), and no actuator call has written them since
+  real *d_ct = nullptr;                    // A.contact: [n][CONTACT_W] per-environment contact softness, allocated by the first cassie_batch_set_env_contact (F_CT instances)
+  std::vector<double> ct_host;             // [n][ngeom][8] solref, solimp, solmix every environment sees while d_ct exists (in double: what get returns)
+  bool ct_mech = false;                    // the mechanics rows were allocated by the contact setter (model values), and no mechanics call has written them since
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -466,7 +484,8 @@ template <typename real> struct Batch : BatchBase {
           for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) {   // and their F_AC twins (per-environment actuators)
             CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
             CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }   // and their F_MC twins
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // and their F_MC twins
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }   // and their F_CT twins
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -818,6 +837,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     hm = src->hm;
     if (!rebuild_model()) return false;
+    if (!src->d_ct && !clear_env_contact()) return false;   // likewise the contact rows and the mechanics rows their setter allocated
     if (!src->d_mech && !clear_env_mechanics()) return false;   // likewise the mechanics rows and the actuator rows their setter allocated
     if (!src->d_act && !clear_env_actuators()) return false;   // likewise the actuator rows and the offset rows their setter allocated
     if (!src->d_bpos && !clear_env_body_pos()) return false;   // before the constant rows are copied: clearing drops rows the offset setter allocated
@@ -846,6 +866,13 @@ template <typename real> struct Batch : BatchBase {
       if (!d_mech) CUDA_OK(cudaMalloc(&d_mech, sizeof(real) * n * MECH_W));
       CUDA_OK(cudaMemcpy(d_mech, src->d_mech, sizeof(real) * n * MECH_W, cudaMemcpyDeviceToDevice));
       A.mech = d_mech;
+    }
+    if (src->d_ct) {   // likewise the contact rows (the mechanics rows came just now)
+      ct_host = src->ct_host; ct_mech = src->ct_mech;
+      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
+      if (!d_ct) CUDA_OK(cudaMalloc(&d_ct, sizeof(real) * n * CONTACT_W));
+      CUDA_OK(cudaMemcpy(d_ct, src->d_ct, sizeof(real) * n * CONTACT_W, cudaMemcpyDeviceToDevice));
+      A.contact = d_ct;
     }
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
@@ -1189,6 +1216,15 @@ template <typename real> struct Batch : BatchBase {
     A.mech = d_mech;
     return true;
   }
+  void model_mech_rows(std::vector<real> &all) {   // the mirror and the rows holding the model's values in every environment (a non-hinge dof's slots too, though the kernel reads the block there)
+    const int w = mech_host_w();
+    mc_host.resize((size_t)n * w); all.assign((size_t)n * MECH_W, real(0));
+    for (int e = 0; e < n; e++) {
+      real *r = &all[(size_t)e * MECH_W];
+      for (int k = 0; k < w; k++) { mc_host[(size_t)e * w + k] = block_mech(k); const int sl = mech_slot(k); if (sl >= 0) r[sl] = (real)block_mech(k); }
+      for (int i = 0; i < h_model_copy.nv; i++) { const int j = hm.dof_jntid[i]; r[MC_STIFF + i] = (real)hm.jnt_stiffness[j]; r[MC_SPRING + i] = (real)hm.qpos_spring[hm.jnt_qposadr[j]]; }
+    }
+  }
   bool set_env_mechanics(const double *inertia, const double *armature, const double *stiffness, const double *springref, const unsigned char *mask) override {
     const std::string verb = "cassie_batch_set_env_mechanics";
     const std::string why = env_mechanics_check(hm, n, h_model_copy.xb, h_model_copy.nv, inertia, armature, stiffness, springref, mask);   // every masked value first
@@ -1197,16 +1233,11 @@ template <typename real> struct Batch : BatchBase {
       if (!set_env_actuators(nullptr, nullptr, nullptr, nullptr)) return false;
       mc_act = true;
     }
+    ct_mech = false;   // the rows are the caller's now, also when the contact setter allocated them
     const int w = mech_host_w(), nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
     std::vector<real> all;
-    if (!d_mech) {   // the first call: every environment starts from the model's values (a non-hinge dof's slots too, though the kernel reads the block there)
-      mc_host.resize((size_t)n * w); all.assign((size_t)n * MECH_W, real(0));
-      for (int e = 0; e < n; e++) {
-        real *r = &all[(size_t)e * MECH_W];
-        for (int k = 0; k < w; k++) { mc_host[(size_t)e * w + k] = block_mech(k); const int sl = mech_slot(k); if (sl >= 0) r[sl] = (real)block_mech(k); }
-        for (int i = 0; i < h_model_copy.nv; i++) { const int j = hm.dof_jntid[i]; r[MC_STIFF + i] = (real)hm.jnt_stiffness[j]; r[MC_SPRING + i] = (real)hm.qpos_spring[hm.jnt_qposadr[j]]; }
-      }
-    } else if (!pull_mech(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    if (!d_mech) model_mech_rows(all);   // the first call: every environment starts from the model's values
+    else if (!pull_mech(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
     const double *part[4] = {inertia, armature, stiffness, springref};
     const int off[5] = {0, nb3, nb3 + nv, nb3 + nv + nj, w};
     for (int e = 0; e < n; e++) {
@@ -1243,13 +1274,111 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
-  // back to the model's values and the instances that ran before (which drops the actuator rows too when this setter brought them)
+  // back to the model's values and the instances that ran before (which drops the actuator rows too when this setter brought them).  A batch with contact
+  // rows keeps mechanics rows, holding the model's values again.
   bool clear_env_mechanics() override {
+    if (d_ct) { std::vector<real> all; model_mech_rows(all); ct_mech = true; return push_mech(all); }
     mc_host.clear();
     if (!d_mech) return true;
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaFree(d_mech)); d_mech = nullptr; A.mech = nullptr;
     if (mc_act) { mc_act = false; return clear_env_actuators(); }
+    return true;
+  }
+  // ---- per-environment contact softness (ground stiffness, damping and impedance: sim-to-real randomisation): MuJoCo's geom_solref, geom_solimp and
+  // geom_solmix per collision geom and environment, mixed per contact row by the F_CT instances' constraint stage.  Those instances are the F_CT twins of
+  // the F_MC ones, so a batch with contact rows carries mechanics rows too: when it has none, the setter allocates them holding the model's values (and
+  // actuator, offset and constant rows with them, as the mechanics setter does); clear drops them again unless a mechanics call has written them since.
+  // The device rows are what the environments run with, and the mirror keeps the doubles the verb was last given.
+  int ct_slot(int g) const { return g < 256 && geom_dev[g] >= 0 && geom_dev[g] < MGT ? geom_dev[g] : -1; }   // the device geom of host geom g, or -1: no contact
+  static int ct_field(int f) { return f < 2 ? CT_SOLREF + f : (f < 7 ? CT_SOLIMP + f - 2 : CT_SOLMIX); }   // mirror field f (solref 2, solimp 5, solmix 1) -> slot offset
+  double model_ct(int g, int f) const { return f < 2 ? hm.geom_solref[2 * g + f] : (f < 7 ? hm.geom_solimp[5 * g + f - 2] : hm.geom_solmix[g]); }
+  void model_ct_rows(std::vector<real> &all) {   // the mirror and the rows holding the model's values in every environment
+    const int ng = hm.ngeom;
+    ct_host.resize((size_t)n * ng * CT_SLOT); all.assign((size_t)n * CONTACT_W, real(0));
+    for (int e = 0; e < n; e++) for (int g = 0; g < ng; g++) {
+      const int s = ct_slot(g);
+      for (int f = 0; f < CT_SLOT; f++) {
+        ct_host[((size_t)e * ng + g) * CT_SLOT + f] = model_ct(g, f);
+        if (s >= 0) all[(size_t)e * CONTACT_W + CT_SLOT * s + ct_field(f)] = (real)model_ct(g, f);
+      }
+    }
+  }
+  bool pull_ct(std::vector<real> &all) {
+    all.assign((size_t)n * CONTACT_W, real(0));
+    if (!d_ct) return true;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemcpyAsync(all.data(), d_ct, sizeof(real) * n * CONTACT_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  bool push_ct(const std::vector<real> &all) {
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    if (!d_ct) CUDA_OK(cudaMalloc(&d_ct, sizeof(real) * n * CONTACT_W));
+    CUDA_OK(cudaMemcpy(d_ct, all.data(), sizeof(real) * n * CONTACT_W, cudaMemcpyHostToDevice));
+    A.contact = d_ct;
+    return true;
+  }
+  bool set_env_contact(const double *solref, const double *solimp, const double *solmix, const unsigned char *mask) override {
+    const std::string verb = "cassie_batch_set_env_contact";
+    const std::string why = env_contact_check(hm, n, geom_dev, solref, solimp, solmix, mask);   // every masked value first
+    if (!why.empty()) { set_err(verb + ": " + why); return false; }
+    if (!d_mech) {   // the F_CT instances read mechanics rows: the model's values, dropped again by clear unless a mechanics call writes them
+      if (!set_env_mechanics(nullptr, nullptr, nullptr, nullptr, nullptr)) return false;
+      ct_mech = true;
+    }
+    const int ng = hm.ngeom;
+    std::vector<real> all;
+    if (!d_ct) model_ct_rows(all);   // the first call: every environment starts from the model's values
+    else if (!pull_ct(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    const double *part[3] = {solref, solimp, solmix};
+    const int off[4] = {0, 2, 7, 8};
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      for (int g = 0; g < ng; g++) {
+        const int s = ct_slot(g); if (s < 0) continue;   // no collision slot: never in contact, the entry is ignored
+        for (int p = 0; p < 3; p++) {
+          if (!part[p]) continue;
+          const int cnt = off[p + 1] - off[p];
+          for (int i = 0; i < cnt; i++) {
+            const double v = part[p][((size_t)e * ng + g) * cnt + i]; const int f = off[p] + i;
+            ct_host[((size_t)e * ng + g) * CT_SLOT + f] = v;
+            all[(size_t)e * CONTACT_W + CT_SLOT * s + ct_field(f)] = (real)v;
+          }
+        }
+      }
+    }
+    return push_ct(all);
+  }
+  // what every environment runs with: a value the device row still holds as the verb stored it is reported as the verb was given it, one written on the
+  // device from the row; geoms without a collision slot report the model's values
+  bool get_env_contact(double *solref, double *solimp, double *solmix) override {
+    const int ng = hm.ngeom;
+    std::vector<real> all;
+    if (!pull_ct(all)) return false;
+    double *part[3] = {solref, solimp, solmix};
+    const int off[4] = {0, 2, 7, 8};
+    for (int e = 0; e < n; e++) for (int g = 0; g < ng; g++) {
+      const int s = ct_slot(g);
+      for (int p = 0; p < 3; p++) {
+        if (!part[p]) continue;
+        const int cnt = off[p + 1] - off[p];
+        for (int i = 0; i < cnt; i++) {
+          const int f = off[p] + i;
+          double v = model_ct(g, f);
+          if (d_ct && s >= 0) { const real dv = all[(size_t)e * CONTACT_W + CT_SLOT * s + ct_field(f)]; const double a = ct_host[((size_t)e * ng + g) * CT_SLOT + f]; v = dv == (real)a ? a : (double)dv; }
+          part[p][((size_t)e * ng + g) * cnt + i] = v;
+        }
+      }
+    }
+    return true;
+  }
+  // back to the model's values and the instances that ran before (which drops the mechanics rows too when this setter brought them)
+  bool clear_env_contact() override {
+    ct_host.clear();
+    if (!d_ct) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_ct)); d_ct = nullptr; A.contact = nullptr;
+    if (ct_mech) { ct_mech = false; return clear_env_mechanics(); }
     return true;
   }
   // ---- the controller-stage state: the delay line, the encoders' filters (views of the cst / dfilt rows; snapshots carry them)
@@ -1457,7 +1586,7 @@ template <typename real> struct Batch : BatchBase {
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1525,7 +1654,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -1609,7 +1738,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
-  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W;
+  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -2042,6 +2171,11 @@ int cassie_batch_set_env_mechanics(cassie_batch_t *b, const double *inertia, con
   return b->impl->set_env_mechanics(inertia, armature, stiffness, springref, mask) ? 0 : -1; }
 int cassie_batch_get_env_mechanics(cassie_batch_t *b, double *inertia, double *armature, double *stiffness, double *springref) { return b->impl->get_env_mechanics(inertia, armature, stiffness, springref) ? 0 : -1; }
 int cassie_batch_clear_env_mechanics(cassie_batch_t *b) { return b->impl->clear_env_mechanics() ? 0 : -1; }
+// per-environment contact softness (solref, solimp, solmix per collision geom); see include/cassie_b200.h
+int cassie_batch_set_env_contact(cassie_batch_t *b, const double *solref, const double *solimp, const double *solmix, const unsigned char *mask) {
+  return b->impl->set_env_contact(solref, solimp, solmix, mask) ? 0 : -1; }
+int cassie_batch_get_env_contact(cassie_batch_t *b, double *solref, double *solimp, double *solmix) { return b->impl->get_env_contact(solref, solimp, solmix) ? 0 : -1; }
+int cassie_batch_clear_env_contact(cassie_batch_t *b) { return b->impl->clear_env_contact() ? 0 : -1; }
 int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) { return b->impl->get_actuator_state(torque_delay, drive_filter, joint_x, joint_y) ? 0 : -1; }
 int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) {
   return b->impl->set_actuator_state(torque_delay, drive_filter, joint_x, joint_y, mask) ? 0 : -1; }

@@ -174,6 +174,44 @@ inline std::string env_mechanics_check(const HostModel &m, int n, int xb, int nv
   return std::string();
 }
 
+// cassie_batch_set_env_contact's check of every masked value, before anything changes: an empty reason, else the first refusal, naming the environment,
+// the geom and the field.  Refused: a non-finite value; a solref in neither MuJoCo form -- standard (timeconst > 0, dampratio > 0) or direct (stiffness
+// <= 0, damping <= 0); a solimp outside MuJoCo's documented ranges 0 < dmin < 1, 0 < dmax < 1, width >= 0, 0 < midpoint < 1, power >= 1 (inside them the
+// impedance and R = (1 - imp) dA / imp stay finite); a negative solmix.  Geoms without a collision slot (geom_dev < 0) never make contact: their entries
+// are not looked at.  solref [n][ngeom][2], solimp [n][ngeom][5], solmix [n][ngeom]; null parts are not checked (kept)
+inline std::string env_contact_check(const HostModel &m, int n, const int *geom_dev, const double *solref, const double *solimp, const double *solmix,
+                                     const unsigned char *mask) {
+  static const char *imp_name[5] = {"dmin", "dmax", "width", "midpoint", "power"};
+  const int ng = m.ngeom;
+  auto geom = [&](int g) { return (size_t)g < m.names_geom.size() && !m.names_geom[g].empty() ? m.names_geom[g] : std::to_string(g); };   // unnamed: the index
+  for (int e = 0; e < n; e++) {
+    if (mask && !mask[e]) continue;
+    for (int g = 0; g < ng; g++) {
+      if (g >= 256 || geom_dev[g] < 0 || geom_dev[g] >= MGT) continue;
+      const std::string at = "environment " + std::to_string(e) + ", geom " + geom(g) + ": ";
+      if (solref) {
+        const double *r = solref + ((size_t)e * ng + g) * 2;
+        if (!std::isfinite(r[0]) || !std::isfinite(r[1])) return at + "geom_solref is not finite";
+        if (!((r[0] > 0 && r[1] > 0) || (r[0] <= 0 && r[1] <= 0)))
+          return at + "geom_solref must be standard (timeconst > 0, dampratio > 0) or direct (stiffness <= 0, damping <= 0), not mixed";
+      }
+      if (solimp) {
+        const double *s = solimp + ((size_t)e * ng + g) * 5;
+        for (int k = 0; k < 5; k++) if (!std::isfinite(s[k])) return at + "geom_solimp[" + std::to_string(k) + "] (" + imp_name[k] + ") is not finite";
+        for (int k : {0, 1, 3}) if (!(s[k] > 0 && s[k] < 1)) return at + "geom_solimp[" + std::to_string(k) + "] (" + imp_name[k] + ") must be in (0, 1)";
+        if (!(s[2] >= 0)) return at + "geom_solimp[2] (width) must be >= 0";
+        if (!(s[4] >= 1)) return at + "geom_solimp[4] (power) must be >= 1";
+      }
+      if (solmix) {
+        const double x = solmix[(size_t)e * ng + g];
+        if (!std::isfinite(x)) return at + "geom_solmix is not finite";
+        if (x < 0) return at + "geom_solmix must be >= 0";
+      }
+    }
+  }
+  return std::string();
+}
+
 // one row of a batch's frame table (FT_W) for body (kind 0) or site (kind 1) `name`; its id, or -1 with a reason for an unknown name or kind
 template <typename real> int frame_table_row(const HostModel &m, const char *name, int kind, real *row, std::string &err) {
   for (int c = 0; c < FT_W; c++) row[c] = 0;

@@ -37,6 +37,7 @@ constexpr int F_TR = 32;  // per-environment terrain: the bank entry from a sele
 constexpr int F_BP = 64;  // per-environment body offsets: each body's position in its parent frame comes from a BP_W row instead of the model block (extended instances only)
 constexpr int F_AC = 128; // per-environment actuators: ctrlrange, no-load speed and torque delay of every motor come from an ACT_W row (with F_BP, extended instances only)
 constexpr int F_MC = 256; // per-environment mechanics: link inertia, rotor armature and hinge springs come from a MECH_W row (with F_BP | F_AC, extended instances only)
+constexpr int F_CT = 512; // per-environment contact softness: each contact row mixes solref / solimp from its geoms' CONTACT_W slots (with F_BP | F_AC | F_MC, extended only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -188,6 +189,13 @@ constexpr int AC_MAXDELAY = 6;   // the length of the delay line (cst CS_DELAY [
 // and free joints keep the model block's (the pelvis slides carry cassie_sim_hold's spring).  A model input like the CE rows.
 constexpr int MECH_W = 192;
 constexpr int MC_INERTIA = 0, MC_ARMATURE = 96, MC_STIFF = 128, MC_SPRING = 160;
+// per-environment contact softness (optional, cassie_batch_set_env_contact; F_CT instances): slot k describes device geom k (moving 0..15, static 16..31,
+// the numbering of CE_FRIC) with MuJoCo's geom_solref [2], geom_solimp [5] and geom_solmix [1].  The constraint stage mixes each contact row's pair from
+// the two slots by mj_contactParam's rule (the record's priority, else solmix); condim, margin, gap and friction stay the record's / CE_FRIC's.  Slots
+// without a collision geom are zero and never read.  A model input like the CE rows.
+constexpr int CT_SLOT = 8;
+constexpr int CONTACT_W = MGT * CT_SLOT;
+constexpr int CT_SOLREF = 0, CT_SOLIMP = 2, CT_SOLMIX = 7;
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

@@ -602,6 +602,33 @@ int cassie_batch_set_env_mechanics(cassie_batch_t *b, const double *inertia, con
                                    const unsigned char *mask);
 int cassie_batch_get_env_mechanics(cassie_batch_t *b, double *inertia, double *armature, double *stiffness, double *springref);
 int cassie_batch_clear_env_mechanics(cassie_batch_t *b);
+/* Per-environment contact softness (domain randomisation of how stiff and how damped the ground and the other contacts are): for each environment and
+ * each geom (host model numbering, ngeom from cassie_batch_ngeom)
+ *   solref [n][ngeom][2]: MuJoCo's geom_solref, standard form (timeconst, dampratio) or direct form (-stiffness, -damping);
+ *   solimp [n][ngeom][5]: MuJoCo's geom_solimp (dmin, dmax, width, midpoint, power);
+ *   solmix [n][ngeom]:    MuJoCo's geom_solmix, the weight of the geom's values when two geoms of equal priority mix.
+ * Each contact mixes its two geoms' values as mj_contactParam does: the geom of higher priority gives its values; otherwise solimp is mixed with
+ * mix = s1 / (s1 + s2) (0.5 when both solmix are below 1e-15, the other geom's values when one is), and solref too when both are in standard form, else
+ * solref is the elementwise min.  condim, margin, gap and the geom priorities stay the model's; friction per geom is cassie_batch_set_geom_friction's.
+ * Any of the three may be NULL (kept); mask [n] (or NULL: all) selects the environments that change.  The first call gives every environment the model's
+ * values.  0, or -1 with nothing changed (cassie_b200_last_error names the environment, the geom and the field) for a non-finite value, a solref in
+ * neither form (timeconst > 0 and dampratio > 0, or stiffness <= 0 and damping <= 0: mixed signs are refused), a solimp outside MuJoCo's documented
+ * ranges 0 < dmin < 1, 0 < dmax < 1, width >= 0, 0 < midpoint < 1, power >= 1, or a negative solmix.  Geoms without a collision slot (visual geoms,
+ * contype = conaffinity = 0) never make contact: their entries are accepted and ignored, and get reports the model's values for them (in MuJoCo,
+ * writing such a geom's solref is legal and has no effect).  A batch with contact rows runs the kernel instances that read them, which also read
+ * mechanics rows: without rows of its own the batch gets mechanics rows holding the model's values (and actuator, offset and constant rows through them,
+ * as cassie_batch_set_env_mechanics does) -- cassie_batch_clear_env_mechanics puts the model's values back instead of dropping the rows, and
+ * cassie_batch_clear_env_contact drops them unless a mechanics call has written them since.  The rows are model inputs: reset and snapshot restore
+ * leave them alone, cassie_sim_copy copies them, cassie_sim_step_pd_batch honours them.  The mj_setConst constants do not depend on them.  get: what
+ * every environment sees (the model's values without rows).  clear: back to the model's values and the kernel instances that ran before.  Device rows:
+ * cassie_batch_device_ptr(b, "contact"), [n][CONTACT_W = 256] in the batch precision: slot k (8 values: solref [2], solimp [5], solmix) is device geom
+ * k -- the collision geoms of moving bodies 0..15, then the static ones 16..31, in the order the model's candidate pairs first meet them --; slots with
+ * no collision geom behind them are zero and never read.  A write takes effect at the next launch, and the rows are what the verbs work on: a masked set
+ * changes the masked environments' rows only, get reports what the rows hold.  The kernel applies no clamps: a value outside the ranges above written
+ * through the device pointer gives unspecified physics, but no index is derived from the row, so it cannot reach memory outside it. */
+int cassie_batch_set_env_contact(cassie_batch_t *b, const double *solref, const double *solimp, const double *solmix, const unsigned char *mask);
+int cassie_batch_get_env_contact(cassie_batch_t *b, double *solref, double *solimp, double *solmix);
+int cassie_batch_clear_env_contact(cassie_batch_t *b);
 /* The controller-stage state of every environment, as the reference's cassie_sim_t holds it: the torque delay line torque_delay [n][10][6] (slot 0
  * newest), the drive encoders' integer FIR taps drive_filter [n][10][9], the joint encoders' IIR filters joint_x [n][6][4] and joint_y [n][6][3].
  * NULL parts are skipped; set changes masked environments only (mask NULL: all).  They are state: reset, snapshots and cassie_sim_copy carry them. */
@@ -610,7 +637,7 @@ int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_dela
                                     const unsigned char *mask);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
