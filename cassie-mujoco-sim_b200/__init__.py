@@ -678,6 +678,46 @@ class CassieBatch:
         if self._contact_lib().cassie_batch_clear_env_contact(self.h) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- per-environment applied forces (perturbation: pushes on any body, joint-space disturbance torques; state, as in mjData)
+    def _applied_lib(self):
+        L = self.L
+        if not getattr(L, '_applied_bound', False):
+            vp, dp = C.c_void_p, C.POINTER(C.c_double)
+            L.cassie_batch_set_applied_forces.argtypes = [vp, dp, dp, vp]
+            L.cassie_batch_get_applied_forces.argtypes = [vp, dp, dp]
+            L.cassie_batch_enable_applied_forces.argtypes = [vp, C.c_int]
+            for n in ('set_applied_forces', 'get_applied_forces', 'enable_applied_forces'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._applied_bound = True
+        return L
+
+    def _applied_shapes(self):
+        return (self.L.cassie_batch_nbody(self.h), 6), (self.nv,)
+
+    def set_applied_forces(self, xfrc=None, qfrc=None, mask=None):
+        """each environment's applied forces: xfrc [nbody, 6] or [n, nbody, 6] -- MuJoCo's xfrc_applied, force xyz and torque xyz in the world frame at the
+        body's centre of mass, model body order --, qfrc [nv] or [n, nv] -- qfrc_applied, the extra free body's dofs included.  A part left None is kept;
+        mask [n]: only the selected environments change.  A non-finite value raises, and nothing changes.  State: reset() zeroes both, clear_forces() the
+        body wrenches; snapshots carry them.  apply_force's slot adds to the rows."""
+        L = self._applied_lib()
+        a = [self._arr(v, np.float64, (self.n,) + sh) for v, sh in zip((xfrc, qfrc), self._applied_shapes())]
+        m = self._arr(mask, np.uint8, (self.n,))
+        if L.cassie_batch_set_applied_forces(self.h, *[None if v is None else self._dp(v) for v in a], None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def applied_forces(self):
+        """dict of xfrc [n, nbody, 6], qfrc [n, nv]: what the rows hold (zeros without rows)"""
+        L = self._applied_lib()
+        out = [np.zeros((self.n,) + sh) for sh in self._applied_shapes()]
+        if L.cassie_batch_get_applied_forces(self.h, *[self._dp(v) for v in out]) != 0:
+            raise RuntimeError(_last_error())
+        return dict(zip(('xfrc', 'qfrc'), out))
+
+    def enable_applied_forces(self, on=True):
+        """on: zeroed rows, for writing through torch_view('applied') only; off: drop the rows and their forces, back to the kernel instances that ran before"""
+        if self._applied_lib().cassie_batch_enable_applied_forces(self.h, 1 if on else 0) != 0:
+            raise RuntimeError(_last_error())
+
     def actuator_state(self):
         """dict of the controller-stage state: torque_delay [n, 10, 6] (slot 0 newest), drive_filter [n, 10, 9] int32, joint_x [n, 6, 4], joint_y [n, 6, 3]"""
         L = self._act_lib()
@@ -966,7 +1006,8 @@ class CassieBatch:
         in rad/s, delay[10], read at the next launch; set_env_actuators first; mechanics [n, 192]: body_inertia[32][3], armature[32], stiffness[32],
         qpos_spring[32] per main-tree dof (the springs of hinge dofs only are read), read at the next launch; set_env_mechanics first; contact [n, 256]:
         32 slots of 8 -- solref[2], solimp[5], solmix -- one per device collision geom (moving 0..15, static 16..31; unused slots zero), read at the next
-        launch; set_env_contact first).  set_frames /
+        launch; set_env_contact first; applied [n, 232]: xfrc_applied[32][6] in model body order, then qfrc_applied[40] by dof column (main tree 0..31,
+        the extra free body 32..37), read at the next launch; set_applied_forces or enable_applied_forces first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -976,7 +1017,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field == 'terrain':
             ts = '<i4'

@@ -50,6 +50,13 @@ MECHANICS_INSTANCES = [('f11c4', 'float', 1, 452), ('f11d7', 'float', 1, 471), (
 # kind, features in hex
 CONTACT_INSTANCES = [('f13c4', 'float', 1, 964), ('f13d7', 'float', 1, 983), ('d13d7', 'double', 1, 983), ('f13df', 'float', 1, 991), ('d13df', 'double', 1, 991),
                      ('f13ff', 'float', 1, 1023), ('d13ff', 'double', 1, 1023)]
+# per-environment applied forces (feature 1024 = F_XF; cassie_batch_set_applied_forces: xfrc_applied per body, qfrc_applied per dof).  The push workload
+# runs the plain kinds: f0404 / f2404 are the F_XF twins of f04 / f24 and run where those would.  Any other batch with applied rows runs the extended
+# kernel, which carries contact rows holding the model's values (and mechanics, actuator and offset rows through them): the chain twins, each the F_XF
+# twin of one CONTACT_INSTANCES entry (f13c4, f13d7 / d13d7, f13df / d13df, f13ff / d13ff); tag = precision, kind, features in hex
+APPLIED_INSTANCES = [('f0404', 'float', 0, 1028), ('f2404', 'float', 2, 1028),
+                     ('f17c4', 'float', 1, 1988), ('f17d7', 'float', 1, 2007), ('d17d7', 'double', 1, 2007), ('f17df', 'float', 1, 2015), ('d17df', 'double', 1, 2015),
+                     ('f17ff', 'float', 1, 2047), ('d17ff', 'double', 1, 2047)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -83,7 +90,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES + APPLIED_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

@@ -36,6 +36,8 @@ CASSIE_STEP_ENTRY(f144) CASSIE_STEP_ENTRY(f157) CASSIE_STEP_ENTRY(d157) CASSIE_S
 CASSIE_STEP_ENTRY(f1c4) CASSIE_STEP_ENTRY(f1d7) CASSIE_STEP_ENTRY(d1d7) CASSIE_STEP_ENTRY(f1df) CASSIE_STEP_ENTRY(d1df) CASSIE_STEP_ENTRY(f1ff) CASSIE_STEP_ENTRY(d1ff)
 CASSIE_STEP_ENTRY(f11c4) CASSIE_STEP_ENTRY(f11d7) CASSIE_STEP_ENTRY(d11d7) CASSIE_STEP_ENTRY(f11df) CASSIE_STEP_ENTRY(d11df) CASSIE_STEP_ENTRY(f11ff) CASSIE_STEP_ENTRY(d11ff)
 CASSIE_STEP_ENTRY(f13c4) CASSIE_STEP_ENTRY(f13d7) CASSIE_STEP_ENTRY(d13d7) CASSIE_STEP_ENTRY(f13df) CASSIE_STEP_ENTRY(d13df) CASSIE_STEP_ENTRY(f13ff) CASSIE_STEP_ENTRY(d13ff)
+CASSIE_STEP_ENTRY(f0404) CASSIE_STEP_ENTRY(f2404)
+CASSIE_STEP_ENTRY(f17c4) CASSIE_STEP_ENTRY(f17d7) CASSIE_STEP_ENTRY(d17d7) CASSIE_STEP_ENTRY(f17df) CASSIE_STEP_ENTRY(d17df) CASSIE_STEP_ENTRY(f17ff) CASSIE_STEP_ENTRY(d17ff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -45,6 +47,19 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_XF) {   // per-environment applied forces: the plain twins of f04 / f24 where those would run, else the F_XF twins of the F_CT instances by their rule
+    const bool dbl = std::is_same<real, double>::value;
+    if (inst != 1) {   // null: the batch runs the extended kind (step_range)
+      if (dbl || (feat & ~F_XF) != F_BOX) return nullptr;
+      if (compiled_feat) *compiled_feat = F_BOX | F_XF;
+      return inst == 2 ? cassie_step_entry_f2404() : cassie_step_entry_f0404();
+    }
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF; return dbl ? cassie_step_entry_d17ff() : cassie_step_entry_f17ff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF; return dbl ? cassie_step_entry_d17df() : cassie_step_entry_f17df(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF; return cassie_step_entry_f17c4(); }
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF;
+    return dbl ? cassie_step_entry_d17d7() : cassie_step_entry_f17d7();
+  }
   if (feat & F_CT) {   // per-environment contact softness: the F_CT twins of the F_MC instances, by the same rule (a batch with contact rows always has mechanics rows)
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value;
@@ -247,16 +262,17 @@ __global__ void copy_rows_kernel(T *__restrict__ dst, const T *__restrict__ src,
 // device-resident copy of every per-environment row array of a batch (cassie_state_t / cassie_batch_get_state); it owns its memory and carries its own
 // sizes, so it can be copied, restored into any batch of the same shape and freed without the batch it was taken from
 struct Snap {
-  enum { R_QPOS, R_QVEL, R_QACC, R_CST, R_XFRC, R_OBS, R_DFILT, R_EST, R_AUX, NROWS };
-  int device = 0, n = 0, esz = 4, qw = 0, vw = 0; bool has_est = false, has_aux = false;
-  void *rows[NROWS] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  enum { R_QPOS, R_QVEL, R_QACC, R_CST, R_XFRC, R_OBS, R_DFILT, R_EST, R_AUX, R_APPL, NROWS };
+  int device = 0, n = 0, esz = 4, qw = 0, vw = 0; bool has_est = false, has_aux = false, has_appl = false;   // has_appl: the applied-force rows
+  void *rows[NROWS] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  bool has(int r) const { return !((r == R_EST && !has_est) || (r == R_AUX && !has_aux) || (r == R_APPL && !has_appl)); }   // the optional rows it holds
   // the frame rows [n][frame_list.size() / 2][FRAME_W] of the batch, with its frame list ((kind, id) pairs); restored only into a batch with the same list
   void *frames = nullptr; std::vector<int> frame_list;
   size_t frame_bytes() const { return (size_t)n * (frame_list.size() / 2) * FRAME_W * esz; }
   // the acceleration rows [n][acc_width(count)] of the batch (mjData's qacc and the cacc of its frames), if it had them; restored like the frame rows
   void *acc = nullptr;
   size_t acc_bytes() const { return (size_t)n * acc_width((int)(frame_list.size() / 2)) * esz; }
-  int width(int r) const { const int w[NROWS] = {qw, vw, vw, CST_W, XFRC_W, OBS_W, DFILT_W, EST_W, AUX_W}; return w[r]; }
+  int width(int r) const { const int w[NROWS] = {qw, vw, vw, CST_W, XFRC_W, OBS_W, DFILT_W, EST_W, AUX_W, APPLIED_W}; return w[r]; }
   int elem(int r) const { return r == R_DFILT ? 4 : (r == R_EST ? 8 : esz); }
   size_t bytes(int r) const { return (size_t)n * width(r) * elem(r); }
 };
@@ -264,14 +280,14 @@ static void snap_delete(Snap *k) { if (!k) return; cudaSetDevice(k->device); for
 static Snap *snap_new(int device, int n, int esz, int qw, int vw) {
   if (cudaSetDevice(device) != cudaSuccess) return nullptr;
   Snap *k = new Snap(); k->device = device; k->n = n; k->esz = esz; k->qw = qw; k->vw = vw;
-  for (int r = 0; r < Snap::NROWS; r++) if (r != Snap::R_EST && r != Snap::R_AUX && cudaMalloc(&k->rows[r], k->bytes(r)) != cudaSuccess) { snap_delete(k); return nullptr; }
+  for (int r = 0; r < Snap::NROWS; r++) if (k->has(r) && cudaMalloc(&k->rows[r], k->bytes(r)) != cudaSuccess) { snap_delete(k); return nullptr; }
   return k;
 }
 static bool snap_clone_into(Snap *d, const Snap *k) {   // same shape required
   if (d->n != k->n || d->esz != k->esz || d->qw != k->qw || d->vw != k->vw || cudaSetDevice(d->device) != cudaSuccess) return false;
-  d->has_est = k->has_est; d->has_aux = k->has_aux;
+  d->has_est = k->has_est; d->has_aux = k->has_aux; d->has_appl = k->has_appl;
   for (int r = 0; r < Snap::NROWS; r++) {
-    if ((r == Snap::R_EST && !k->has_est) || (r == Snap::R_AUX && !k->has_aux)) continue;
+    if (!k->has(r)) continue;
     if (!d->rows[r] && cudaMalloc(&d->rows[r], d->bytes(r)) != cudaSuccess) return false;
     if (cudaMemcpy(d->rows[r], k->rows[r], k->bytes(r), cudaMemcpyDefault) != cudaSuccess) return false;
   }
@@ -351,6 +367,12 @@ struct BatchBase {
   virtual bool set_env_contact(const double *solref, const double *solimp, const double *solmix, const unsigned char *mask) = 0;
   virtual bool get_env_contact(double *solref, double *solimp, double *solmix) = 0;
   virtual bool clear_env_contact() = 0;
+  // per-environment applied forces (F_XF instances; state): xfrc [n][nbody][6], qfrc [n][nv], either may be null (kept); only masked environments
+  // change; checked as a whole before anything changes.  enable(false) drops the rows; clear_applied_xfrc zeroes the body wrenches of every environment
+  virtual bool set_applied_forces(const double *xfrc, const double *qfrc, const unsigned char *mask) = 0;
+  virtual bool get_applied_forces(double *xfrc, double *qfrc) = 0;
+  virtual bool enable_applied_forces(bool on) = 0;
+  virtual bool clear_applied_xfrc() = 0;
   // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
   // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
   virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
@@ -411,9 +433,11 @@ template <typename real> struct Batch : BatchBase {
   real *d_ct = nullptr;                    // A.contact: [n][CONTACT_W] per-environment contact softness, allocated by the first cassie_batch_set_env_contact (F_CT instances)
   std::vector<double> ct_host;             // [n][ngeom][8] solref, solimp, solmix every environment sees while d_ct exists (in double: what get returns)
   bool ct_mech = false;                    // the mechanics rows were allocated by the contact setter (model values), and no mechanics call has written them since
+  real *d_app = nullptr;                   // A.applied: [n][APPLIED_W] per-environment applied forces (state), allocated by the first applied-force verb (F_XF instances)
+  bool xf_ct = false;                      // the contact rows were allocated for the chain twin (model values), and no contact call has written them since
   ~Batch() override {
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -485,7 +509,10 @@ template <typename real> struct Batch : BatchBase {
             CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
             CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
             CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // and their F_MC twins
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }   // and their F_CT twins
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // and their F_CT twins
+            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }   // and their F_XF twins
+        if (ext != 1 && step_entry<real>(ext, feat | F_XF))   // the plain F_XF twins (applied forces), where this model runs f04 / f24
+          CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, feat | F_XF), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -500,6 +527,7 @@ template <typename real> struct Batch : BatchBase {
       std::vector<real> buf((size_t)n * CST_W); std::vector<int> ibuf((size_t)n * DFILT_W, 0);
       auto fill = [&](real *dst, const std::vector<real> &row, int w) -> bool { for (int e = 0; e < n; e++) memcpy(&buf[(size_t)e * w], row.data(), sizeof(real) * w); CUDA_OK(cudaMemcpyAsync(dst, buf.data(), sizeof(real) * n * w, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream)); return true; };
       if (!fill(A.qpos, qpos, QW) || !fill(A.qvel, qvel, VW) || !fill(A.qacc_ws, qa, VW) || !fill(A.cst, cst, CST_W) || !fill(A.xfrc, xf, XFRC_W)) return false;
+      if (d_app) CUDA_OK(cudaMemsetAsync(d_app, 0, sizeof(real) * n * APPLIED_W, stream));   // applied forces are state, as in mjData
       CUDA_OK(cudaMemcpyAsync(A.dfilt, ibuf.data(), sizeof(int) * n * DFILT_W, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream));
       return step(0, 1);
     }
@@ -507,6 +535,7 @@ template <typename real> struct Batch : BatchBase {
     if (!upload_mask(mask)) return false;
     if (!fill_masked(A.qpos, qpos.data(), QW) || !fill_masked(A.qvel, qvel.data(), VW) || !fill_masked(A.qacc_ws, qa.data(), VW) || !fill_masked(A.cst, cst.data(), CST_W) ||
         !fill_masked(A.xfrc, xf.data(), XFRC_W) || !fill_masked(A.dfilt, df.data(), DFILT_W)) return false;
+    if (d_app) { const std::vector<real> zero(APPLIED_W, real(0)); if (!fill_masked(d_app, zero.data(), APPLIED_W)) return false; }
     return step_masked(1);
   }
   bool upload_mask(const unsigned char *mask) {
@@ -770,13 +799,13 @@ template <typename real> struct Batch : BatchBase {
   // ---- snapshots (the Snap object owns its device memory and knows its own sizes: it may outlive this batch)
   Snap *snap_alloc() override { Snap *k = snap_new(device, n, (int)sizeof(real), QW, VW); if (!k) set_err("snapshot: out of device memory"); return k; }
   bool snap_compatible(const Snap *k) { if (k && k->n == n && k->esz == (int)sizeof(real) && k->qw == QW && k->vw == VW) return true; set_err("snapshot: taken from a batch of another size, precision or model"); return false; }
-  void *snap_src(int r) { void *t[Snap::NROWS] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux}; return t[r]; }
+  void *snap_src(int r) { void *t[Snap::NROWS] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux, d_app}; return t[r]; }
   bool snap_get(Snap *k) override {
     if (!snap_compatible(k)) return false;
     CUDA_OK(cudaSetDevice(device));
-    k->has_est = A.est != nullptr; k->has_aux = A.aux != nullptr;
+    k->has_est = A.est != nullptr; k->has_aux = A.aux != nullptr; k->has_appl = d_app != nullptr;
     for (int r = 0; r < Snap::NROWS; r++) {
-      if ((r == Snap::R_EST && !k->has_est) || (r == Snap::R_AUX && !k->has_aux)) continue;
+      if (!k->has(r)) continue;
       if (!k->rows[r]) CUDA_OK(cudaMalloc(&k->rows[r], k->bytes(r)));
       CUDA_OK(cudaMemcpyAsync(k->rows[r], snap_src(r), k->bytes(r), cudaMemcpyDeviceToDevice, stream));
     }
@@ -793,8 +822,13 @@ template <typename real> struct Batch : BatchBase {
     if (mask) { if (!upload_mask(mask)) return false; dm = d_mask; }
     if (k->has_est && !A.est && !enable_estimator_device(true)) return false;
     if (!k->has_est && A.est && !reset_estimator_device(mask)) return false;   // the snapshot was taken before the estimator ran: it starts afresh
+    if (k->has_appl && !d_app && !enable_applied_forces(true)) return false;   // likewise the applied-force rows: allocated by a snapshot that has them,
+    if (!k->has_appl && d_app) {                                               // zeroed by one taken without them
+      if (!dm) CUDA_OK(cudaMemsetAsync(d_app, 0, sizeof(real) * n * APPLIED_W, stream));
+      else { const std::vector<real> zero(APPLIED_W, real(0)); if (!fill_masked(d_app, zero.data(), APPLIED_W)) return false; }
+    }
     for (int r = 0; r < Snap::NROWS; r++) {
-      if ((r == Snap::R_EST && !k->has_est) || (r == Snap::R_AUX && (!k->has_aux || !A.aux))) continue;
+      if (!k->has(r) || (r == Snap::R_AUX && !A.aux)) continue;
       if (!dm) { CUDA_OK(cudaMemcpyAsync(snap_src(r), k->rows[r], k->bytes(r), cudaMemcpyDeviceToDevice, stream)); continue; }
       const int w = k->width(r);
       if (k->elem(r) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)snap_src(r), (const unsigned long long *)k->rows[r], w, dm, n);
@@ -868,7 +902,7 @@ template <typename real> struct Batch : BatchBase {
       A.mech = d_mech;
     }
     if (src->d_ct) {   // likewise the contact rows (the mechanics rows came just now)
-      ct_host = src->ct_host; ct_mech = src->ct_mech;
+      ct_host = src->ct_host; ct_mech = src->ct_mech; xf_ct = src->xf_ct;
       CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
       if (!d_ct) CUDA_OK(cudaMalloc(&d_ct, sizeof(real) * n * CONTACT_W));
       CUDA_OK(cudaMemcpy(d_ct, src->d_ct, sizeof(real) * n * CONTACT_W, cudaMemcpyDeviceToDevice));
@@ -1322,6 +1356,7 @@ template <typename real> struct Batch : BatchBase {
     const std::string verb = "cassie_batch_set_env_contact";
     const std::string why = env_contact_check(hm, n, geom_dev, solref, solimp, solmix, mask);   // every masked value first
     if (!why.empty()) { set_err(verb + ": " + why); return false; }
+    xf_ct = false;   // the rows are the caller's now, also when the chain twin's launch allocated them
     if (!d_mech) {   // the F_CT instances read mechanics rows: the model's values, dropped again by clear unless a mechanics call writes them
       if (!set_env_mechanics(nullptr, nullptr, nullptr, nullptr, nullptr)) return false;
       ct_mech = true;
@@ -1374,11 +1409,66 @@ template <typename real> struct Batch : BatchBase {
   }
   // back to the model's values and the instances that ran before (which drops the mechanics rows too when this setter brought them)
   bool clear_env_contact() override {
-    ct_host.clear();
+    ct_host.clear(); xf_ct = false;
     if (!d_ct) return true;
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaFree(d_ct)); d_ct = nullptr; A.contact = nullptr;
     if (ct_mech) { ct_mech = false; return clear_env_mechanics(); }
+    return true;
+  }
+  // ---- per-environment applied forces (pushes on any body, joint-space disturbances): MuJoCo's xfrc_applied and qfrc_applied per environment.  They are
+  // state, as in mjData: reset zeroes them, snapshots carry them.  The device rows are what the environments run with (a write through the device
+  // pointer takes effect at the next launch), so the verbs read them back and keep no mirror.  A batch with rows runs f0404 / f2404 where f04 / f24
+  // would run, else the chain twins, which read contact rows: step_range allocates those holding the model's values (xf_ct) when the batch has none.
+  int ap_col(int i) const { const int nvm = h_model_copy.nv; return i < nvm ? i : 32 + (i - nvm); }   // host dof i -> its column in AP_QFRC
+  bool enable_applied_forces(bool on) override {
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    if (on) {
+      if (!d_app) { CUDA_OK(cudaMalloc(&d_app, sizeof(real) * n * APPLIED_W)); CUDA_OK(cudaMemset(d_app, 0, sizeof(real) * n * APPLIED_W)); }
+      A.applied = d_app;
+      return true;
+    }
+    if (d_app) { CUDA_OK(cudaFree(d_app)); d_app = nullptr; A.applied = nullptr; }
+    if (xf_ct) return clear_env_contact();   // back to the instances that ran before (clear resets xf_ct)
+    return true;
+  }
+  bool set_applied_forces(const double *xfrc, const double *qfrc, const unsigned char *mask) override {
+    const int nb = hm.nbody, nv = hm.nv;
+    for (int e = 0; e < n; e++) {   // every masked value first
+      if (mask && !mask[e]) continue;
+      for (int b = 0; xfrc && b < nb; b++) for (int k = 0; k < 6; k++) if (!std::isfinite(xfrc[((size_t)e * nb + b) * 6 + k])) {
+        const std::string name = (size_t)b < hm.names_body.size() && !hm.names_body[b].empty() ? hm.names_body[b] : std::to_string(b);
+        set_err("cassie_batch_set_applied_forces: environment " + std::to_string(e) + ", body " + name + ": xfrc_applied[" + std::to_string(k) + "] is not finite"); return false; }
+      for (int i = 0; qfrc && i < nv; i++) if (!std::isfinite(qfrc[(size_t)e * nv + i])) {
+        set_err("cassie_batch_set_applied_forces: environment " + std::to_string(e) + ", dof " + std::to_string(i) + ": qfrc_applied is not finite"); return false; }
+    }
+    if (!enable_applied_forces(true)) return false;   // the first call: zeroed rows
+    std::vector<real> all((size_t)n * APPLIED_W);
+    CUDA_OK(cudaMemcpy(all.data(), d_app, sizeof(real) * n * APPLIED_W, cudaMemcpyDeviceToHost));   // unmasked environments keep what their rows hold
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      real *r = &all[(size_t)e * APPLIED_W];
+      if (xfrc) for (int b = 0; b < nb; b++) for (int k = 0; k < 6; k++) r[AP_XFRC + 6 * b + k] = (real)xfrc[((size_t)e * nb + b) * 6 + k];
+      if (qfrc) for (int i = 0; i < nv; i++) r[AP_QFRC + ap_col(i)] = (real)qfrc[(size_t)e * nv + i];
+    }
+    CUDA_OK(cudaMemcpy(d_app, all.data(), sizeof(real) * n * APPLIED_W, cudaMemcpyHostToDevice));
+    return true;
+  }
+  bool get_applied_forces(double *xfrc, double *qfrc) override {   // what the rows hold; zeros without rows
+    const int nb = hm.nbody, nv = hm.nv;
+    std::vector<real> all((size_t)n * APPLIED_W, real(0));
+    if (d_app) { CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaMemcpyAsync(all.data(), d_app, sizeof(real) * n * APPLIED_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
+    for (int e = 0; e < n; e++) {
+      const real *r = &all[(size_t)e * APPLIED_W];
+      if (xfrc) for (int b = 0; b < nb; b++) for (int k = 0; k < 6; k++) xfrc[((size_t)e * nb + b) * 6 + k] = (double)r[AP_XFRC + 6 * b + k];
+      if (qfrc) for (int i = 0; i < nv; i++) qfrc[(size_t)e * nv + i] = (double)r[AP_QFRC + ap_col(i)];
+    }
+    return true;
+  }
+  bool clear_applied_xfrc() override {   // cassie_batch_clear_forces: MuJoCo's xfrc_applied of every environment; qfrc_applied stays (src/cassiemujoco.c:1969-1972)
+    if (!d_app) return true;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemset2DAsync(d_app + AP_XFRC, sizeof(real) * APPLIED_W, 0, sizeof(real) * AP_QFRC, n, stream)); CUDA_OK(cudaStreamSynchronize(stream));
     return true;
   }
   // ---- the controller-stage state: the delay line, the encoders' filters (views of the cst / dfilt rows; snapshots carry them)
@@ -1580,13 +1670,17 @@ template <typename real> struct Batch : BatchBase {
     A.nsub = nsub_override;
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
-    const int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    if (A.applied) {   // applied forces: a plain twin where f04 / f24 would run, else the chain twin, which reads contact rows (the model's values when none were set)
+      if (ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF)) ext = 1;
+      if (ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }
+    }
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1655,6 +1749,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
+    if (!strcmp(f, "applied")) return d_app;
     return nullptr;
   }
   bool get_counters(int *out) override {
@@ -1682,6 +1777,7 @@ static_assert(CASSIE_RAY_MAX == RAY_MAX && CASSIE_RAY_SLOT == RAY_SLOT && CASSIE
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
+static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
 static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
 struct cassie_batch { BatchBase *impl; std::vector<double> obs, radio; };
 struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[64], qvel_dev[64], time_dev, aux[AUX_W]; std::vector<float> hfield, hfield_dev; std::string path; double timestep = 0, timestep_dev = 0;
@@ -1699,7 +1795,10 @@ struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[6
   // the controller-stage state lent out by cassie_sim_joint_filter / drive_filter / ctrl: host mirrors laid out as joint_filter_t[6] (x[4], y[3]),
   // drive_filter_t[10] (int x[9]) and mjData's ctrl[nu].  Refreshed after every launch once one was lent; the filter mirrors are uploaded before the
   // next launch when they were written, ctrl is read-only in effect (the next step overwrites it, as cassie_motor_data does in the reference)
-  double jfilt[6][7], jfilt_dev[6][7], ctrl[MU]; int dfilt[10][9], dfilt_dev[10][9]; bool act_lent = false, ctrl_zero = false; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
+  double jfilt[6][7], jfilt_dev[6][7], ctrl[MU]; int dfilt[10][9], dfilt_dev[10][9]; bool act_lent = false, ctrl_zero = false;
+  // qfrc_applied lent out by cassie_sim_qfrc: a host mirror of the batch's applied-force row [nv] (empty until the first call), uploaded before the next
+  // launch when it was written, refreshed after every launch
+  std::vector<double> qfrc, qfrc_dev; };   // geom placement (stair boxes): host mirrors, the constant block is rebuilt when they change   // host mirrors of the model arrays handed out as borrowed pointers
 
 // cassie_state_t (include/cassiemujoco.h:434-463): a device-resident snapshot of one simulator's rows plus the host mirrors the reference hands out as
 // borrowed pointers (time, qpos, qvel); the snapshot is allocated by the first cassie_get_state, which also fixes the owning simulator's sizes
@@ -1738,7 +1837,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
-  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W;
+  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -1789,7 +1888,7 @@ int cassie_batch_apply_force(cassie_batch_t *b, const double *xfrc, const char *
   if (id <= 0) { set_err("cassie_batch_apply_force: unknown body (no-op)"); return -1; }
   return b->impl->set_xfrc(xfrc, id) ? 0 : -1;
 }
-void cassie_batch_clear_forces(cassie_batch_t *b) { b->impl->set_xfrc(nullptr, 0); }
+void cassie_batch_clear_forces(cassie_batch_t *b) { b->impl->set_xfrc(nullptr, 0); b->impl->clear_applied_xfrc(); }
 void cassie_batch_integrate_pos(cassie_batch_t *b) { b->impl->integrate(); }
 int cassie_batch_set_hfielddata(cassie_batch_t *b, const float *data, int n_terrains) { return b->impl->set_hfield(data, n_terrains) ? 0 : -1; }
 int cassie_batch_hfield_nrow(const cassie_batch_t *b) { return b->impl->hm.nhfield ? b->impl->hm.hfield_nrow[0] : 0; }
@@ -1837,6 +1936,7 @@ static void sim_pull(cassie_sim_t *c) {
   if (!c->acc.empty() && c->b->impl->get("acc", c->acc.data())) for (int i = 0; i < c->b->impl->hm.nv; i++) c->qacc[i] = c->acc[AC_QACC + i];
   memcpy(c->qpos_dev, c->qpos, sizeof c->qpos); memcpy(c->qvel_dev, c->qvel, sizeof c->qvel); c->time_dev = c->time;
   if (c->act_lent) sim_pull_act(c);
+  if (!c->qfrc.empty() && c->b->impl->get_applied_forces(nullptr, c->qfrc.data())) c->qfrc_dev = c->qfrc;
 }
 static void sim_lend_act(cassie_sim_t *c) { if (!c->act_lent) { c->act_lent = true; sim_pull_act(c); } }   // the first lend fills the mirrors
 static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote through the borrowed pointers
@@ -1862,6 +1962,7 @@ static void sim_push(cassie_sim_t *c) {  // upload whatever the caller wrote thr
     c->b->impl->set_actuator_state(nullptr, nullptr, jx, jy, nullptr); memcpy(c->jfilt_dev, c->jfilt, sizeof c->jfilt); }
   if (c->act_lent && memcmp(c->dfilt, c->dfilt_dev, sizeof c->dfilt)) {   // written through cassie_sim_drive_filter (:2151-2153)
     c->b->impl->set_actuator_state(nullptr, &c->dfilt[0][0], nullptr, nullptr, nullptr); memcpy(c->dfilt_dev, c->dfilt, sizeof c->dfilt); }
+  if (c->qfrc != c->qfrc_dev && c->b->impl->set_applied_forces(nullptr, c->qfrc.data(), nullptr)) c->qfrc_dev = c->qfrc;   // written through cassie_sim_qfrc
 }
 cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   std::string path;
@@ -1895,6 +1996,17 @@ void cassie_sim_step_pd(cassie_sim_t *c, state_out_t *y, const pd_in_t *u) { sim
 double *cassie_sim_time(cassie_sim_t *c) { return &c->time; }
 double *cassie_sim_qpos(cassie_sim_t *c) { return c->qpos; }
 double *cassie_sim_qvel(cassie_sim_t *c) { return c->qvel; }
+// :1232-1235: mjData's qfrc_applied [nv] as a borrowed host mirror, uploaded before the next launch like qpos; the first call gives the simulator's batch
+// its applied-force rows
+double *cassie_sim_qfrc(cassie_sim_t *c) {
+  if (c->qfrc.empty()) {
+    if (!c->b->impl->enable_applied_forces(true)) return nullptr;
+    c->qfrc.assign(c->b->impl->hm.nv, 0.0);
+    if (!c->b->impl->get_applied_forces(nullptr, c->qfrc.data())) return nullptr;
+    c->qfrc_dev = c->qfrc;
+  }
+  return c->qfrc.data();
+}
 int cassie_sim_nv(const cassie_sim_t *c) { return c->b->impl->hm.nv; }
 int cassie_sim_nq(const cassie_sim_t *c) { return c->b->impl->hm.nq; }
 void cassie_sim_apply_force(cassie_sim_t *c, double xfrc[6], const char *name) { cassie_batch_apply_force(c->b, xfrc, name); }
@@ -2105,6 +2217,7 @@ void cassie_sim_full_reset(cassie_sim_t *c) {
   c->b->impl->set("cst", cst.data());
   memcpy(c->qpos, q, sizeof q); memset(c->qvel, 0, sizeof c->qvel);   // 35 entries only (:2025): qpos beyond them (the cup of cassie_tray_box.xml) keeps its values
   c->b->impl->set("qpos", c->qpos); c->b->impl->set("qvel", c->qvel); cassie_batch_clear_forces(c->b);
+  if (c->b->impl->dev_ptr("applied")) { const std::vector<double> zero(c->b->impl->hm.nv, 0.0); c->b->impl->set_applied_forces(nullptr, zero.data(), nullptr); }   // qfrc_applied <- 0 (:2024)
   if (!c->acc.empty()) {   // qacc <- 0 (:2025): what the reference's query then gives, with qvel = qacc = 0, is cacc = (0, 0, 0, -g) for every body
     const HostModel &hm = c->b->impl->hm; std::vector<double> row(c->acc.size(), 0.0);
     for (int b = 0; b < (int)c->xquat.size() / 4; b++) for (int k = 0; k < 3; k++) row[AC_CACC + AC_SLOT * b + 3 + k] = -hm.gravity[k];
@@ -2176,6 +2289,10 @@ int cassie_batch_set_env_contact(cassie_batch_t *b, const double *solref, const 
   return b->impl->set_env_contact(solref, solimp, solmix, mask) ? 0 : -1; }
 int cassie_batch_get_env_contact(cassie_batch_t *b, double *solref, double *solimp, double *solmix) { return b->impl->get_env_contact(solref, solimp, solmix) ? 0 : -1; }
 int cassie_batch_clear_env_contact(cassie_batch_t *b) { return b->impl->clear_env_contact() ? 0 : -1; }
+// per-environment applied forces (xfrc_applied per body, qfrc_applied per dof); see include/cassie_b200.h
+int cassie_batch_set_applied_forces(cassie_batch_t *b, const double *xfrc, const double *qfrc, const unsigned char *mask) { return b->impl->set_applied_forces(xfrc, qfrc, mask) ? 0 : -1; }
+int cassie_batch_get_applied_forces(cassie_batch_t *b, double *xfrc, double *qfrc) { return b->impl->get_applied_forces(xfrc, qfrc) ? 0 : -1; }
+int cassie_batch_enable_applied_forces(cassie_batch_t *b, int on) { return b->impl->enable_applied_forces(on != 0) ? 0 : -1; }
 int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) { return b->impl->get_actuator_state(torque_delay, drive_filter, joint_x, joint_y) ? 0 : -1; }
 int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) {
   return b->impl->set_actuator_state(torque_delay, drive_filter, joint_x, joint_y, mask) ? 0 : -1; }

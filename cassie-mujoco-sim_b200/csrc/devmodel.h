@@ -38,6 +38,7 @@ constexpr int F_BP = 64;  // per-environment body offsets: each body's position 
 constexpr int F_AC = 128; // per-environment actuators: ctrlrange, no-load speed and torque delay of every motor come from an ACT_W row (with F_BP, extended instances only)
 constexpr int F_MC = 256; // per-environment mechanics: link inertia, rotor armature and hinge springs come from a MECH_W row (with F_BP | F_AC, extended instances only)
 constexpr int F_CT = 512; // per-environment contact softness: each contact row mixes solref / solimp from its geoms' CONTACT_W slots (with F_BP | F_AC | F_MC, extended only)
+constexpr int F_XF = 1024; // per-environment applied forces: xfrc_applied / qfrc_applied from an APPLIED_W row (plain F_BOX twins, and extended with F_BP | F_AC | F_MC | F_CT)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -196,6 +197,11 @@ constexpr int MC_INERTIA = 0, MC_ARMATURE = 96, MC_STIFF = 128, MC_SPRING = 160;
 constexpr int CT_SLOT = 8;
 constexpr int CONTACT_W = MGT * CT_SLOT;
 constexpr int CT_SOLREF = 0, CT_SOLIMP = 2, CT_SOLMIX = 7;
+// per-environment applied forces (optional, cassie_batch_set_applied_forces; F_XF instances): MuJoCo's xfrc_applied of every body [MB][6] in model body
+// order (force xyz, torque xyz in the world frame, at the body's centre of mass xipos), then qfrc_applied per dof column (main tree 0..31, the extra free
+// body 32..37, as the DYN columns).  State like qvel: resets zero it, snapshots carry it.  The XFRC slot keeps its meaning and adds to its body's entry.
+constexpr int APPLIED_W = 232;
+constexpr int AP_XFRC = 0, AP_QFRC = 192;
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

@@ -41,13 +41,16 @@ void cassie_sim_step_pd(cassie_sim_t *sim, state_out_t *y, const pd_in_t *u);
 double *cassie_sim_time(cassie_sim_t *sim);
 double *cassie_sim_qpos(cassie_sim_t *sim);
 double *cassie_sim_qvel(cassie_sim_t *sim);
+/* src/cassiemujoco.c:1232-1235: mjData's qfrc_applied [nv] as a borrowed read-write host mirror, uploaded before the next launch and refreshed after it
+ * like cassie_sim_qpos; the first call gives the simulator's batch its applied-force rows (cassie_batch_set_applied_forces) */
+double *cassie_sim_qfrc(cassie_sim_t *sim);
 /* src/cassiemujoco.c:1038-1052 */
 int cassie_sim_nv(const cassie_sim_t *sim);
 int cassie_sim_nq(const cassie_sim_t *sim);
 /* include/cassiemujoco.h:263 (src/cassiemujoco.c:1963-1967): xfrc = force xyz, torque xyz in the world frame; unknown name: no-op */
-/* LIMIT of this library: an environment carries ONE (wrench, body) slot.  A call that names another body REPLACES the earlier wrench (the reference
- * keeps xfrc_applied per body, so several bodies can be pushed at once); cassie_sim_clear_forces empties the slot.  The BASELINE configurations push the
- * pelvis only. */
+/* This verb fills ONE (wrench, body) slot per environment: a call that names another body REPLACES the earlier wrench.  For several bodies at once (the
+ * reference keeps xfrc_applied per body) use the applied-force rows, cassie_batch_set_applied_forces on cassie_sim_batch(sim); the slot adds to them.
+ * cassie_sim_clear_forces empties the slot and zeroes the rows' xfrc_applied.  The BASELINE configurations push the pelvis only. */
 void cassie_sim_apply_force(cassie_sim_t *sim, double xfrc[6], const char *name);
 /* include/cassiemujoco.h:268 (src/cassiemujoco.c:1969-1972) */
 void cassie_sim_clear_forces(cassie_sim_t *sim);
@@ -508,7 +511,8 @@ int cassie_batch_get_state(cassie_batch_t *b, void *state);
 int cassie_batch_set_state(cassie_batch_t *b, const void *state, const unsigned char *mask);
 /* re-run mj_forward on the current state (after set_qpos / set_qvel), like cassie_sim_forward (src/cassiemujoco.c:1221-1225) */
 void cassie_batch_forward(cassie_batch_t *b);
-/* batched cassie_sim_apply_force / cassie_sim_clear_forces: xfrc [n][6]; one perturbed body per env */
+/* batched cassie_sim_apply_force / cassie_sim_clear_forces: xfrc [n][6]; one (wrench, body) slot per env, added to the applied-force rows
+ * (cassie_batch_set_applied_forces) when the batch has them; clear_forces empties the slot and zeroes the rows' xfrc_applied, keeping qfrc_applied */
 int cassie_batch_apply_force(cassie_batch_t *b, const double *xfrc, const char *body_name);
 void cassie_batch_clear_forces(cassie_batch_t *b);
 /* batched cassie_integrate_pos (src/cassiemujoco.c:1183-1189 -> mj_integratePos): qpos <- qpos (+) h * qvel, the HBM-bound kernel */
@@ -629,6 +633,31 @@ int cassie_batch_clear_env_mechanics(cassie_batch_t *b);
 int cassie_batch_set_env_contact(cassie_batch_t *b, const double *solref, const double *solimp, const double *solmix, const unsigned char *mask);
 int cassie_batch_get_env_contact(cassie_batch_t *b, double *solref, double *solimp, double *solmix);
 int cassie_batch_clear_env_contact(cassie_batch_t *b);
+/* Per-environment applied forces (perturbation: pushes on any body, joint-space disturbance torques), MuJoCo's mjData arrays per environment:
+ * xfrc [n][nbody][6] -- xfrc_applied, force xyz and torque xyz in the world frame, applied at the body's centre of mass (xipos) -- and qfrc [n][nv] --
+ * qfrc_applied, generalised forces, the extra free body's 6 dofs included.  Either may be NULL (kept); mask [n] (or NULL: all) selects the environments
+ * that change.  The first call allocates the rows, zeroed.  0, or -1 with nothing changed for a non-finite value (cassie_b200_last_error names the
+ * environment, the body or dof, and the field).  The world body and bodies welded to the world are accepted; their values have no effect, as in MuJoCo.
+ * The values are state, as in mjData: cassie_batch_reset (masked) and cassie_sim_full_reset zero both parts, cassie_batch_clear_forces /
+ * cassie_sim_clear_forces zero xfrc and keep qfrc, cassie_batch_set_const leaves both alone; snapshots (cassie_batch_get_state / set_state,
+ * cassie_get_state / set_state, cassie_sim_copy) carry them -- a snapshot with rows restored into a batch without them allocates them, one without rows
+ * zeroes the restored environments' rows.  The (wrench, body) slot of cassie_batch_apply_force keeps its meaning and adds to the rows: a body's total
+ * xfrc_applied is its row plus the slot when the slot names it, and with rows the slot reaches the extra free body too.  The step, cassie_batch_forward
+ * and cassie_sim_step_pd_batch honour the rows, and so do qacc and cacc through the solve; the dynamics rows keep MuJoCo's qfrc_bias (applied forces
+ * excluded); Jacobians, the frames' contact wrenches, rays and depth images do not change.  A batch with rows runs the plain kernel instances f0404 /
+ * f2404 where it would run f04 / f24, and otherwise extended instances that also read contact rows: without rows of its own the batch then gets contact
+ * rows holding the model's values (and mechanics, actuator, offset and constant rows through them, as cassie_batch_set_env_contact does), dropped again
+ * by enable(0) unless a contact call has written them since.  get: what the rows hold (zeros without rows); either pointer may be NULL.  enable: on = 1
+ * allocates zeroed rows (for callers who only write on the device); on = 0 drops the rows and their forces, and the batch returns to the kernel
+ * instances it ran before.  Device rows: cassie_batch_device_ptr(b, "applied"), [n][CASSIE_APPLIED_WIDTH] in the batch precision: xfrc_applied
+ * [32][6] in model body order from CASSIE_APPLIED_XFRC, qfrc_applied [40] by dof column from CASSIE_APPLIED_QFRC (main tree 0..31, the extra free body
+ * 32..37, as the DYN columns).  A write takes effect at the next launch; the kernel derives no index from the row. */
+#define CASSIE_APPLIED_WIDTH 232
+#define CASSIE_APPLIED_XFRC 0
+#define CASSIE_APPLIED_QFRC 192
+int cassie_batch_set_applied_forces(cassie_batch_t *b, const double *xfrc, const double *qfrc, const unsigned char *mask);
+int cassie_batch_get_applied_forces(cassie_batch_t *b, double *xfrc, double *qfrc);
+int cassie_batch_enable_applied_forces(cassie_batch_t *b, int on);
 /* The controller-stage state of every environment, as the reference's cassie_sim_t holds it: the torque delay line torque_delay [n][10][6] (slot 0
  * newest), the drive encoders' integer FIR taps drive_filter [n][10][9], the joint encoders' IIR filters joint_x [n][6][4] and joint_y [n][6][3].
  * NULL parts are skipped; set changes masked environments only (mask NULL: all).  They are state: reset, snapshots and cassie_sim_copy carry them. */
@@ -637,7 +666,7 @@ int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_dela
                                     const unsigned char *mask);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
