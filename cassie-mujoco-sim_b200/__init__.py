@@ -313,6 +313,7 @@ class CassieBatch:
             raise RuntimeError('cassie_batch_init failed: ' + _last_error())
         self.nq, self.nv = self.L.cassie_batch_nq(self.h), self.L.cassie_batch_nv(self.h)
         self.precision = precision
+        self.device = int(device)
 
     def close(self):
         if getattr(self, 'h', None):
@@ -969,6 +970,84 @@ class CassieBatch:
     def free_state(self, snap):
         self.L.cassie_batch_state_free.argtypes = [C.c_void_p, C.c_void_p]
         self.L.cassie_batch_state_free(self.h, C.c_void_p(snap))
+
+    # ---- device-side resets: a bank of start states, restored under a device mask with no host round trip
+    def _reset_lib(self):
+        L = self.L
+        if not getattr(L, '_reset_bound', False):
+            vp = C.c_void_p
+            L.cassie_batch_set_reset_bank.argtypes = [vp, vp, C.POINTER(C.c_int), C.c_int]
+            L.cassie_batch_reset_bank_size.argtypes = [vp]
+            L.cassie_batch_reset_where.argtypes = [vp, vp, vp]
+            L.cassie_batch_forward_where.argtypes = [vp, vp]
+            for n in ('set_reset_bank', 'reset_bank_size', 'reset_where', 'forward_where'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._reset_bound = True
+        return L
+
+    def set_reset_bank(self, snap, envs=None, k=None):
+        """the reset bank: entry i is environment envs[i] of the snapshot `snap` (get_state of this or any batch of the same precision and model,
+        of any size); envs None: the first k environments (k defaults to this batch's size).  Every call replaces the bank; snap None frees it.
+        An envs index outside the snapshot or a snapshot of another precision or model raises, and the old bank is kept."""
+        L = self._reset_lib()
+        if snap is None:
+            rc = L.cassie_batch_set_reset_bank(self.h, None, None, 0)
+        elif envs is None:
+            rc = L.cassie_batch_set_reset_bank(self.h, C.c_void_p(snap), None, self.n if k is None else int(k))
+        else:
+            e = np.ascontiguousarray(envs, dtype=np.int64).ravel()
+            if e.size and (e.min() < -2 ** 31 or e.max() >= 2 ** 31):
+                raise ValueError('envs must fit int32')
+            e = e.astype(np.int32)
+            rc = L.cassie_batch_set_reset_bank(self.h, C.c_void_p(snap), e.ctypes.data_as(C.POINTER(C.c_int)), int(e.size))
+        if rc != 0:
+            raise RuntimeError(_last_error())
+
+    def reset_bank_size(self):
+        return int(self._reset_lib().cassie_batch_reset_bank_size(self.h))
+
+    def _device_rows(self, t, what, dtypes):
+        import torch
+        if not isinstance(t, torch.Tensor):
+            raise TypeError('%s must be a CUDA torch tensor, not %s' % (what, type(t).__name__))
+        if not t.is_cuda or t.device.index != self.device:
+            raise ValueError('%s must be on cuda:%d (the batch\'s device), not %s' % (what, self.device, t.device))
+        if t.dtype not in dtypes or t.numel() != self.n or not t.is_contiguous():
+            raise ValueError('%s must be a contiguous tensor of %d elements of %s, not %s %s' % (what, self.n, ' / '.join(str(d) for d in dtypes), t.dtype, tuple(t.shape)))
+        return t
+
+    def _mask_ptr(self, mask, what):
+        import torch
+        m = self._device_rows(mask, what, (torch.bool, torch.uint8))
+        return (m.view(torch.uint8) if m.dtype == torch.bool else m).data_ptr()   # bool is one byte per element: reinterpreted, not copied
+
+    def reset_where(self, done, entry=None):
+        """environments with done[e] set take bank entry entry[e] mod K (entry None: e mod K), as set_state would restore that entry; the others are
+        untouched.  done: CUDA bool / uint8 tensor [n]; entry: CUDA int32 / int64 tensor [n] (int64 is converted, and the int32 copy kept until the
+        next call so that it outlives the launch).  One launch on the batch's stream: no host synchronisation, capturable in a CUDA graph.
+
+        Stream rule (as torch_view's): done and entry are written on torch's stream and must be ordered before the batch's stream, so either run the
+        batch on torch's stream (set_stream(torch.cuda.current_stream().cuda_stream)) or synchronise before the call."""
+        import torch
+        L = self._reset_lib()
+        mp = self._mask_ptr(done, 'done')
+        ep = None
+        if entry is not None:
+            e = self._device_rows(entry, 'entry', (torch.int32, torch.int64))
+            if e.dtype == torch.int64:
+                e = e.to(torch.int32)
+            self._entry_tmp = e
+            ep = e.data_ptr()
+        if L.cassie_batch_reset_where(self.h, C.c_void_p(mp), None if ep is None else C.c_void_p(ep)) != 0:
+            raise RuntimeError(_last_error())
+
+    def forward_where(self, mask):
+        """mj_forward for the environments with mask[e] set (CUDA bool / uint8 tensor [n]), each on its own model rows; the others are untouched.
+        Asynchronous and capturable like reset_where, with its stream rule: e.g. reset_where, noise written into torch_view('qpos') / ('qvel') of the
+        reset environments, forward_where."""
+        L = self._reset_lib()
+        if L.cassie_batch_forward_where(self.h, C.c_void_p(self._mask_ptr(mask, 'mask'))) != 0:
+            raise RuntimeError(_last_error())
 
     def set_timestep(self, dt):
         self.L.cassie_batch_set_timestep.argtypes = [C.c_void_p, C.c_double]

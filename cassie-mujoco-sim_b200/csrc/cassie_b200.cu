@@ -22,6 +22,7 @@
 #include "step_kernel.cuh"
 #include "raycast.inl"
 #include "camera.inl"
+#include "reset.inl"
 
 // the step-kernel instances live in their own translation units (step_inst.cu, one compilation per instance)
 #define CASSIE_STEP_ENTRY(tag) extern "C" const void *cassie_step_entry_##tag(void);
@@ -44,6 +45,7 @@ namespace cassie {
 
 template <typename real> cudaError_t launch_raycast(const RayArgs<real> &A, int device, cudaStream_t stream);   // raycast.cu
 template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int device, cudaStream_t stream);   // camera.cu
+template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device, cudaStream_t stream);       // reset.cu
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
@@ -251,13 +253,6 @@ __global__ void fill_rows_kernel(T *__restrict__ dst, const T *__restrict__ row,
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) { const size_t e = i / w; if ((!mask || mask[e]) && (int)(i - e * w) < ncols) dst[i] = row[i - e * w]; }
 }
 
-// rows of the selected environments <- the same rows of another array (snapshot restore of a subset)
-template <typename T>
-__global__ void copy_rows_kernel(T *__restrict__ dst, const T *__restrict__ src, int w, const unsigned char *__restrict__ mask, int n) {
-  const size_t total = (size_t)n * w;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) { const size_t e = i / w; if (!mask || mask[e]) dst[i] = src[i]; }
-}
-
 // ------------------------------------------------------------------ host side
 // device-resident copy of every per-environment row array of a batch (cassie_state_t / cassie_batch_get_state); it owns its memory and carries its own
 // sizes, so it can be copied, restored into any batch of the same shape and freed without the batch it was taken from
@@ -335,6 +330,14 @@ struct BatchBase {
   virtual Snap *snap_alloc() = 0;
   virtual bool snap_get(Snap *snap) = 0;
   virtual bool snap_set(const Snap *snap, const unsigned char *mask) = 0;
+  // the reset bank: k start states gathered on the device from environments envs (null: 0 .. k - 1) of a snapshot of the same precision and model
+  // (any size); k = 0 or a null snapshot drops it.  Checked before anything changes: a refused call keeps the old bank
+  virtual bool set_reset_bank(const Snap *snap, const int *envs, int k) = 0;
+  virtual int reset_bank_size() const = 0;
+  // device-masked restore from the bank and device-masked mj_forward: enqueued on the batch's stream, no host synchronisation, copy or allocation
+  virtual bool reset_where(const void *d_mask, const void *d_entry) = 0;
+  virtual bool forward_where(const void *d_mask) = 0;
+  bool legacy = false;   // the batch of a cassie_sim_t: its host mirrors are pushed before every launch, so device-side resets are refused
   virtual bool copy_model_from(BatchBase *src) = 0;     // per-environment constants, height fields, timestep (mj_copyModel in cassie_sim_copy, :1083-1091)
   virtual bool rebuild_model() = 0;                     // after hm was edited (timestep, hold / release): rebuild and upload the constant block
   // per-environment placement of static planes / boxes (GEOM_ENV_W rows): pos / quat / size [n][3] / [n][4] / [n][3] or null (that part unchanged)
@@ -403,6 +406,14 @@ struct BatchBase {
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
 };
 
+// the step instances' dynamic shared-memory limit is a property of the function, shared by every batch of the process: a batch raises it to its own
+// launch size and never lowers it, so a smaller batch created later does not invalidate the launches of a larger one
+static cudaError_t raise_smem_limit(const void *entry, int bytes) {
+  cudaFuncAttributes fa; cudaError_t e = cudaFuncGetAttributes(&fa, entry);
+  if (e != cudaSuccess || fa.maxDynamicSharedSizeBytes >= bytes) return e;
+  return cudaFuncSetAttribute(entry, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+}
+
 template <typename real> struct Batch : BatchBase {
   DevModel<real> *d_model = nullptr; EnvArrays<real> A{}; int QW = QPOS_W_MAIN, VW = QVEL_W_MAIN;
   struct LaunchCfg { int wpb = 1; size_t smem = 0; int resident_ctas = 1; } cfg[3];   // [0] plain instance, [1] extended instance, [2] plain + estimator
@@ -435,7 +446,9 @@ template <typename real> struct Batch : BatchBase {
   bool ct_mech = false;                    // the mechanics rows were allocated by the contact setter (model values), and no mechanics call has written them since
   real *d_app = nullptr;                   // A.applied: [n][APPLIED_W] per-environment applied forces (state), allocated by the first applied-force verb (F_XF instances)
   bool xf_ct = false;                      // the contact rows were allocated for the chain twin (model values), and no contact call has written them since
+  Snap *bank = nullptr;                    // the reset bank (cassie_batch_set_reset_bank): a snapshot of k entries
   ~Batch() override {
+    snap_delete(bank);
     cudaSetDevice(device);
     cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
@@ -498,21 +511,21 @@ template <typename real> struct Batch : BatchBase {
       cfg[ext].wpb = k_sel; cfg[ext].smem = model_bytes<real>() + (size_t)k_sel * wb;
       int per_sm = 0;
       { const void *entry = step_entry<real>(ext, feat);
-        CUDA_OK(cudaFuncSetAttribute(entry, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
-        CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, feat | F_EG), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // same scratch, same shape
-        if (ext == 1) for (int fe : {feat | F_FR, feat | F_EG | F_FR}) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+        CUDA_OK(raise_smem_limit(entry, (int)cfg[ext].smem));
+        CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_EG), (int)cfg[ext].smem));   // same scratch, same shape
+        if (ext == 1) for (int fe : {feat | F_FR, feat | F_EG | F_FR}) CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe), (int)cfg[ext].smem));
         if (hm.nhfield == 1) {   // per-environment terrain: F_ALL | F_EG | F_TR (the scratch of F_ALL)
-          CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
-          if (ext == 1) CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, F_ALL | F_EG | F_TR | F_FR), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }
+          CUDA_OK(raise_smem_limit(step_entry<real>(ext, F_ALL | F_EG | F_TR), (int)cfg[ext].smem));
+          if (ext == 1) CUDA_OK(raise_smem_limit(step_entry<real>(ext, F_ALL | F_EG | F_TR | F_FR), (int)cfg[ext].smem)); }
         if (ext == 1)   // per-environment body offsets: every instance step_entry routes F_BP launches to (the extended scratch)
           for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) {   // and their F_AC twins (per-environment actuators)
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // and their F_MC twins
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));   // and their F_CT twins
-            CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem)); }   // and their F_XF twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe), (int)cfg[ext].smem));
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC), (int)cfg[ext].smem));
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC), (int)cfg[ext].smem));   // and their F_MC twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), (int)cfg[ext].smem));   // and their F_CT twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), (int)cfg[ext].smem)); }   // and their F_XF twins
         if (ext != 1 && step_entry<real>(ext, feat | F_XF))   // the plain F_XF twins (applied forces), where this model runs f04 / f24
-          CUDA_OK(cudaFuncSetAttribute(step_entry<real>(ext, feat | F_XF), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg[ext].smem));
+          CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF), (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -818,42 +831,96 @@ template <typename real> struct Batch : BatchBase {
   bool snap_set(const Snap *k, const unsigned char *mask) override {
     if (!snap_compatible(k)) return false;
     CUDA_OK(cudaSetDevice(device));
-    const unsigned char *dm = nullptr;
-    if (mask) { if (!upload_mask(mask)) return false; dm = d_mask; }
-    if (k->has_est && !A.est && !enable_estimator_device(true)) return false;
-    if (!k->has_est && A.est && !reset_estimator_device(mask)) return false;   // the snapshot was taken before the estimator ran: it starts afresh
-    if (k->has_appl && !d_app && !enable_applied_forces(true)) return false;   // likewise the applied-force rows: allocated by a snapshot that has them,
-    if (!k->has_appl && d_app) {                                               // zeroed by one taken without them
-      if (!dm) CUDA_OK(cudaMemsetAsync(d_app, 0, sizeof(real) * n * APPLIED_W, stream));
-      else { const std::vector<real> zero(APPLIED_W, real(0)); if (!fill_masked(d_app, zero.data(), APPLIED_W)) return false; }
-    }
+    if (mask && !upload_mask(mask)) return false;
+    if (k->has_est && !A.est && !enable_estimator_device(true)) return false;   // optional rows the snapshot has are allocated where the batch lacks them
+    if (k->has_appl && !d_app && !enable_applied_forces(true)) return false;
+    if (mask) return restore_rows(k, d_mask, nullptr) && sync();   // one launch: the snapshot as a bank of n entries, environment e taking entry e
+    if (!k->has_est && A.est && !reset_estimator_device(nullptr)) return false;   // the snapshot was taken before the estimator ran: it starts afresh
+    if (!k->has_appl && d_app) CUDA_OK(cudaMemsetAsync(d_app, 0, sizeof(real) * n * APPLIED_W, stream));   // likewise the applied forces: zeroed
     for (int r = 0; r < Snap::NROWS; r++) {
       if (!k->has(r) || (r == Snap::R_AUX && !A.aux)) continue;
-      if (!dm) { CUDA_OK(cudaMemcpyAsync(snap_src(r), k->rows[r], k->bytes(r), cudaMemcpyDeviceToDevice, stream)); continue; }
-      const int w = k->width(r);
-      if (k->elem(r) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)snap_src(r), (const unsigned long long *)k->rows[r], w, dm, n);
-      else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)snap_src(r), (const unsigned int *)k->rows[r], w, dm, n);
-      CUDA_OK(cudaGetLastError());
+      CUDA_OK(cudaMemcpyAsync(snap_src(r), k->rows[r], k->bytes(r), cudaMemcpyDeviceToDevice, stream));
     }
-    if (A.frames && k->frames && k->frame_list == frame_list) {   // frame rows: only between batches with the same frame list, like the aux rows
-      if (!dm) CUDA_OK(cudaMemcpyAsync(A.frames, k->frames, k->frame_bytes(), cudaMemcpyDeviceToDevice, stream));
-      else {
-        const int w = (int)(frame_list.size() / 2) * FRAME_W;
-        if (sizeof(real) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)A.frames, (const unsigned long long *)k->frames, w, dm, n);
-        else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)A.frames, (const unsigned int *)k->frames, w, dm, n);
-        CUDA_OK(cudaGetLastError());
-      }
-    }
-    if (A.acc && k->acc && k->frame_list == frame_list) {   // acceleration rows: likewise
-      if (!dm) CUDA_OK(cudaMemcpyAsync(A.acc, k->acc, k->acc_bytes(), cudaMemcpyDeviceToDevice, stream));
-      else {
-        const int w = acc_width(A.nfr);
-        if (sizeof(real) == 8) copy_rows_kernel<unsigned long long><<<256, 256, 0, stream>>>((unsigned long long *)A.acc, (const unsigned long long *)k->acc, w, dm, n);
-        else copy_rows_kernel<unsigned int><<<256, 256, 0, stream>>>((unsigned int *)A.acc, (const unsigned int *)k->acc, w, dm, n);
-        CUDA_OK(cudaGetLastError());
-      }
-    }
+    if (A.frames && k->frames && k->frame_list == frame_list) CUDA_OK(cudaMemcpyAsync(A.frames, k->frames, k->frame_bytes(), cudaMemcpyDeviceToDevice, stream));   // frame
+    if (A.acc && k->acc && k->frame_list == frame_list) CUDA_OK(cudaMemcpyAsync(A.acc, k->acc, k->acc_bytes(), cudaMemcpyDeviceToDevice, stream));   // and acceleration rows: only between batches with the same frame list, like the aux rows
     return sync();
+  }
+  // one launch of the restore kernel (reset.cu) from the entries of k into the rows of this batch: environment e, when d_mask[e] is non-zero (null: every
+  // environment), takes entry (unsigned)d_entry[e] % k->n (null: e % k->n), by reset_table's rules.  Enqueued only: no synchronisation, copy or allocation
+  bool restore_rows(const Snap *k, const unsigned char *dmask, const int *dentry) {
+    void *dst[RR_N] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux, d_app, A.frames, A.acc};
+    const void *src[RR_N];
+    for (int r = 0; r < Snap::NROWS; r++) src[r] = k->has(r) ? k->rows[r] : nullptr;
+    src[RR_FRAMES] = k->frames; src[RR_ACC] = k->acc;
+    ResetArgs R; std::string err;
+    if (!reset_table(R, dst, src, (int)sizeof(real), QW, VW, A.nfr, k->frame_list == frame_list, err)) { set_err(err); return false; }
+    R.mask = dmask; R.entry = dentry; R.k = k->n; R.n = n;
+    CUDA_OK(launch_reset<real>(R, device, stream));
+    launches++;
+    return true;
+  }
+  // ---- the reset bank and the device-masked verbs
+  bool set_reset_bank(const Snap *k, const int *envs, int nk) override {
+    if (nk < 0) { set_err("cassie_batch_set_reset_bank: k must be >= 0"); return false; }
+    if (nk == 0 || !k) { CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream)); snap_delete(bank); bank = nullptr; return true; }   // no launch reads the old bank any more
+    if (k->esz != (int)sizeof(real) || k->qw != QW || k->vw != VW || k->device != device) { set_err("cassie_batch_set_reset_bank: the snapshot is of another precision, model or device"); return false; }
+    if (!envs && nk > k->n) { set_err("cassie_batch_set_reset_bank: k = " + std::to_string(nk) + " exceeds the snapshot's " + std::to_string(k->n) + " environments (envs is NULL)"); return false; }
+    if (envs) for (int i = 0; i < nk; i++) if (envs[i] < 0 || envs[i] >= k->n) {
+      set_err("cassie_batch_set_reset_bank: envs[" + std::to_string(i) + "] = " + std::to_string(envs[i]) + " is outside the snapshot's " + std::to_string(k->n) + " environments"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    Snap *nb = snap_new(device, nk, k->esz, k->qw, k->vw);
+    if (!nb) { set_err("cassie_batch_set_reset_bank: out of device memory"); return false; }
+    nb->has_est = k->has_est; nb->has_aux = k->has_aux; nb->has_appl = k->has_appl; nb->frame_list = k->frame_list;
+    int *d_envs = nullptr; bool ok = true;
+    for (int r = 0; r < Snap::NROWS && ok; r++) if (nb->has(r) && !nb->rows[r]) ok = cudaMalloc(&nb->rows[r], nb->bytes(r)) == cudaSuccess;
+    if (ok && k->frames) ok = cudaMalloc(&nb->frames, nb->frame_bytes()) == cudaSuccess;
+    if (ok && k->acc) ok = cudaMalloc(&nb->acc, nb->acc_bytes()) == cudaSuccess;
+    if (ok && envs) ok = cudaMalloc(&d_envs, sizeof(int) * nk) == cudaSuccess && cudaMemcpyAsync(d_envs, envs, sizeof(int) * nk, cudaMemcpyHostToDevice, stream) == cudaSuccess;
+    if (ok) {   // the gather runs on the device: entry i of the bank <- environment envs[i] of the snapshot, every row kind the snapshot holds
+      void *dst[RR_N]; const void *src[RR_N];
+      for (int r = 0; r < Snap::NROWS; r++) { dst[r] = nb->has(r) ? nb->rows[r] : nullptr; src[r] = k->has(r) ? k->rows[r] : nullptr; }
+      dst[RR_FRAMES] = nb->frames; src[RR_FRAMES] = k->frames; dst[RR_ACC] = nb->acc; src[RR_ACC] = k->acc;
+      ResetArgs R; std::string err;
+      if (!reset_table(R, dst, src, k->esz, k->qw, k->vw, (int)(k->frame_list.size() / 2), true, err)) { set_err(err); ok = false; }
+      else {
+        R.mask = nullptr; R.entry = d_envs; R.k = k->n; R.n = nk;
+        const cudaError_t e = launch_reset<real>(R, device, stream);
+        if (e != cudaSuccess) { set_err(std::string("cassie_batch_set_reset_bank: ") + cudaGetErrorString(e)); ok = false; }
+      }
+    } else set_err("cassie_batch_set_reset_bank: out of device memory");
+    const cudaError_t es = cudaStreamSynchronize(stream);   // the gather is done (and no launch reads the old bank) before anything is freed
+    cudaFree(d_envs);
+    if (ok && es != cudaSuccess) { set_err(std::string("cassie_batch_set_reset_bank: ") + cudaGetErrorString(es)); ok = false; }
+    if (!ok) { snap_delete(nb); return false; }
+    snap_delete(bank); bank = nb;
+    return true;
+  }
+  int reset_bank_size() const override { return bank ? bank->n : 0; }
+  // a pointer the device-masked verbs accept: device or managed memory of the batch's device (a host array passed by mistake is refused, not launched)
+  bool device_rows(const void *p, const char *verb, const char *what) {
+    if (!p) { set_err(std::string(verb) + ": " + what + " is required"); return false; }
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); set_err(std::string(verb) + ": " + what + " is not a CUDA pointer"); return false; }
+    if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != device) {
+      set_err(std::string(verb) + ": " + what + " must be device or managed memory of device " + std::to_string(device) + " (a host array cannot be read by the launch)"); return false; }
+    return true;
+  }
+  bool reset_where(const void *d_mask, const void *d_entry) override {
+    const char *verb = "cassie_batch_reset_where";
+    if (!bank) { set_err(std::string(verb) + ": no reset bank (cassie_batch_set_reset_bank first)"); return false; }
+    if (!device_rows(d_mask, verb, "the mask") || (d_entry && !device_rows(d_entry, verb, "the entry array"))) return false;
+    if (est_filter) { set_err(std::string(verb) + ": the host-side estimator filters are on (cassie_batch_enable_estimator_filter): they cannot follow a device reset"); return false; }
+    if (legacy) { set_err(std::string(verb) + ": the batch belongs to a cassie_sim_t, whose host mirrors would overwrite the reset"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    return restore_rows(bank, (const unsigned char *)d_mask, (const int *)d_entry);
+  }
+  bool forward_where(const void *d_mask) override {
+    const char *verb = "cassie_batch_forward_where";
+    if (!device_rows(d_mask, verb, "the mask")) return false;
+    if (A.applied && !A.contact && launch_kind(1) == 1) {   // step_range would allocate the chain twin's contact rows here
+      set_err(std::string(verb) + ": this batch gets model-valued contact rows at its first extended launch; run cassie_batch_step or cassie_batch_forward once first"); return false; }
+    A.mask = (const unsigned char *)d_mask; const bool ok = step(0, 1); A.mask = nullptr;
+    return ok;
   }
   bool rebuild_model() override {
     CUDA_OK(cudaSetDevice(device));
@@ -1662,19 +1729,23 @@ template <typename real> struct Batch : BatchBase {
     return true;
   }
   bool step(int nticks, int mode) override { return step_range(nticks, mode, 0, n, stream); }
+  // the instance kind a launch of `mode` runs: 0 plain, 1 extended, 2 plain + estimator
+  int launch_kind(int mode) {
+    // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
+    // the in-kernel estimator alone: the plain instance with the estimator stage
+    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    // applied forces: a plain twin where f04 / f24 would run, else the chain twin
+    if (A.applied && ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF)) ext = 1;
+    return ext;
+  }
   bool step_range(int nticks, int mode, int env0, int count, cudaStream_t on) {   // the launch covers environments [env0, env0 + count)
     CUDA_OK(cudaSetDevice(device));
     if (mode == 2 && !A.aux) { set_err("query needs the derived-quantity rows (cassie_batch_enable_aux)"); return false; }
     if (mode == 4 && (!A.frames || !A.jac)) { set_err("the frame Jacobian needs frames (cassie_batch_set_frames)"); return false; }
     if (mode == 5 && !A.dyn) { set_err("the dynamics launch needs its rows (cassie_batch_dynamics)"); return false; }
     A.nsub = nsub_override;
-    // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
-    // the in-kernel estimator alone: the plain instance with the estimator stage
-    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
-    if (A.applied) {   // applied forces: a plain twin where f04 / f24 would run, else the chain twin, which reads contact rows (the model's values when none were set)
-      if (ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF)) ext = 1;
-      if (ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }
-    }
+    const int ext = launch_kind(mode);
+    if (A.applied && ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }   // the chain twin reads contact rows (the model's values when none were set)
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
@@ -1970,6 +2041,7 @@ cassie_sim_t *cassie_sim_init(const char *modelfile, bool reinit) {
   cassie_batch_t *b = cassie_batch_init(path.c_str(), 1, 0, CASSIE_B200_FP64);
   if (!b) return nullptr;
   cassie_sim_t *c = new cassie_sim(); memset(c->qpos, 0, sizeof c->qpos); memset(c->qvel, 0, sizeof c->qvel); memset(c->aux, 0, sizeof c->aux); c->b = b; c->path = path; c->timestep = c->timestep_dev = b->impl->hm.timestep;
+  b->impl->legacy = true;
   b->impl->enable_aux(true);   // a single environment always carries the derived-quantity row ...
   { const HostModel &hm = b->impl->hm; std::vector<const char *> names; std::vector<int> kinds;   // ... and a frame per body and site (cassie_sim_xpos & co.)
     for (const std::string &s : hm.names_body) { names.push_back(s.c_str()); kinds.push_back(0); }
@@ -2447,5 +2519,9 @@ void *cassie_batch_state_alloc(cassie_batch_t *b) { return b->impl->snap_alloc()
 void cassie_batch_state_free(cassie_batch_t *b, void *state) { (void)b; snap_delete((Snap *)state); }
 int cassie_batch_get_state(cassie_batch_t *b, void *state) { return state && b->impl->snap_get((Snap *)state) ? 0 : -1; }
 int cassie_batch_set_state(cassie_batch_t *b, const void *state, const unsigned char *mask) { return state && b->impl->snap_set((const Snap *)state, mask) ? 0 : -1; }
+int cassie_batch_set_reset_bank(cassie_batch_t *b, const void *state, const int *envs, int k) { return b->impl->set_reset_bank((const Snap *)state, envs, k) ? 0 : -1; }
+int cassie_batch_reset_bank_size(const cassie_batch_t *b) { return b->impl->reset_bank_size(); }
+int cassie_batch_reset_where(cassie_batch_t *b, const void *d_mask, const void *d_entry) { return b->impl->reset_where(d_mask, d_entry) ? 0 : -1; }
+int cassie_batch_forward_where(cassie_batch_t *b, const void *d_mask) { return b->impl->forward_where(d_mask) ? 0 : -1; }
 #include "legacy_stubs.inc"
 }  // extern "C"

@@ -511,6 +511,36 @@ int cassie_batch_get_state(cassie_batch_t *b, void *state);
 int cassie_batch_set_state(cassie_batch_t *b, const void *state, const unsigned char *mask);
 /* re-run mj_forward on the current state (after set_qpos / set_qvel), like cassie_sim_forward (src/cassiemujoco.c:1221-1225) */
 void cassie_batch_forward(cassie_batch_t *b);
+/* Device-side resets (new): environments restored from a bank of K start states under a mask that lives on the device, with no host round trip.
+ *
+ * cassie_batch_set_reset_bank: entry i of the bank becomes environment envs[i] (envs NULL: i) of `state`, a snapshot taken with
+ * cassie_batch_state_alloc / cassie_batch_get_state.  The snapshot may come from another batch of any size, so K may exceed n and poses prepared in a
+ * helper batch (qpos / qvel written through the device pointers, cassie_batch_forward, cassie_batch_get_state) can be banked; it must have the same
+ * precision and model (qpos / qvel widths) and live on the same device.  The gather runs on the device.  Every call replaces the bank; k == 0 or state
+ * NULL frees it.  0, or -1 with the old bank kept for k < 0, an envs index outside the snapshot, or a snapshot of another precision or model.
+ * cassie_batch_reset_bank_size: K (0 without a bank).
+ *
+ * cassie_batch_reset_where: environment e with d_mask[e] != 0 (device uint8[n]; a torch.bool tensor as it is) takes bank entry
+ * (unsigned)d_entry[e] % K (device int32[n]; NULL: e % K), so no value can address outside the bank.  The semantics are those of
+ * cassie_batch_set_state applied to the chosen entry, per environment; the rows of unmasked environments are not touched.  Optional rows: estimator
+ * and applied-force rows the batch has are copied from the entry, or zeroed when the bank lacks them (the filters start afresh); aux rows are copied
+ * when both have them, else left alone; frame and acceleration rows are copied when the frame lists are equal, else left alone.  A row kind the bank
+ * has and the batch lacks is ignored (nothing is allocated).  counters, PD, task and gait rows and every model input are left alone; time is the
+ * entry's own.  One launch, enqueued on the batch's stream: no host synchronisation, no copy, no allocation, so it can be captured in a CUDA graph.
+ * The mask and entries must be written before the launch in the batch's stream order.  -1, with nothing enqueued, for: no bank, a NULL mask, a
+ * pointer that is not device or managed memory of the batch's device, the host-side estimator filters on (cassie_batch_enable_estimator_filter),
+ * or the batch of a cassie_sim_t (cassie_sim_batch).
+ *
+ * cassie_batch_forward_where: mj_forward for the environments with d_mask[e] != 0 (as cassie_batch_forward, on their own model rows), the others
+ * untouched; asynchronous and capture-safe like reset_where, with its pointer checks.  Use it after writing qpos / qvel of reset environments on the
+ * device (per-episode noise), or after an entry taken under other model rows, to recompute the sensor data, aux, frame and acceleration rows
+ * with each environment's own model rows (the observation row follows at the next control tick, as after cassie_batch_forward).  A batch with applied-force rows gets
+ * model-valued contact rows at its first extended launch, which allocates: until an ordinary cassie_batch_step or cassie_batch_forward has run,
+ * forward_where refuses with -1. */
+int cassie_batch_set_reset_bank(cassie_batch_t *b, const void *state, const int *envs, int k);
+int cassie_batch_reset_bank_size(const cassie_batch_t *b);
+int cassie_batch_reset_where(cassie_batch_t *b, const void *d_mask, const void *d_entry);
+int cassie_batch_forward_where(cassie_batch_t *b, const void *d_mask);
 /* batched cassie_sim_apply_force / cassie_sim_clear_forces: xfrc [n][6]; one (wrench, body) slot per env, added to the applied-force rows
  * (cassie_batch_set_applied_forces) when the batch has them; clear_forces empties the slot and zeroes the rows' xfrc_applied, keeping qfrc_applied */
 int cassie_batch_apply_force(cassie_batch_t *b, const double *xfrc, const char *body_name);
