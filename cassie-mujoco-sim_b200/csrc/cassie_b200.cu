@@ -1821,6 +1821,9 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
     if (!strcmp(f, "applied")) return d_app;
+#ifdef CASSIE_STAGE_CLOCKS
+    if (!strcmp(f, "stage_clocks")) return A.qM;   // [n][2 NM_MAX] reals, words 0.. the stage clocks of the last step sub-step (step_core.inl STAGE_CLOCK)
+#endif
     return nullptr;
   }
   bool get_counters(int *out) override {
