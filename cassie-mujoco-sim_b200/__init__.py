@@ -41,6 +41,9 @@ def acc_width(nframes):
 # slices of a derived-quantity row (CASSIE_AUX_* in include/cassie_b200.h)
 AUX = dict(foot_force=slice(0, 12), toe_force=slice(12, 18), heel_force=slice(18, 24), foot_pos=slice(24, 30), foot_vel=slice(30, 42),
            cm_pos=slice(42, 45), cm_vel=slice(45, 48), angmom=slice(48, 51), obstacle=51, self_collision=52, group_mask=53, ncon=54)
+# per-tick trace sources (include/cassie_b200.h CASSIE_TRACE_*): CassieBatch.set_trace columns are (source, column) pairs, columns as OBS / AUX / FRAME slice
+# the rows (a frame column is frame * FRAME_WIDTH + an offset of FRAME)
+TRACE_QPOS, TRACE_QVEL, TRACE_OBS, TRACE_AUX, TRACE_FRAME, TRACE_MAX = 0, 1, 2, 3, 4, 64
 # observation row layout (cassie_batch_get_obs)
 OBS = dict(motor_pos=slice(0, 10), motor_vel=slice(10, 20), motor_torque=slice(20, 30), joint_pos=slice(30, 36), joint_vel=slice(36, 42),
            quat=slice(42, 46), gyro=slice(46, 49), accel=slice(49, 52), mag=slice(52, 55), time=55,
@@ -719,6 +722,44 @@ class CassieBatch:
         if self._applied_lib().cassie_batch_enable_applied_forces(self.h, 1 if on else 0) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- per-tick traces of multi-tick launches
+    def _trace_lib(self):
+        L = self.L
+        if not getattr(L, '_trace_bound', False):
+            vp, ip = C.c_void_p, C.POINTER(C.c_int)
+            L.cassie_batch_set_trace.argtypes = [vp, ip, ip, C.c_int, C.c_int]
+            L.cassie_batch_trace_ticks.argtypes = [vp]
+            L.cassie_batch_get_trace.argtypes = [vp, C.POINTER(C.c_double)]
+            for n in ('set_trace', 'trace_ticks', 'get_trace'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._trace_bound = True
+        return L
+
+    def set_trace(self, columns, max_ticks=50):
+        """trace k <= TRACE_MAX columns at every tick of a step launch: columns is a list of (source, column) pairs, source one of TRACE_QPOS,
+        TRACE_QVEL, TRACE_OBS, TRACE_AUX (enable_aux first), TRACE_FRAME (set_frames first); max_ticks slots T per environment, the last T ticks of a
+        longer launch kept in order.  An empty list drops the trace.  A bad column raises, and nothing changes.  See include/cassie_b200.h."""
+        cols = [(int(s), int(c)) for s, c in columns]
+        src = (C.c_int * max(1, len(cols)))(*[s for s, _ in cols])
+        col = (C.c_int * max(1, len(cols)))(*[c for _, c in cols])
+        if self._trace_lib().cassie_batch_set_trace(self.h, src, col, len(cols), int(max_ticks)) != 0:
+            raise RuntimeError(_last_error())
+        self._trace_shape = (int(max_ticks), len(cols)) if cols else None
+
+    def trace_ticks(self):
+        """slots the last step launch wrote: min(nticks, max_ticks)"""
+        return int(self._trace_lib().cassie_batch_trace_ticks(self.h))
+
+    def trace(self):
+        """the slots the last step launch wrote, [n, trace_ticks(), k] (a synchronous copy)"""
+        shape = getattr(self, '_trace_shape', None)
+        if shape is None:
+            raise RuntimeError('no trace is set (set_trace)')
+        out = np.zeros((self.n,) + shape)
+        if self._trace_lib().cassie_batch_get_trace(self.h, self._dp(out)) != 0:
+            raise RuntimeError(_last_error())
+        return out[:, :self.trace_ticks()]
+
     def actuator_state(self):
         """dict of the controller-stage state: torque_delay [n, 10, 6] (slot 0 newest), drive_filter [n, 10, 9] int32, joint_x [n, 6, 4], joint_y [n, 6, 3]"""
         L = self._act_lib()
@@ -1086,7 +1127,8 @@ class CassieBatch:
         qpos_spring[32] per main-tree dof (the springs of hinge dofs only are read), read at the next launch; set_env_mechanics first; contact [n, 256]:
         32 slots of 8 -- solref[2], solimp[5], solmix -- one per device collision geom (moving 0..15, static 16..31; unused slots zero), read at the next
         launch; set_env_contact first; applied [n, 232]: xfrc_applied[32][6] in model body order, then qfrc_applied[40] by dof column (main tree 0..31,
-        the extra free body 32..37), read at the next launch; set_applied_forces or enable_applied_forces first).  set_frames /
+        the extra free body 32..37), read at the next launch; set_applied_forces or enable_applied_forces first; trace [n, T, k]: the per-tick trace of
+        the last step launch, slot s of every environment, written by step launches only; set_trace first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -1096,7 +1138,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field == 'terrain':
             ts = '<i4'
@@ -1108,6 +1150,8 @@ class CassieBatch:
         t = torch.as_tensor(a, device='cuda')
         if field == 'terrain':
             return t.view(self.n)
+        if field == 'trace':
+            return t.view(self.n, *self._trace_shape)
         return t.view(self.n, *self._cam_hw) if field == 'depth' else t
 
 

@@ -39,6 +39,7 @@ CASSIE_STEP_ENTRY(f11c4) CASSIE_STEP_ENTRY(f11d7) CASSIE_STEP_ENTRY(d11d7) CASSI
 CASSIE_STEP_ENTRY(f13c4) CASSIE_STEP_ENTRY(f13d7) CASSIE_STEP_ENTRY(d13d7) CASSIE_STEP_ENTRY(f13df) CASSIE_STEP_ENTRY(d13df) CASSIE_STEP_ENTRY(f13ff) CASSIE_STEP_ENTRY(d13ff)
 CASSIE_STEP_ENTRY(f0404) CASSIE_STEP_ENTRY(f2404)
 CASSIE_STEP_ENTRY(f17c4) CASSIE_STEP_ENTRY(f17d7) CASSIE_STEP_ENTRY(d17d7) CASSIE_STEP_ENTRY(f17df) CASSIE_STEP_ENTRY(d17df) CASSIE_STEP_ENTRY(f17ff) CASSIE_STEP_ENTRY(d17ff)
+CASSIE_STEP_ENTRY(f1fc4) CASSIE_STEP_ENTRY(f1fd7) CASSIE_STEP_ENTRY(d1fd7) CASSIE_STEP_ENTRY(f1fdf) CASSIE_STEP_ENTRY(d1fdf) CASSIE_STEP_ENTRY(f1fff) CASSIE_STEP_ENTRY(d1fff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -49,6 +50,15 @@ template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_TC) {   // per-tick traces: the F_TC twins of the F_XF chain twins, by their rule (a batch with a trace always has applied rows)
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC; return dbl ? cassie_step_entry_d1fff() : cassie_step_entry_f1fff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC; return dbl ? cassie_step_entry_d1fdf() : cassie_step_entry_f1fdf(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC; return cassie_step_entry_f1fc4(); }
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC;
+    return dbl ? cassie_step_entry_d1fd7() : cassie_step_entry_f1fd7();
+  }
   if (feat & F_XF) {   // per-environment applied forces: the plain twins of f04 / f24 where those would run, else the F_XF twins of the F_CT instances by their rule
     const bool dbl = std::is_same<real, double>::value;
     if (inst != 1) {   // null: the batch runs the extended kind (step_range)
@@ -376,6 +386,12 @@ struct BatchBase {
   virtual bool get_applied_forces(double *xfrc, double *qfrc) = 0;
   virtual bool enable_applied_forces(bool on) = 0;
   virtual bool clear_applied_xfrc() = 0;
+  // per-tick trace (F_TC instances; an output): k columns (source, column), the last max_ticks ticks of every step launch; k = 0 drops it.  Checked as a
+  // whole before anything changes.  get copies [n][T][k]; trace_ticks is the number of slots the last step launch wrote
+  virtual bool set_trace(const int *source, const int *column, int k, int max_ticks) = 0;
+  virtual bool get_trace(double *out) = 0;
+  virtual int trace_ticks() const = 0;
+  virtual int trace_width() const = 0;   // T * k, 0 without a trace
   // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
   // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
   virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
@@ -446,11 +462,13 @@ template <typename real> struct Batch : BatchBase {
   bool ct_mech = false;                    // the mechanics rows were allocated by the contact setter (model values), and no mechanics call has written them since
   real *d_app = nullptr;                   // A.applied: [n][APPLIED_W] per-environment applied forces (state), allocated by the first applied-force verb (F_XF instances)
   bool xf_ct = false;                      // the contact rows were allocated for the chain twin (model values), and no contact call has written them since
+  bool tc_app = false;                     // the applied-force rows were allocated for the trace instances (zero), and no applied-force verb has written them since
+  int tc_ticks = 0;                        // slots the last step launch wrote into the trace rows (A.trace: [n][T][k], allocated by cassie_batch_set_trace)
   Snap *bank = nullptr;                    // the reset bank (cassie_batch_set_reset_bank): a snapshot of k entries
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -523,7 +541,8 @@ template <typename real> struct Batch : BatchBase {
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC), (int)cfg[ext].smem));
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC), (int)cfg[ext].smem));   // and their F_MC twins
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), (int)cfg[ext].smem));   // and their F_CT twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), (int)cfg[ext].smem)); }   // and their F_XF twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), (int)cfg[ext].smem));   // and their F_XF twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_TC), (int)cfg[ext].smem)); }   // and their F_TC twins
         if (ext != 1 && step_entry<real>(ext, feat | F_XF))   // the plain F_XF twins (applied forces), where this model runs f04 / f24
           CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF), (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
@@ -774,6 +793,7 @@ template <typename real> struct Batch : BatchBase {
   }
   // derived-quantity rows [n][AUX_W]: allocated on first use; while present every launch fills them (a few percent of a step)
   bool enable_aux(bool on) override {
+    if (!on && A.aux && ((A.trace.need >> TC_AUX) & 1)) { set_err("cassie_batch_enable_aux: a traced column reads the derived-quantity rows (cassie_batch_set_trace)"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (on && !A.aux) { CUDA_OK(cudaMalloc(&A.aux, sizeof(real) * n * AUX_W)); CUDA_OK(cudaMemsetAsync(A.aux, 0, sizeof(real) * n * AUX_W, stream)); }
     if (!on && A.aux) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.aux)); A.aux = nullptr; }
@@ -1490,6 +1510,7 @@ template <typename real> struct Batch : BatchBase {
   int ap_col(int i) const { const int nvm = h_model_copy.nv; return i < nvm ? i : 32 + (i - nvm); }   // host dof i -> its column in AP_QFRC
   bool enable_applied_forces(bool on) override {
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    tc_app = false;   // the rows are the caller's now, also when the trace allocated them
     if (on) {
       if (!d_app) { CUDA_OK(cudaMalloc(&d_app, sizeof(real) * n * APPLIED_W)); CUDA_OK(cudaMemset(d_app, 0, sizeof(real) * n * APPLIED_W)); }
       A.applied = d_app;
@@ -1538,6 +1559,55 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaMemset2DAsync(d_app + AP_XFRC, sizeof(real) * APPLIED_W, 0, sizeof(real) * AP_QFRC, n, stream)); CUDA_OK(cudaStreamSynchronize(stream));
     return true;
   }
+  // ---- per-tick trace: the rows are an output, written by step launches only.  The trace instances are the F_TC twins of the chain twins, so a batch
+  // with a trace carries applied-force rows (zero when it has none: tc_app) and, through them, model-valued contact, mechanics, actuator and offset rows
+  // (xf_ct); they are allocated here, so that a step allocates nothing, and dropped again with the trace unless a verb has written them since
+  bool trace_rows_for_twin() {
+    if (!d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }
+    if (!A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }
+    return true;
+  }
+  bool set_trace(const int *source, const int *column, int k, int max_ticks) override {
+    const std::string verb = "cassie_batch_set_trace: ";
+    if (legacy) { set_err(verb + "the batch belongs to a cassie_sim_t"); return false; }
+    if (k < 0 || k > TRACE_MAX) { set_err(verb + "between 0 and " + std::to_string(TRACE_MAX) + " columns"); return false; }
+    std::vector<int> codes((size_t)k);
+    int need = 0;
+    if (k > 0) {
+      if (!source || !column) { set_err(verb + "source and column are required"); return false; }
+      if (max_ticks < 1) { set_err(verb + "max_ticks must be at least 1"); return false; }
+      static const char *const names[TC_NSRC] = {"qpos", "qvel", "observation", "derived-quantity", "frame"};
+      for (int c = 0; c < k; c++) {
+        const int src = source[c], col = column[c];
+        if (src < 0 || src >= TC_NSRC) { set_err(verb + "column " + std::to_string(c) + ": unknown source " + std::to_string(src)); return false; }
+        if (src == TC_AUX && !A.aux) { set_err(verb + "column " + std::to_string(c) + ": derived-quantity columns need cassie_batch_enable_aux"); return false; }
+        if (src == TC_FRAME && !A.frames) { set_err(verb + "column " + std::to_string(c) + ": frame columns need cassie_batch_set_frames"); return false; }
+        const int width = src == TC_QPOS ? hm.nq : src == TC_QVEL ? hm.nv : src == TC_OBS ? OBS_W : src == TC_AUX ? AUX_W : A.nfr * FRAME_W;
+        if (col < 0 || col >= width) { set_err(verb + "column " + std::to_string(c) + ": " + names[src] + " column " + std::to_string(col) + " is outside 0.." + std::to_string(width - 1)); return false; }
+        codes[c] = (src << TC_SHIFT) | col;
+        if (src >= TC_OBS) need |= 1 << src;
+      }
+    }
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight writes the rows
+    CUDA_OK(cudaFree(A.trace.rows)); CUDA_OK(cudaFree((void *)A.trace.cols)); A.trace = TraceArgs<real>{}; tc_ticks = 0;
+    if (k == 0) {   // back to the instances that ran before
+      if (tc_app) { tc_app = false; return enable_applied_forces(false); }
+      return true;
+    }
+    if (!trace_rows_for_twin()) return false;
+    int *cols = nullptr;
+    CUDA_OK(cudaMalloc(&cols, sizeof(int) * k)); CUDA_OK(cudaMemcpy(cols, codes.data(), sizeof(int) * k, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc(&A.trace.rows, sizeof(real) * n * max_ticks * k)); CUDA_OK(cudaMemset(A.trace.rows, 0, sizeof(real) * n * max_ticks * k));
+    A.trace.cols = cols; A.trace.k = k; A.trace.T = max_ticks; A.trace.need = need;
+    return true;
+  }
+  bool get_trace(double *out) override {
+    if (!A.trace.rows) { set_err("cassie_batch_get_trace: no trace is set (cassie_batch_set_trace)"); return false; }
+    if (!out) { set_err("cassie_batch_get_trace: out is required"); return false; }
+    return d2h(A.trace.rows, A.trace.T * A.trace.k, A.trace.T * A.trace.k, 0, out);
+  }
+  int trace_ticks() const override { return tc_ticks; }
+  int trace_width() const override { return A.trace.T * A.trace.k; }
   // ---- the controller-stage state: the delay line, the encoders' filters (views of the cst / dfilt rows; snapshots carry them)
   bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) override {
     CUDA_OK(cudaSetDevice(device));
@@ -1575,6 +1645,7 @@ template <typename real> struct Batch : BatchBase {
   // ---- frame rows: the table is checked as a whole before anything changes; the rows start at zero and are filled by the next step / forward launch
   bool set_frames(const char *const *names, const int *kinds, int count) override {
     if (count < 0 || count > FRAME_MAX || (count > 0 && (!names || !kinds))) { set_err("cassie_batch_set_frames: between 0 and " + std::to_string(FRAME_MAX) + " frames, with names and kinds"); return false; }
+    if ((A.trace.need >> TC_FRAME) & 1) { set_err("cassie_batch_set_frames: a traced column reads the frame rows (cassie_batch_set_trace)"); return false; }
     std::vector<real> tab((size_t)count * FT_W); std::vector<int> list;
     for (int f = 0; f < count; f++) {
       std::string err; const int id = frame_table_row(hm, names[f], kinds[f], &tab[(size_t)f * FT_W], err);
@@ -1733,7 +1804,7 @@ template <typename real> struct Batch : BatchBase {
   int launch_kind(int mode) {
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
-    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || A.trace.rows || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
     // applied forces: a plain twin where f04 / f24 would run, else the chain twin
     if (A.applied && ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF)) ext = 1;
     return ext;
@@ -1745,16 +1816,18 @@ template <typename real> struct Batch : BatchBase {
     if (mode == 5 && !A.dyn) { set_err("the dynamics launch needs its rows (cassie_batch_dynamics)"); return false; }
     A.nsub = nsub_override;
     const int ext = launch_kind(mode);
+    if (A.trace.rows && !trace_rows_for_twin()) return false;   // only after a verb dropped the rows set_trace allocated
     if (A.applied && ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }   // the chain twin reads contact rows (the model's values when none were set)
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
     if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
+    if (mode == 0 && A.trace.rows) tc_ticks = nticks < A.trace.T ? nticks : A.trace.T;
     CUDA_OK(cudaGetLastError());
     return true;
   }
@@ -1821,6 +1894,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
     if (!strcmp(f, "applied")) return d_app;
+    if (!strcmp(f, "trace")) return A.trace.rows;
 #ifdef CASSIE_STAGE_CLOCKS
     if (!strcmp(f, "stage_clocks")) return A.qM;   // [n][2 NM_MAX] reals, words 0.. the stage clocks of the last step sub-step (step_core.inl STAGE_CLOCK)
 #endif
@@ -1852,6 +1926,7 @@ static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == 
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
 static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
+static_assert(CASSIE_TRACE_QPOS == TC_QPOS && CASSIE_TRACE_QVEL == TC_QVEL && CASSIE_TRACE_OBS == TC_OBS && CASSIE_TRACE_AUX == TC_AUX && CASSIE_TRACE_FRAME == TC_FRAME && CASSIE_TRACE_MAX == TRACE_MAX, "trace sources");
 static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
 struct cassie_batch { BatchBase *impl; std::vector<double> obs, radio; };
 struct cassie_sim { cassie_batch *b; double qpos[64], qvel[64], time, qpos_dev[64], qvel_dev[64], time_dev, aux[AUX_W]; std::vector<float> hfield, hfield_dev; std::string path; double timestep = 0, timestep_dev = 0;
@@ -1912,6 +1987,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
   if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
+  if (!strcmp(field, "trace")) return b->impl->trace_width();
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -2368,6 +2444,10 @@ int cassie_batch_clear_env_contact(cassie_batch_t *b) { return b->impl->clear_en
 int cassie_batch_set_applied_forces(cassie_batch_t *b, const double *xfrc, const double *qfrc, const unsigned char *mask) { return b->impl->set_applied_forces(xfrc, qfrc, mask) ? 0 : -1; }
 int cassie_batch_get_applied_forces(cassie_batch_t *b, double *xfrc, double *qfrc) { return b->impl->get_applied_forces(xfrc, qfrc) ? 0 : -1; }
 int cassie_batch_enable_applied_forces(cassie_batch_t *b, int on) { return b->impl->enable_applied_forces(on != 0) ? 0 : -1; }
+// per-tick traces of step launches; see include/cassie_b200.h
+int cassie_batch_set_trace(cassie_batch_t *b, const int *source, const int *column, int k, int max_ticks) { return b->impl->set_trace(source, column, k, max_ticks) ? 0 : -1; }
+int cassie_batch_trace_ticks(const cassie_batch_t *b) { return b->impl->trace_ticks(); }
+int cassie_batch_get_trace(cassie_batch_t *b, double *out) { return b->impl->get_trace(out) ? 0 : -1; }
 int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) { return b->impl->get_actuator_state(torque_delay, drive_filter, joint_x, joint_y) ? 0 : -1; }
 int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) {
   return b->impl->set_actuator_state(torque_delay, drive_filter, joint_x, joint_y, mask) ? 0 : -1; }

@@ -39,6 +39,7 @@ constexpr int F_AC = 128; // per-environment actuators: ctrlrange, no-load speed
 constexpr int F_MC = 256; // per-environment mechanics: link inertia, rotor armature and hinge springs come from a MECH_W row (with F_BP | F_AC, extended instances only)
 constexpr int F_CT = 512; // per-environment contact softness: each contact row mixes solref / solimp from its geoms' CONTACT_W slots (with F_BP | F_AC | F_MC, extended only)
 constexpr int F_XF = 1024; // per-environment applied forces: xfrc_applied / qfrc_applied from an APPLIED_W row (plain F_BOX twins, and extended with F_BP | F_AC | F_MC | F_CT)
+constexpr int F_TC = 2048; // per-tick trace: every tick of a step launch stores the traced columns into a TRACE row slot (the F_XF chain twins' twins only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -202,6 +203,12 @@ constexpr int CT_SOLREF = 0, CT_SOLIMP = 2, CT_SOLMIX = 7;
 // body 32..37, as the DYN columns).  State like qvel: resets zero it, snapshots carry it.  The XFRC slot keeps its meaning and adds to its body's entry.
 constexpr int APPLIED_W = 232;
 constexpr int AP_XFRC = 0, AP_QFRC = 192;
+// per-tick trace (optional, cassie_batch_set_trace; F_TC instances): per environment a row [T][k] of reals, slot s = what the traced columns held after
+// tick s of the last step launch (its last T ticks when it ran more).  Column c of the trace is described by the batch's table entry
+// (source << TC_SHIFT) | column; the sources below.  An output like the aux row: resets and snapshots leave it alone, only step launches write it.
+constexpr int TC_QPOS = 0, TC_QVEL = 1, TC_OBS = 2, TC_AUX = 3, TC_FRAME = 4, TC_NSRC = 5;
+constexpr int TC_SHIFT = 16, TC_COLMASK = 0xffff;
+constexpr int TRACE_MAX = 64;   // columns
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

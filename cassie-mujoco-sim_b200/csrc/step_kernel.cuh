@@ -29,6 +29,7 @@ template <typename real> struct EnvArrays {
   const real *mech;                           // [n][MECH_W] inertia, armature and hinge springs of each environment (F_MC instances)
   const real *contact;                        // [n][CONTACT_W] solref, solimp and solmix per collision geom of each environment (F_CT instances)
   const real *applied;                        // [n][APPLIED_W] xfrc_applied and qfrc_applied of each environment (F_XF instances)
+  TraceArgs<real> trace;                      // [n][T][k] per-tick trace rows and their column table (F_TC instances)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -118,8 +119,10 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     if (FEAT & F_MC) E.env = env;   // and the mechanics rows, at the cinert, CRB and passive phases, from A.mech
     if (FEAT & F_CT) E.env = env;   // and the contact rows, at the contact rows' constants, from A.contact
     if (FEAT & F_XF) E.env = env;   // and the applied-force rows, at the bias sum, the applied dof forces and the extra body's acceleration, from A.applied
+    if (FEAT & F_TC) E.env = env;   // and the trace rows, after every tick, from A.trace
     step_env<real, INST == 1, FEAT, INST >= 1>(cm, sm, E, qvel, qacc_ws, xqvel, xqacc_ws, nticks, mode, (FEAT & F_BP) ? A.bpos : (const real *)0, (FEAT & F_AC) ? A.act : (const real *)0,
-                                               (FEAT & F_MC) ? A.mech : (const real *)0, (FEAT & F_CT) ? A.contact : (const real *)0, (FEAT & F_XF) ? A.applied : (const real *)0);
+                                               (FEAT & F_MC) ? A.mech : (const real *)0, (FEAT & F_CT) ? A.contact : (const real *)0, (FEAT & F_XF) ? A.applied : (const real *)0,
+                                               (FEAT & F_TC) ? A.trace : TraceArgs<real>{});
     __syncwarp();
     if (mode >= 2) {   // query / set_const / frame Jacobian / dynamics: only the aux row / the constant row / the Jacobian row / the dynamics row is written
       if constexpr ((FEAT & F_FR) != 0) { if (mode == 5) dynamics_row(cm, sm, A.dyn, A.cenv, env, (FEAT & F_XB) ? cm.xb : -1); }   // from what mode 5's sub-step left in shared memory

@@ -688,6 +688,36 @@ int cassie_batch_clear_env_contact(cassie_batch_t *b);
 int cassie_batch_set_applied_forces(cassie_batch_t *b, const double *xfrc, const double *qfrc, const unsigned char *mask);
 int cassie_batch_get_applied_forces(cassie_batch_t *b, double *xfrc, double *qfrc);
 int cassie_batch_enable_applied_forces(cassie_batch_t *b, int on);
+/* Per-tick traces for multi-tick launches.  A step launch of nticks control ticks normally leaves only what its last tick wrote; with a trace, every
+ * tick stores k chosen columns per environment into the trace rows [n][T][k] (T = max_ticks), so that rewards and termination checks built from
+ * per-tick values (foot forces, foot positions, pelvis height, motor torques, ...) can be reduced on the device after one launch.  Column c is
+ * (source[c], column[c]):
+ *   CASSIE_TRACE_QPOS   qpos column (0 .. nq - 1) after the tick
+ *   CASSIE_TRACE_QVEL   qvel column (0 .. nv - 1) after the tick
+ *   CASSIE_TRACE_OBS    observation-row column (0 .. CASSIE_OBS_WIDTH - 1) of the tick: cassie_out / state_out numbers, estimator columns included
+ *   CASSIE_TRACE_AUX    derived-quantity column (0 .. CASSIE_AUX_WIDTH - 1) after the tick; needs cassie_batch_enable_aux first
+ *   CASSIE_TRACE_FRAME  frame-row column (0 .. nframes * CASSIE_FRAME_WIDTH - 1) after the tick; needs cassie_batch_set_frames first
+ * Slot s holds what the rows would hold had the launch stopped after that tick (what cassie_batch_get_* returns after a 1-tick launch).  A launch of
+ * nticks <= T writes slots 0 .. nticks - 1 and leaves the others alone; a longer one keeps its last T ticks, in order.  cassie_sim_step_pd_batch
+ * writes slot 0.  The rows are an output: only step launches write them; forward, query, set_const, Jacobian and dynamics launches, resets, set_state,
+ * reset_where and snapshots leave them alone.  set_trace allocates the rows (zeroed), so that a step allocates and synchronises nothing; k = 0 drops
+ * the trace.  0, or -1 with nothing changed (cassie_b200_last_error says why) for: an unknown source, a column outside its source's range, k outside
+ * 0 .. CASSIE_TRACE_MAX, max_ticks < 1 with k > 0, an aux or frame column without those rows, the batch of a cassie_sim_t.  While a traced column
+ * reads them, cassie_batch_enable_aux(b, 0) and cassie_batch_set_frames are refused.
+ * A traced batch runs the F_TC twins of the extended applied-force instances: it carries applied-force rows (zeroed ones when it has none, dropped
+ * again by k = 0 unless an applied-force verb has written them since) and, through them, model-valued contact rows as with applied forces; the
+ * physics is bitwise that of the same batch without a trace.  trace_ticks: the slots the last step launch wrote (min(nticks, T); 0 before the first).
+ * get_trace: synchronous host copy [n][T][k] doubles.  Device rows: cassie_batch_device_ptr(b, "trace"), [n][T * k] in the batch precision
+ * (cassie_batch_row_width(b, "trace") = T * k). */
+#define CASSIE_TRACE_QPOS 0
+#define CASSIE_TRACE_QVEL 1
+#define CASSIE_TRACE_OBS 2
+#define CASSIE_TRACE_AUX 3
+#define CASSIE_TRACE_FRAME 4
+#define CASSIE_TRACE_MAX 64
+int cassie_batch_set_trace(cassie_batch_t *b, const int *source, const int *column, int k, int max_ticks);
+int cassie_batch_trace_ticks(const cassie_batch_t *b);
+int cassie_batch_get_trace(cassie_batch_t *b, double *out);
 /* The controller-stage state of every environment, as the reference's cassie_sim_t holds it: the torque delay line torque_delay [n][10][6] (slot 0
  * newest), the drive encoders' integer FIR taps drive_filter [n][10][9], the joint encoders' IIR filters joint_x [n][6][4] and joint_y [n][6][3].
  * NULL parts are skipped; set changes masked environments only (mask NULL: all).  They are state: reset, snapshots and cassie_sim_copy carry them. */
@@ -696,7 +726,7 @@ int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_dela
                                     const unsigned char *mask);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232], "trace" [n][T * k]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
