@@ -29,6 +29,10 @@ RAY_FRAMES = dict(heading=RAY_HEADING, root=RAY_ROOT, world=RAY_WORLD)
 # depth camera (include/cassie_b200.h CASSIE_CAM_*): largest image side
 CAM_MAXDIM = 256
 DYN = dict(M=slice(0, 1600), bias=slice(1600, 1640), J_eq=slice(1640, 2120), eq_err=slice(2120, 2132), rcm=slice(2132, 2135))
+# inverse row (include/cassie_b200.h CASSIE_INV_*): qfrc_inverse [40], qfrc_constraint [40] (column = dof as in DYN), then the row count, the contacts with
+# rows and the contacts dropped at the capacities, as reals; padded to 96.  The input rows ('inv_qacc') are qvel-wide, column = dof
+INV_WIDTH, INV_COLS = 96, 40
+INV = dict(qfrc_inverse=slice(0, 40), qfrc_constraint=slice(40, 80), nefc=80, ncon=81, dropped=82)
 # acceleration row (include/cassie_b200.h CASSIE_ACC_*): qacc [40] (column = dof), then per frame f a slot of ACC_SLOT at ACC_QCOLS + ACC_SLOT f holding
 # cacc [6] (com-based [angular; linear]) and 2 pad.  ACC['qacc'] slices the row, ACC['cacc'] a frame's slot
 ACC_QCOLS, ACC_SLOT = 40, 8
@@ -879,6 +883,30 @@ class CassieBatch:
             raise RuntimeError(_last_error())
         return out
 
+    # ---- inverse dynamics at the current state (MuJoCo 2.1.0's mj_inverse, continuous time): the generalised force that produces a given qacc, contact and
+    # loop-closure forces included; applied forces and actuation are part of what it returns
+    def compute_inverse(self, qacc=None):
+        """enqueue one inverse launch on the batch's stream (asynchronous) at the CURRENT state: qacc [n, nv] (host) is uploaded first; None uses
+        torch_view('inv_qacc') as the caller left it on the device (for example copied from torch_view('acc')[:, ACC['qacc']]), with no host
+        synchronisation, copy or allocation after the first call.  The result goes to the device rows (torch_view('inv')); nothing else is written"""
+        self.L.cassie_batch_inverse.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        a = None
+        if qacc is not None:
+            a = np.ascontiguousarray(np.asarray(qacc, dtype=np.float64).reshape(self.n, self.nv))
+        if self.L.cassie_batch_inverse(self.h, self._dp(a) if a is not None else None) != 0:
+            raise RuntimeError(_last_error())
+
+    def inverse(self):
+        """what the last compute_inverse() wrote, as numpy arrays: qfrc_inverse [n, nv] (M qacc + qfrc_bias - qfrc_passive - qfrc_constraint),
+        qfrc_constraint [n, nv], and per environment nefc, ncon and dropped [n] (constraint rows, contacts with rows, contacts dropped at the capacities)"""
+        out = dict(qfrc_inverse=np.zeros((self.n, self.nv)), qfrc_constraint=np.zeros((self.n, self.nv)))
+        counts = np.zeros((self.n, 3), dtype=np.int32)
+        self.L.cassie_batch_get_inverse.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int)]
+        if self.L.cassie_batch_get_inverse(self.h, self._dp(out['qfrc_inverse']), self._dp(out['qfrc_constraint']), counts.ctypes.data_as(C.POINTER(C.c_int))) != 0:
+            raise RuntimeError(_last_error())
+        out.update(nefc=counts[:, 0].copy(), ncon=counts[:, 1].copy(), dropped=counts[:, 2].copy())
+        return out
+
     # ---- terrain rays (height scans; the reference's rangefinders, example/cassiemujoco.py sense_ground): cast against each environment's static
     # geoms (floor, height field, boxes, with its own placement and terrain) at the CURRENT state; the robot and the extra free body are not seen
     def set_rays(self, origin, direction, frame='heading', max_dist=3.0):
@@ -1128,7 +1156,8 @@ class CassieBatch:
         32 slots of 8 -- solref[2], solimp[5], solmix -- one per device collision geom (moving 0..15, static 16..31; unused slots zero), read at the next
         launch; set_env_contact first; applied [n, 232]: xfrc_applied[32][6] in model body order, then qfrc_applied[40] by dof column (main tree 0..31,
         the extra free body 32..37), read at the next launch; set_applied_forces or enable_applied_forces first; trace [n, T, k]: the per-tick trace of
-        the last step launch, slot s of every environment, written by step launches only; set_trace first).  set_frames /
+        the last step launch, slot s of every environment, written by step launches only; set_trace first; inv_qacc [n, qvel width]: the qacc of
+        compute_inverse(None), column = dof; inv [n, INV_WIDTH] laid out as INV; both allocated by the first request).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),

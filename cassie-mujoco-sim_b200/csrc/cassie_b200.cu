@@ -401,6 +401,11 @@ struct BatchBase {
   virtual bool dynamics() = 0;                                                            // one launch of mode 5 (asynchronous): the dynamics rows [n][DYN_W]
   virtual bool get_dynamics(double *M, double *bias, double *J_eq, double *eq_err, double *Icm) = 0;   // what the last mode-5 launch wrote; any pointer may be null
   bool dyn_done = false;                                // a mode-5 launch was enqueued since the rows were allocated
+  // inverse dynamics (mode 6): qacc [n][nv] uploaded into the inverse-input rows [n][qvel width], or null: those rows as the caller left them on the
+  // device; then one launch (asynchronous).  get_inverse: qfrc_inverse, qfrc_constraint [n][nv] and counts [n][3] of the last launch; any may be null
+  virtual bool inverse(const double *qacc) = 0;
+  virtual bool get_inverse(double *qfrc_inverse, double *qfrc_constraint, int *counts) = 0;
+  bool inv_done = false;                                // a mode-6 launch was enqueued since the rows were allocated
   // acceleration rows [n][acc_width(count)]: allocated (zero) by enable_accelerations(true), filled by every step / forward launch, reallocated by set_frames
   virtual bool enable_accelerations(bool on) = 0;
   virtual bool get_accelerations(double *qacc, double *cacc) = 0;   // qacc [n][nv], cacc [n][count][6]; either may be null
@@ -432,6 +437,8 @@ static cudaError_t raise_smem_limit(const void *entry, int bytes) {
 
 template <typename real> struct Batch : BatchBase {
   DevModel<real> *d_model = nullptr; EnvArrays<real> A{}; int QW = QPOS_W_MAIN, VW = QVEL_W_MAIN;
+  real *d_iq = nullptr;   // inverse-input rows [n][VW]: the qacc of the next mode-6 launch, which passes them as its warm start
+  real *d_idbg = nullptr, *d_icst = nullptr; int *d_icnt = nullptr;   // a mode-6 launch's stage dump [n][D_SIZE], controller state [n][CST_W], counters [n][8]
   struct LaunchCfg { int wpb = 1; size_t smem = 0; int resident_ctas = 1; } cfg[3];   // [0] plain instance, [1] extended instance, [2] plain + estimator
   int feat = F_ALL;   // model features (F_XB | F_HFIELD | F_BOX): selects the kernel instance
   std::vector<real> h_tmp;
@@ -468,7 +475,7 @@ template <typename real> struct Batch : BatchBase {
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -1729,6 +1736,46 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
+  // inverse dynamics at the current state of every environment and the qacc of the inverse-input rows: one mode-6 launch on the batch stream.  The input
+  // and output rows and the launch's scratch rows are allocated (the rows zeroed) on first use, by this or by the device pointers, freed with the batch;
+  // snapshots and resets leave them alone.
+  bool alloc_inverse() {
+    CUDA_OK(cudaSetDevice(device));
+    if (d_iq) return true;
+    CUDA_OK(cudaMalloc(&d_iq, sizeof(real) * n * VW)); CUDA_OK(cudaMemsetAsync(d_iq, 0, sizeof(real) * n * VW, stream));
+    CUDA_OK(cudaMalloc(&A.inv, sizeof(real) * n * INV_W)); CUDA_OK(cudaMemsetAsync(A.inv, 0, sizeof(real) * n * INV_W, stream));
+    CUDA_OK(cudaMalloc(&d_idbg, sizeof(real) * n * D_SIZE)); CUDA_OK(cudaMalloc(&d_icst, sizeof(real) * n * CST_W));
+    CUDA_OK(cudaMalloc(&d_icnt, sizeof(int) * n * 8)); CUDA_OK(cudaMemsetAsync(d_icnt, 0, sizeof(int) * n * 8, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));   // zeroed before a caller writes the input rows on another stream
+    return true;
+  }
+  bool inverse(const double *qacc) override {
+    if (!qacc && !d_iq) { set_err("cassie_batch_inverse: no qacc: pass one, or write the rows of cassie_batch_device_ptr(b, \"inv_qacc\") first"); return false; }
+    if (!alloc_inverse()) return false;
+    if (qacc) {
+      const int nv = hm.nv;
+      h_tmp.assign((size_t)n * VW, 0);
+      for (int e = 0; e < n; e++) for (int i = 0; i < nv; i++) h_tmp[(size_t)e * VW + i] = (real)qacc[(size_t)e * nv + i];   // column = dof (the extra body at 32..37)
+      CUDA_OK(cudaMemcpyAsync(d_iq, h_tmp.data(), sizeof(real) * n * VW, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    }
+    if (!step(0, 6)) return false;
+    inv_done = true;
+    return true;
+  }
+  bool get_inverse(double *qfrc_inverse, double *qfrc_constraint, int *counts) override {
+    if (!inv_done) { set_err("cassie_batch_get_inverse: no inverse launch yet (cassie_batch_inverse)"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    h_tmp.resize((size_t)n * INV_W);
+    CUDA_OK(cudaMemcpyAsync(h_tmp.data(), A.inv, sizeof(real) * n * INV_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    const int nv = hm.nv;
+    for (int e = 0; e < n; e++) {
+      const real *r = &h_tmp[(size_t)e * INV_W];
+      if (qfrc_inverse) for (int i = 0; i < nv; i++) qfrc_inverse[(size_t)e * nv + i] = (double)r[IV_QFRC + i];
+      if (qfrc_constraint) for (int i = 0; i < nv; i++) qfrc_constraint[(size_t)e * nv + i] = (double)r[IV_QFRCC + i];
+      if (counts) { counts[3 * e] = (int)r[IV_NEFC]; counts[3 * e + 1] = (int)r[IV_NCON]; counts[3 * e + 2] = (int)r[IV_DROPPED]; }
+    }
+    return true;
+  }
   bool set_rays(const int *frame, const double *origin, const double *dir, const double *max_dist, int k) override {
     std::vector<double> tab; std::string err;
     if (!ray_table(frame, origin, dir, max_dist, k, tab, err)) { set_err("cassie_batch_set_rays: " + err); return false; }
@@ -1814,6 +1861,7 @@ template <typename real> struct Batch : BatchBase {
     if (mode == 2 && !A.aux) { set_err("query needs the derived-quantity rows (cassie_batch_enable_aux)"); return false; }
     if (mode == 4 && (!A.frames || !A.jac)) { set_err("the frame Jacobian needs frames (cassie_batch_set_frames)"); return false; }
     if (mode == 5 && !A.dyn) { set_err("the dynamics launch needs its rows (cassie_batch_dynamics)"); return false; }
+    if (mode == 6 && !d_iq) { set_err("the inverse launch needs its rows (cassie_batch_inverse)"); return false; }
     A.nsub = nsub_override;
     const int ext = launch_kind(mode);
     if (A.trace.rows && !trace_rows_for_twin()) return false;   // only after a verb dropped the rows set_trace allocated
@@ -1822,8 +1870,11 @@ template <typename real> struct Batch : BatchBase {
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
     EnvArrays<real> La = A; La.env0 = env0; La.n = count;   // the argument block of this launch
-    if (mode == 5) La.dbg = nullptr;   // the dynamics launch writes its rows only, also in a debug batch
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | ((A.frames || A.acc || mode == 5) ? F_FR : 0);   // frame, acceleration and dynamics rows: the extended F_FR instance (set_const launches too: they write no frames)
+    if (mode == 5 || mode == 6) La.dbg = nullptr;   // the dynamics and inverse launches write their rows only, also in a debug batch
+    // mode 6: the caller's qacc reaches the lanes through the warm-start load (mode 6 writes no state back); the forward's stage dump, sensor data and
+    // counters go to the launch's scratch rows, for inverse_row; no aux or frame rows
+    if (mode == 6) { La.qacc_ws = d_iq; La.dbg = d_idbg; La.cst = d_icst; La.counters = d_icnt; La.aux = nullptr; La.nfr = 0; }
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | ((A.frames || A.acc || mode == 5 || mode == 6) ? F_FR : 0);   // frame, acceleration, dynamics and inverse rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1894,6 +1945,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
     if (!strcmp(f, "applied")) return d_app;
+    if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
 #ifdef CASSIE_STAGE_CLOCKS
     if (!strcmp(f, "stage_clocks")) return A.qM;   // [n][2 NM_MAX] reals, words 0.. the stage clocks of the last step sub-step (step_core.inl STAGE_CLOCK)
@@ -1924,6 +1976,7 @@ static_assert(CASSIE_CAM_MAXDIM == CAM_MAXDIM, "camera image size");
 static_assert(CASSIE_RAY_MAX == RAY_MAX && CASSIE_RAY_SLOT == RAY_SLOT && CASSIE_RAY_HEADING == RAY_HEADING && CASSIE_RAY_ROOT == RAY_ROOT && CASSIE_RAY_WORLD == RAY_WORLD, "ray table and rows");
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
+static_assert(CASSIE_INV_WIDTH == INV_W && CASSIE_INV_COLS == IV_COLS && CASSIE_INV_QFRC == IV_QFRC && CASSIE_INV_QFRCC == IV_QFRCC && CASSIE_INV_NEFC == IV_NEFC && CASSIE_INV_NCON == IV_NCON && CASSIE_INV_DROPPED == IV_DROPPED, "inverse row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
 static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
 static_assert(CASSIE_TRACE_QPOS == TC_QPOS && CASSIE_TRACE_QVEL == TC_QVEL && CASSIE_TRACE_OBS == TC_OBS && CASSIE_TRACE_AUX == TC_AUX && CASSIE_TRACE_FRAME == TC_FRAME && CASSIE_TRACE_MAX == TRACE_MAX, "trace sources");
@@ -1988,6 +2041,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
   if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "trace")) return b->impl->trace_width();
+  if (!strcmp(field, "inv_qacc")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN; if (!strcmp(field, "inv")) return INV_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
 long cassie_batch_launch_count(const cassie_batch_t *b) { return b->impl->launches; }
@@ -2487,6 +2541,8 @@ int cassie_batch_render_depth(cassie_batch_t *b) { return b->impl->render_depth(
 int cassie_batch_get_depth(cassie_batch_t *b, double *out) { return b->impl->get_depth(out) ? 0 : -1; }
 int cassie_batch_dynamics(cassie_batch_t *b) { return b->impl->dynamics() ? 0 : -1; }
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm) { return b->impl->get_dynamics(M, bias, J_eq, eq_err, Icm) ? 0 : -1; }
+int cassie_batch_inverse(cassie_batch_t *b, const double *qacc) { return b->impl->inverse(qacc) ? 0 : -1; }
+int cassie_batch_get_inverse(cassie_batch_t *b, double *qfrc_inverse, double *qfrc_constraint, int *counts) { return b->impl->get_inverse(qfrc_inverse, qfrc_constraint, counts) ? 0 : -1; }
 int cassie_batch_neq(const cassie_batch_t *b) { return b->impl->hm.neq; }
 int cassie_batch_enable_accelerations(cassie_batch_t *b, int on) { return b->impl->enable_accelerations(on != 0) ? 0 : -1; }
 int cassie_batch_get_accelerations(cassie_batch_t *b, double *qacc, double *cacc) { return b->impl->get_accelerations(qacc, cacc) ? 0 : -1; }

@@ -230,6 +230,13 @@ constexpr int FRAME_JAC_W = 6 * FJ_COLS;
 constexpr int DY_COLS = 40, DY_EQ_ROWS = 3 * ME;
 constexpr int DY_M = 0, DY_BIAS = DY_M + DY_COLS * DY_COLS, DY_JEQ = DY_BIAS + DY_COLS, DY_EQPOS = DY_JEQ + DY_EQ_ROWS * DY_COLS, DY_RCM = DY_EQPOS + DY_EQ_ROWS;
 constexpr int DYN_W = (DY_RCM + 3 + 31) / 32 * 32;
+// inverse dynamics at the current state and a caller's qacc (launch mode 6, cassie_batch_inverse; mj_inverse of MuJoCo 2.1.0): per environment
+// qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint and qfrc_constraint = J' f of the constraint rows at that qacc, column = dof as in the
+// dynamics row, then the row count, the contacts with rows and the contacts dropped at the capacities, as reals; the row is padded to a multiple of 32.
+// The caller's qacc comes from the batch's inverse-input rows [n][qvel width], which the launch passes as its warm start
+constexpr int IV_COLS = 40;
+constexpr int IV_QFRC = 0, IV_QFRCC = IV_QFRC + IV_COLS, IV_NEFC = IV_QFRCC + IV_COLS, IV_NCON = IV_NEFC + 1, IV_DROPPED = IV_NCON + 1;
+constexpr int INV_W = (IV_DROPPED + 1 + 31) / 32 * 32;
 // accelerations (optional, cassie_batch_enable_accelerations): per environment a row [ACC_W(count)] filled in the last sub-step of a step or forward
 // launch (F_FR instances): the constraint-solved qacc (cassie_sim_qacc, src/cassiemujoco.c:1216-1219; column = dof as in the dynamics row, zeros beyond
 // nv), then per frame of the batch's frame list cacc after mj_comVel + mj_rnePostConstraint (cassie_sim_body_acceleration, :1762-1771) in com-based

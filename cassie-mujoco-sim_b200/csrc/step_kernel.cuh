@@ -30,6 +30,8 @@ template <typename real> struct EnvArrays {
   const real *contact;                        // [n][CONTACT_W] solref, solimp and solmix per collision geom of each environment (F_CT instances)
   const real *applied;                        // [n][APPLIED_W] xfrc_applied and qfrc_applied of each environment (F_XF instances)
   TraceArgs<real> trace;                      // [n][T][k] per-tick trace rows and their column table (F_TC instances)
+  real *inv;                                  // mode 6: inverse rows [n][INV_W] (F_FR instances); the launch's qacc_ws is the batch's inverse input, its
+                                              // dbg, cst and counters are scratch rows
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -53,7 +55,7 @@ __device__ __forceinline__ void tma_stage(void *dst_smem, const void *src_gmem, 
 template <typename real> __host__ __device__ constexpr size_t model_bytes() { return (sizeof(DevModel<real>) + 127) / 128 * 128; }
 template <typename real> __host__ __device__ constexpr size_t warp_bytes(int ystride, bool ext) { return ((size_t)(ext ? scratch_reals_ext(ystride) : scratch_reals(ystride)) * sizeof(real) + 127) / 128 * 128; }
 
-// mode 0: step nticks; mode 1: mj_forward only; 2 / 3 / 4 / 5: query, set_const, frame Jacobian, dynamics row (see mj_substep).  INST: 0 plain instance, 1 extended instance (per-env constants, derived quantities, task PD, set_const,
+// mode 0: step nticks; mode 1: mj_forward only; 2 / 3 / 4 / 5 / 6: query, set_const, frame Jacobian, dynamics row, inverse row (see mj_substep).  INST: 0 plain instance, 1 extended instance (per-env constants, derived quantities, task PD, set_const,
 // estimator), 2 plain instance + estimator stage (what cassie_sim_step_pd_batch runs when nothing else asks for the extended one)
 template <typename real, int INST, int FEAT>
 __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *__restrict__ gmodel, EnvArrays<real> A, int nticks, int mode) {
@@ -124,8 +126,11 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
                                                (FEAT & F_MC) ? A.mech : (const real *)0, (FEAT & F_CT) ? A.contact : (const real *)0, (FEAT & F_XF) ? A.applied : (const real *)0,
                                                (FEAT & F_TC) ? A.trace : TraceArgs<real>{});
     __syncwarp();
-    if (mode >= 2) {   // query / set_const / frame Jacobian / dynamics: only the aux row / the constant row / the Jacobian row / the dynamics row is written
-      if constexpr ((FEAT & F_FR) != 0) { if (mode == 5) dynamics_row(cm, sm, A.dyn, A.cenv, env, (FEAT & F_XB) ? cm.xb : -1); }   // from what mode 5's sub-step left in shared memory
+    if (mode >= 2) {   // query / set_const / frame Jacobian / dynamics / inverse: only the aux row / the constant row / the Jacobian row / the dynamics row / the inverse row is written
+      if constexpr ((FEAT & F_FR) != 0) {   // from what mode 5's / mode 6's sub-step left in shared memory (mode 6: and in its scratch rows)
+        if (mode == 5) dynamics_row(cm, sm, A.dyn, A.cenv, env, (FEAT & F_XB) ? cm.xb : -1);
+        else if (mode == 6) inverse_row(cm, sm, A.inv, A.cenv, A.dbg, A.qacc_ws, A.counters, env);
+      }
       continue;
     }
     for (int i = l; i < qw; i += 32) A.qpos[(size_t)env * qw + i] = sm[S_QPOS + i];

@@ -171,6 +171,39 @@ int cassie_batch_frame_jacobian(cassie_batch_t *b, int frame, double *jacp, doub
 int cassie_batch_dynamics(cassie_batch_t *b);
 int cassie_batch_get_dynamics(cassie_batch_t *b, double *M, double *bias, double *J_eq, double *eq_err, double *Icm);
 int cassie_batch_neq(const cassie_batch_t *b);
+/* Inverse dynamics at the CURRENT state of every environment and a caller's joint acceleration, as MuJoCo 2.1.0's mj_inverse (continuous time): the
+ * generalised force that produces qacc there, for torque labels of reference motions, system identification from logs, holding torques and forward /
+ * inverse consistency checks.  With the constraint rows of the state (connect equalities, joint limits, contacts with the environment's own softness,
+ * friction and terrain; the forward's capacities of 48 rows and 12 contacts) evaluated at that qacc, as mj_constraintUpdate does:
+ *   jar = J qacc - aref;  f = -jar / R on equality rows; on limit and contact rows f = -jar / R if jar < 0, else 0;  qfrc_constraint = J' f
+ *   qfrc_inverse = M qacc + qfrc_bias - qfrc_passive - qfrc_constraint   (M with the armature; passive: damping and springs)
+ * Applied forces (xfrc_applied, qfrc_applied, the XFRC slot) and actuation are not subtracted: they are part of what qfrc_inverse returns, as in MuJoCo.
+ * At the qacc of the acceleration rows (the continuous-time one, before mj_Euler's implicit-damping correction) it gives back the forward's actuator
+ * and applied forces, to solver accuracy.  The extra free body's block is diag(m, m, m, I1, I2, I3) qacc + [-m g; w x I w] minus its constraint
+ * columns.  Every per-environment row of the model is honoured (masses, inertial offsets, damping, body offsets, inertia, armature, springs, contact
+ * softness, static geoms, terrain).
+ * cassie_batch_inverse: qacc [n][nv] (host) is uploaded into the inverse-input rows, then one launch on the batch stream (asynchronous).  qacc NULL:
+ * the inverse-input rows as the caller left them, for example copied on the device from the acceleration rows; after the first call that path
+ * synchronises, copies and allocates nothing.  It writes nothing else (state, warm start, observations, aux, frame and acceleration rows, counters).
+ * 0, or -1 (cassie_b200_last_error): NULL before the input rows exist.
+ * cassie_batch_get_inverse: synchronous copy of what the last inverse launch wrote: qfrc_inverse [n][nv], qfrc_constraint [n][nv], counts [n][3] (rows,
+ * contacts with rows, contacts dropped at the capacities: a lying-flat environment can be discarded); any pointer may be NULL.  -1 before any inverse
+ * launch.  Device rows, in the batch precision, allocated (zero) by the first call or device-pointer request, freed with the batch, left alone by
+ * snapshots and resets:
+ *   cassie_batch_device_ptr(b, "inv_qacc") [n][cassie_batch_row_width(b, "qvel")]  the input: column = dof (main tree 0..31, the extra free body 32..37)
+ *   cassie_batch_device_ptr(b, "inv")      [n][CASSIE_INV_WIDTH]                    the output, column = dof as in the dynamics row, unused entries zero:
+ *   CASSIE_INV_QFRC    [40]  qfrc_inverse
+ *   CASSIE_INV_QFRCC   [40]  qfrc_constraint
+ *   CASSIE_INV_NEFC, CASSIE_INV_NCON, CASSIE_INV_DROPPED  [1] each: the counts, as reals */
+#define CASSIE_INV_COLS 40
+#define CASSIE_INV_QFRC 0
+#define CASSIE_INV_QFRCC 40
+#define CASSIE_INV_NEFC 80
+#define CASSIE_INV_NCON 81
+#define CASSIE_INV_DROPPED 82
+#define CASSIE_INV_WIDTH 96
+int cassie_batch_inverse(cassie_batch_t *b, const double *qacc);
+int cassie_batch_get_inverse(cassie_batch_t *b, double *qfrc_inverse, double *qfrc_constraint, int *counts);
 /* Accelerations, as step / forward by-products (joint-acceleration penalties, impact rewards, IMU-like observations at any body, acceleration-level
  * controllers): per environment a row [CASSIE_ACC_WIDTH(count)] in the batch precision, count = cassie_batch_nframes, filled in the last physics sub-step
  * of every step and forward launch (also the forward of cassie_batch_reset):
@@ -726,7 +759,7 @@ int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_dela
                                     const unsigned char *mask);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232], "trace" [n][T * k]) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232], "trace" [n][T * k], "inv_qacc" [n][32] ([n][40]), "inv" [n][96]; the inverse rows are allocated by the request) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
