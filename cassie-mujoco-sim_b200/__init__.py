@@ -48,6 +48,10 @@ AUX = dict(foot_force=slice(0, 12), toe_force=slice(12, 18), heel_force=slice(18
 # per-tick trace sources (include/cassie_b200.h CASSIE_TRACE_*): CassieBatch.set_trace columns are (source, column) pairs, columns as OBS / AUX / FRAME slice
 # the rows (a frame column is frame * FRAME_WIDTH + an offset of FRAME)
 TRACE_QPOS, TRACE_QVEL, TRACE_OBS, TRACE_AUX, TRACE_FRAME, TRACE_MAX = 0, 1, 2, 3, 4, 64
+# contact-list row layout (include/cassie_b200.h CASSIE_CON_*): a header of CON_HEAD reals (listed, found, dropped), then CON_MAX slots of CON_SLOT reals;
+# CON slices a slot
+CON_HEAD, CON_SLOT, CON_MAX, CON_WIDTH = 8, 24, 12, 296
+CON = dict(geom1=0, geom2=1, dim=2, dist=3, pos=slice(4, 7), frame=slice(7, 16), force=slice(16, 22), mu=22, efc=23)
 # observation row layout (cassie_batch_get_obs)
 OBS = dict(motor_pos=slice(0, 10), motor_vel=slice(10, 20), motor_torque=slice(20, 30), joint_pos=slice(30, 36), joint_vel=slice(36, 42),
            quat=slice(42, 46), gyro=slice(46, 49), accel=slice(49, 52), mag=slice(52, 55), time=55,
@@ -764,6 +768,52 @@ class CassieBatch:
             raise RuntimeError(_last_error())
         return out[:, :self.trace_ticks()]
 
+    # ---- contact lists of step and forward launches
+    def _contacts_lib(self):
+        L = self.L
+        if not getattr(L, '_contacts_bound', False):
+            vp = C.c_void_p
+            L.cassie_batch_enable_contacts.argtypes = [vp, C.c_int]
+            L.cassie_batch_get_contacts.argtypes = [vp, C.POINTER(C.c_double)]
+            L.cassie_batch_name2id.argtypes = [vp, C.c_char_p, C.c_char_p]
+            L.cassie_batch_id2name.argtypes = [vp, C.c_char_p, C.c_int]
+            L.cassie_batch_id2name.restype = C.c_char_p
+            for n in ('enable_contacts', 'get_contacts', 'name2id'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._contacts_bound = True
+        return L
+
+    def enable_contacts(self, on=True):
+        """contact-list rows: every step and forward launch then lists the contacts of its last sub-step (contacts()); on=False frees them and the
+        batch runs the instance it ran before.  A batch with a per-tick trace refuses them.  See include/cassie_b200.h."""
+        if self._contacts_lib().cassie_batch_enable_contacts(self.h, 1 if on else 0) != 0:
+            raise RuntimeError(_last_error())
+
+    def contacts(self):
+        """dict of the contact lists (a synchronous copy): count, found, dropped [n]; geom [n, 12, 2] int (model geom ids, -1 in unused slots); dim,
+        dist, mu [n, 12]; pos [n, 12, 3]; frame [n, 12, 3, 3] (row 0 the normal from geom1 to geom2); force [n, 12, 6] (mj_contactForce, contact
+        frame); world_force [n, 12, 3] = frame' force[:3], the force on geom2 in the world frame; efc [n, 12] int (first constraint row)"""
+        rows = np.zeros((self.n, CON_WIDTH))
+        if self._contacts_lib().cassie_batch_get_contacts(self.h, self._dp(rows)) != 0:
+            raise RuntimeError(_last_error())
+        s = rows[:, CON_HEAD:].reshape(self.n, CON_MAX, CON_SLOT)
+        frame = s[:, :, CON['frame']].reshape(self.n, CON_MAX, 3, 3)
+        force = s[:, :, CON['force']].copy()
+        return dict(count=rows[:, 0].astype(int), found=rows[:, 1].astype(int), dropped=rows[:, 2].astype(int),
+                    geom=s[:, :, 0:2].astype(int), dim=s[:, :, CON['dim']].astype(int), dist=s[:, :, CON['dist']].copy(), mu=s[:, :, CON['mu']].copy(),
+                    efc=s[:, :, CON['efc']].astype(int), pos=s[:, :, CON['pos']].copy(), frame=frame.copy(), force=force,
+                    world_force=np.einsum('ecji,ecj->eci', frame, force[:, :, :3]))
+
+    def name2id(self, kind, name):
+        """id of a named body ('body' / 'xbody'), joint, geom, site or camera of the compiled model, or -1: an unknown name, or a kind the compiled
+        model keeps no names of (mj_name2id)"""
+        return int(self._contacts_lib().cassie_batch_name2id(self.h, kind.encode(), name.encode()))
+
+    def id2name(self, kind, i):
+        """name of object i of a kind name2id resolves, or None: out of range, unnamed, or a kind without names (mj_id2name)"""
+        r = self._contacts_lib().cassie_batch_id2name(self.h, kind.encode(), int(i))
+        return None if r is None else r.decode()
+
     def actuator_state(self):
         """dict of the controller-stage state: torque_delay [n, 10, 6] (slot 0 newest), drive_filter [n, 10, 9] int32, joint_x [n, 6, 4], joint_y [n, 6, 3]"""
         L = self._act_lib()
@@ -1157,7 +1207,8 @@ class CassieBatch:
         launch; set_env_contact first; applied [n, 232]: xfrc_applied[32][6] in model body order, then qfrc_applied[40] by dof column (main tree 0..31,
         the extra free body 32..37), read at the next launch; set_applied_forces or enable_applied_forces first; trace [n, T, k]: the per-tick trace of
         the last step launch, slot s of every environment, written by step launches only; set_trace first; inv_qacc [n, qvel width]: the qacc of
-        compute_inverse(None), column = dof; inv [n, INV_WIDTH] laid out as INV; both allocated by the first request).  set_frames /
+        compute_inverse(None), column = dof; inv [n, INV_WIDTH] laid out as INV; both allocated by the first request; contacts [n, CON_WIDTH]: the contact
+        lists of the last step / forward launch, a header and CON_MAX slots laid out as CON; enable_contacts first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -1167,7 +1218,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field == 'terrain':
             ts = '<i4'
@@ -1301,6 +1352,12 @@ class CassieSim:
 
     def time(self):
         return self.L.cassie_sim_time(self.c)[0]
+
+    def mj_name2id(self, obj_type, name):
+        """id of a named body, joint, geom, site or camera, or -1 (reference: example/cassiemujoco.py:821-822)"""
+        self.L.cassie_sim_mj_name2id.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
+        self.L.cassie_sim_mj_name2id.restype = C.c_int
+        return int(self.L.cassie_sim_mj_name2id(self.c, obj_type.encode(), name.encode()))
 
     def qpos(self):
         return np.array(self.L.cassie_sim_qpos(self.c)[:self.nq])

@@ -63,6 +63,12 @@ APPLIED_INSTANCES = [('f0404', 'float', 0, 1028), ('f2404', 'float', 2, 1028),
 # tag = precision, kind, features in hex
 TRACE_INSTANCES = [('f1fc4', 'float', 1, 4036), ('f1fd7', 'float', 1, 4055), ('d1fd7', 'double', 1, 4055), ('f1fdf', 'float', 1, 4063), ('d1fdf', 'double', 1, 4063),
                    ('f1fff', 'float', 1, 4095), ('d1fff', 'double', 1, 4095)]
+# contact lists (feature 4096 = F_CL; cassie_batch_enable_contacts): the last sub-step of a step or forward launch stores MuJoCo's contact list and
+# mj_contactForce into the contact-list rows.  Any batch with contact lists runs one of these, each the F_CL twin of one F_FR chain twin of
+# APPLIED_INSTANCES (f17d7 / d17d7, f17df / d17df, f17ff / d17ff), with the model-valued applied, contact, mechanics, actuator and offset rows the chain
+# twins read; tag = precision, kind, features in hex
+CONTACT_LIST_INSTANCES = [('f117d7', 'float', 1, 6103), ('d117d7', 'double', 1, 6103), ('f117df', 'float', 1, 6111), ('d117df', 'double', 1, 6111),
+                          ('f117ff', 'float', 1, 6143), ('d117ff', 'double', 1, 6143)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -96,7 +102,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES + APPLIED_INSTANCES + TRACE_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES + APPLIED_INSTANCES + TRACE_INSTANCES + CONTACT_LIST_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

@@ -40,6 +40,7 @@ CASSIE_STEP_ENTRY(f13c4) CASSIE_STEP_ENTRY(f13d7) CASSIE_STEP_ENTRY(d13d7) CASSI
 CASSIE_STEP_ENTRY(f0404) CASSIE_STEP_ENTRY(f2404)
 CASSIE_STEP_ENTRY(f17c4) CASSIE_STEP_ENTRY(f17d7) CASSIE_STEP_ENTRY(d17d7) CASSIE_STEP_ENTRY(f17df) CASSIE_STEP_ENTRY(d17df) CASSIE_STEP_ENTRY(f17ff) CASSIE_STEP_ENTRY(d17ff)
 CASSIE_STEP_ENTRY(f1fc4) CASSIE_STEP_ENTRY(f1fd7) CASSIE_STEP_ENTRY(d1fd7) CASSIE_STEP_ENTRY(f1fdf) CASSIE_STEP_ENTRY(d1fdf) CASSIE_STEP_ENTRY(f1fff) CASSIE_STEP_ENTRY(d1fff)
+CASSIE_STEP_ENTRY(f117d7) CASSIE_STEP_ENTRY(d117d7) CASSIE_STEP_ENTRY(f117df) CASSIE_STEP_ENTRY(d117df) CASSIE_STEP_ENTRY(f117ff) CASSIE_STEP_ENTRY(d117ff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -50,6 +51,14 @@ template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_CL) {   // contact lists: the F_CL twins of the F_FR chain twins (a batch with contact lists always has applied rows)
+    if (inst != 1) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_CL; return dbl ? cassie_step_entry_d117ff() : cassie_step_entry_f117ff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_CL; return dbl ? cassie_step_entry_d117df() : cassie_step_entry_f117df(); }
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_CL;
+    return dbl ? cassie_step_entry_d117d7() : cassie_step_entry_f117d7();
+  }
   if (feat & F_TC) {   // per-tick traces: the F_TC twins of the F_XF chain twins, by their rule (a batch with a trace always has applied rows)
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value;
@@ -392,6 +401,10 @@ struct BatchBase {
   virtual bool get_trace(double *out) = 0;
   virtual int trace_ticks() const = 0;
   virtual int trace_width() const = 0;   // T * k, 0 without a trace
+  // contact lists (F_CL instances; an output): on allocates zeroed rows [n][CON_W], off frees them and returns the batch to the instance it ran before;
+  // get copies [n][CON_W]
+  virtual bool enable_contacts(bool on) = 0;
+  virtual bool get_contacts(double *out) = 0;
   // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
   // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
   virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
@@ -475,7 +488,7 @@ template <typename real> struct Batch : BatchBase {
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.cl.geom); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -549,7 +562,8 @@ template <typename real> struct Batch : BatchBase {
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC), (int)cfg[ext].smem));   // and their F_MC twins
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), (int)cfg[ext].smem));   // and their F_CT twins
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), (int)cfg[ext].smem));   // and their F_XF twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_TC), (int)cfg[ext].smem)); }   // and their F_TC twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_TC), (int)cfg[ext].smem));   // and their F_TC twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_CL), (int)cfg[ext].smem)); }   // and their F_CL twins
         if (ext != 1 && step_entry<real>(ext, feat | F_XF))   // the plain F_XF twins (applied forces), where this model runs f04 / f24
           CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF), (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
@@ -1569,7 +1583,7 @@ template <typename real> struct Batch : BatchBase {
   // ---- per-tick trace: the rows are an output, written by step launches only.  The trace instances are the F_TC twins of the chain twins, so a batch
   // with a trace carries applied-force rows (zero when it has none: tc_app) and, through them, model-valued contact, mechanics, actuator and offset rows
   // (xf_ct); they are allocated here, so that a step allocates nothing, and dropped again with the trace unless a verb has written them since
-  bool trace_rows_for_twin() {
+  bool chain_twin_rows() {
     if (!d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }
     if (!A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }
     return true;
@@ -1577,6 +1591,7 @@ template <typename real> struct Batch : BatchBase {
   bool set_trace(const int *source, const int *column, int k, int max_ticks) override {
     const std::string verb = "cassie_batch_set_trace: ";
     if (legacy) { set_err(verb + "the batch belongs to a cassie_sim_t"); return false; }
+    if (k > 0 && A.cl.rows) { set_err(verb + "the batch has contact lists (cassie_batch_enable_contacts); a trace and contact lists do not combine"); return false; }
     if (k < 0 || k > TRACE_MAX) { set_err(verb + "between 0 and " + std::to_string(TRACE_MAX) + " columns"); return false; }
     std::vector<int> codes((size_t)k);
     int need = 0;
@@ -1601,7 +1616,7 @@ template <typename real> struct Batch : BatchBase {
       if (tc_app) { tc_app = false; return enable_applied_forces(false); }
       return true;
     }
-    if (!trace_rows_for_twin()) return false;
+    if (!chain_twin_rows()) return false;
     int *cols = nullptr;
     CUDA_OK(cudaMalloc(&cols, sizeof(int) * k)); CUDA_OK(cudaMemcpy(cols, codes.data(), sizeof(int) * k, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMalloc(&A.trace.rows, sizeof(real) * n * max_ticks * k)); CUDA_OK(cudaMemset(A.trace.rows, 0, sizeof(real) * n * max_ticks * k));
@@ -1614,6 +1629,33 @@ template <typename real> struct Batch : BatchBase {
     return d2h(A.trace.rows, A.trace.T * A.trace.k, A.trace.T * A.trace.k, 0, out);
   }
   int trace_ticks() const override { return tc_ticks; }
+  // ---- contact lists: the rows are an output, written by step and forward launches only.  The contact-list instances are the F_CL twins of the F_FR
+  // chain twins, so the batch carries applied-force and contact rows as with a trace (chain_twin_rows), dropped again with the lists unless a verb has
+  // written them since
+  bool enable_contacts(bool on) override {
+    if (on && A.trace.rows) { set_err("cassie_batch_enable_contacts: the batch has a per-tick trace (cassie_batch_set_trace); a trace and contact lists do not combine"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    if (on && !A.cl.rows) {
+      if (!chain_twin_rows()) return false;
+      int tab[MGT]; for (int k = 0; k < MGT; k++) tab[k] = -1;   // device geom -> model geom
+      for (int g = 0; g < hm.ngeom && g < 256; g++) if (geom_dev[g] >= 0 && geom_dev[g] < MGT) tab[geom_dev[g]] = g;
+      int *geom = nullptr; real *rows = nullptr;
+      CUDA_OK(cudaMalloc(&geom, sizeof tab)); CUDA_OK(cudaMemcpy(geom, tab, sizeof tab, cudaMemcpyHostToDevice));
+      CUDA_OK(cudaMalloc(&rows, sizeof(real) * n * CON_W)); CUDA_OK(cudaMemset(rows, 0, sizeof(real) * n * CON_W));
+      A.cl.rows = rows; A.cl.geom = geom;
+    }
+    if (!on && A.cl.rows) {
+      CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight writes the rows
+      CUDA_OK(cudaFree(A.cl.rows)); CUDA_OK(cudaFree((void *)A.cl.geom)); A.cl = ContactListArgs<real>{};
+      if (tc_app) { tc_app = false; return enable_applied_forces(false); }   // back to the instances that ran before
+    }
+    return true;
+  }
+  bool get_contacts(double *out) override {
+    if (!A.cl.rows) { set_err("cassie_batch_get_contacts: no contact-list rows (cassie_batch_enable_contacts)"); return false; }
+    if (!out) { set_err("cassie_batch_get_contacts: out is required"); return false; }
+    return d2h(A.cl.rows, CON_W, CON_W, 0, out);
+  }
   int trace_width() const override { return A.trace.T * A.trace.k; }
   // ---- the controller-stage state: the delay line, the encoders' filters (views of the cst / dfilt rows; snapshots carry them)
   bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) override {
@@ -1851,7 +1893,7 @@ template <typename real> struct Batch : BatchBase {
   int launch_kind(int mode) {
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
-    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || A.trace.rows || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || A.trace.rows || A.cl.rows || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
     // applied forces: a plain twin where f04 / f24 would run, else the chain twin
     if (A.applied && ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF)) ext = 1;
     return ext;
@@ -1864,7 +1906,7 @@ template <typename real> struct Batch : BatchBase {
     if (mode == 6 && !d_iq) { set_err("the inverse launch needs its rows (cassie_batch_inverse)"); return false; }
     A.nsub = nsub_override;
     const int ext = launch_kind(mode);
-    if (A.trace.rows && !trace_rows_for_twin()) return false;   // only after a verb dropped the rows set_trace allocated
+    if ((A.trace.rows || A.cl.rows) && !chain_twin_rows()) return false;   // only after a verb dropped the rows set_trace / enable_contacts allocated
     if (A.applied && ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }   // the chain twin reads contact rows (the model's values when none were set)
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
@@ -1874,7 +1916,7 @@ template <typename real> struct Batch : BatchBase {
     // mode 6: the caller's qacc reaches the lanes through the warm-start load (mode 6 writes no state back); the forward's stage dump, sensor data and
     // counters go to the launch's scratch rows, for inverse_row; no aux or frame rows
     if (mode == 6) { La.qacc_ws = d_iq; La.dbg = d_idbg; La.cst = d_icst; La.counters = d_icnt; La.aux = nullptr; La.nfr = 0; }
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | ((A.frames || A.acc || mode == 5 || mode == 6) ? F_FR : 0);   // frame, acceleration, dynamics and inverse rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | (A.cl.rows ? F_CL : 0) | ((A.frames || A.acc || A.cl.rows || mode == 5 || mode == 6) ? F_FR : 0);   // frame, acceleration, dynamics and inverse rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -1947,6 +1989,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "applied")) return d_app;
     if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
+    if (!strcmp(f, "contacts")) return A.cl.rows;
 #ifdef CASSIE_STAGE_CLOCKS
     if (!strcmp(f, "stage_clocks")) return A.qM;   // [n][2 NM_MAX] reals, words 0.. the stage clocks of the last step sub-step (step_core.inl STAGE_CLOCK)
 #endif
@@ -1979,6 +2022,9 @@ static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_
 static_assert(CASSIE_INV_WIDTH == INV_W && CASSIE_INV_COLS == IV_COLS && CASSIE_INV_QFRC == IV_QFRC && CASSIE_INV_QFRCC == IV_QFRCC && CASSIE_INV_NEFC == IV_NEFC && CASSIE_INV_NCON == IV_NCON && CASSIE_INV_DROPPED == IV_DROPPED, "inverse row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
 static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
+static_assert(CASSIE_CON_WIDTH == CON_W && CASSIE_CON_MAX == MAXCON && CASSIE_CON_HEAD == CON_HEAD && CASSIE_CON_SLOT == CON_SLOT && CASSIE_CON_GEOM1 == CN_GEOM1 && CASSIE_CON_GEOM2 == CN_GEOM2 &&
+              CASSIE_CON_DIM == CN_DIM && CASSIE_CON_DIST == CN_DIST && CASSIE_CON_POS == CN_POS && CASSIE_CON_FRAME == CN_FRAME && CASSIE_CON_FORCE == CN_FORCE && CASSIE_CON_MU == CN_MU &&
+              CASSIE_CON_EFC == CN_EFC, "contact-list row layout");
 static_assert(CASSIE_TRACE_QPOS == TC_QPOS && CASSIE_TRACE_QVEL == TC_QVEL && CASSIE_TRACE_OBS == TC_OBS && CASSIE_TRACE_AUX == TC_AUX && CASSIE_TRACE_FRAME == TC_FRAME && CASSIE_TRACE_MAX == TRACE_MAX, "trace sources");
 static_assert(CASSIE_FRAME_WIDTH == FRAME_W && CASSIE_FRAME_POS == FR_POS && CASSIE_FRAME_QUAT == FR_QUAT && CASSIE_FRAME_VEL == FR_VEL && CASSIE_FRAME_CFRC == FR_CFRC && CASSIE_FRAME_MAX == FRAME_MAX, "frame row layout");
 struct cassie_batch { BatchBase *impl; std::vector<double> obs, radio; };
@@ -2009,6 +2055,22 @@ struct cassie_state { cassie::Snap *snap = nullptr; double qpos[64], qvel[64], t
 
 static std::mutex g_model_mutex;
 static std::string g_model_path;   // what cassie_mujoco_init cached (the reference caches the parsed model, src/cassiemujoco.c:48-59)
+
+// the name table of an object kind (mj_name2id's type strings), or null with a recorded error: the compiled model keeps the names of bodies (also as
+// "xbody", as MuJoCo does), joints, geoms, sites and cameras; mj_name2id's other kinds have no table here, and an unknown kind is MuJoCo's mjOBJ_UNKNOWN
+static const std::vector<std::string> *name_table(const HostModel &m, const char *type, const char *verb) {
+  const std::string t = type ? type : "";
+  if (t == "body" || t == "xbody") return &m.names_body;
+  if (t == "joint") return &m.names_joint;
+  if (t == "geom") return &m.names_geom;
+  if (t == "site") return &m.names_site;
+  if (t == "camera") return &m.names_camera;
+  static const char *const others[] = {"dof", "light", "mesh", "skin", "hfield", "texture", "material", "pair", "exclude", "equality", "tendon", "actuator",
+                                       "sensor", "numeric", "text", "tuple", "key"};
+  for (const char *o : others) if (t == o) { set_err(std::string(verb) + ": the compiled model keeps no names of kind " + t); return nullptr; }
+  set_err(std::string(verb) + ": unknown object type " + (type ? "\"" + t + "\"" : std::string("(null)")));
+  return nullptr;
+}
 
 extern "C" {
 
@@ -2041,6 +2103,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
   if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "trace")) return b->impl->trace_width();
+  if (!strcmp(field, "contacts")) return CON_W;
   if (!strcmp(field, "inv_qacc")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN; if (!strcmp(field, "inv")) return INV_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
@@ -2502,6 +2565,22 @@ int cassie_batch_enable_applied_forces(cassie_batch_t *b, int on) { return b->im
 int cassie_batch_set_trace(cassie_batch_t *b, const int *source, const int *column, int k, int max_ticks) { return b->impl->set_trace(source, column, k, max_ticks) ? 0 : -1; }
 int cassie_batch_trace_ticks(const cassie_batch_t *b) { return b->impl->trace_ticks(); }
 int cassie_batch_get_trace(cassie_batch_t *b, double *out) { return b->impl->get_trace(out) ? 0 : -1; }
+// contact lists of step and forward launches; see include/cassie_b200.h
+int cassie_batch_enable_contacts(cassie_batch_t *b, int on) { return b->impl->enable_contacts(on != 0) ? 0 : -1; }
+int cassie_batch_get_contacts(cassie_batch_t *b, double *out) { return b->impl->get_contacts(out) ? 0 : -1; }
+// names of the compiled model's objects (mj_name2id / mj_id2name for the kinds it keeps names of); see include/cassie_b200.h
+int cassie_batch_name2id(const cassie_batch_t *b, const char *type, const char *name) {
+  const std::vector<std::string> *t = name_table(b->impl->hm, type, "cassie_batch_name2id");
+  if (!t || !name || !*name) return -1;
+  for (int i = 0; i < (int)t->size(); i++) if ((*t)[i] == name) return i;
+  return -1;
+}
+const char *cassie_batch_id2name(const cassie_batch_t *b, const char *type, int id) {
+  const std::vector<std::string> *t = name_table(b->impl->hm, type, "cassie_batch_id2name");
+  if (!t || id < 0 || id >= (int)t->size() || (*t)[id].empty()) return nullptr;
+  return (*t)[id].c_str();
+}
+int cassie_sim_mj_name2id(cassie_sim_t *c, char *mj_type, char *name) { return cassie_batch_name2id(c->b, mj_type, name); }
 int cassie_batch_get_actuator_state(cassie_batch_t *b, double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) { return b->impl->get_actuator_state(torque_delay, drive_filter, joint_x, joint_y) ? 0 : -1; }
 int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_delay, const int *drive_filter, const double *joint_x, const double *joint_y, const unsigned char *mask) {
   return b->impl->set_actuator_state(torque_delay, drive_filter, joint_x, joint_y, mask) ? 0 : -1; }

@@ -40,6 +40,7 @@ constexpr int F_MC = 256; // per-environment mechanics: link inertia, rotor arma
 constexpr int F_CT = 512; // per-environment contact softness: each contact row mixes solref / solimp from its geoms' CONTACT_W slots (with F_BP | F_AC | F_MC, extended only)
 constexpr int F_XF = 1024; // per-environment applied forces: xfrc_applied / qfrc_applied from an APPLIED_W row (plain F_BOX twins, and extended with F_BP | F_AC | F_MC | F_CT)
 constexpr int F_TC = 2048; // per-tick trace: every tick of a step launch stores the traced columns into a TRACE row slot (the F_XF chain twins' twins only)
+constexpr int F_CL = 4096; // contact lists: the last sub-step of a step / forward launch stores its contacts into a CON_W row (the F_FR chain twins' twins only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -209,6 +210,16 @@ constexpr int AP_XFRC = 0, AP_QFRC = 192;
 constexpr int TC_QPOS = 0, TC_QVEL = 1, TC_OBS = 2, TC_AUX = 3, TC_FRAME = 4, TC_NSRC = 5;
 constexpr int TC_SHIFT = 16, TC_COLMASK = 0xffff;
 constexpr int TRACE_MAX = 64;   // columns
+// contact lists (optional, cassie_batch_enable_contacts; F_CL instances): per environment MuJoCo's d->contact and mj_contactForce of the last sub-step of a
+// step or forward launch (the state that sub-step started from, as the reference's queries read them after mj_step, src/cassiemujoco.c:1586-1606,
+// 1781-1898): a header of CON_HEAD reals -- contacts listed (those that entered the solve, in MuJoCo's order), contacts the collision stage found,
+// contacts dropped at the capacities (found - listed), zeros -- then MAXCON slots of CON_SLOT reals.  Slot: geom1, geom2 in the model's numbering, condim,
+// dist, pos [3], frame [9] (row 0 the normal from geom1 to geom2, rows 1 and 2 the tangents), the contact-frame force [6] (normal, two tangential, three
+// torques that are zero at condim <= 3), the friction the pyramid used, the contact's first constraint row; unused slots are zero with geoms -1.  An
+// output like the aux row: resets, set_state and snapshots leave it alone.  Both widths are multiples of 16 bytes in either precision.
+constexpr int CON_HEAD = 8, CON_SLOT = 24, CON_W = CON_HEAD + MAXCON * CON_SLOT;
+constexpr int CN_GEOM1 = 0, CN_GEOM2 = 1, CN_DIM = 2, CN_DIST = 3, CN_POS = 4, CN_FRAME = 7, CN_FORCE = 16, CN_MU = 22, CN_EFC = 23;
+static_assert(CON_W == 296 && CON_HEAD % 4 == 0 && CON_SLOT % 4 == 0, "contact-list row layout");
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

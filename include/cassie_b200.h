@@ -89,6 +89,7 @@ double *cassie_sim_geom_pos(cassie_sim_t *sim);
 double *cassie_sim_geom_quat(cassie_sim_t *sim);
 double *cassie_sim_geom_size(cassie_sim_t *sim);
 double *cassie_sim_geom_name_pos(cassie_sim_t *sim, const char *name);
+int cassie_sim_mj_name2id(cassie_sim_t *sim, char *mj_type, char *name);   /* cassie_batch_name2id on the sim's batch */
 double *cassie_sim_geom_name_quat(cassie_sim_t *sim, const char *name);
 double *cassie_sim_geom_name_size(cassie_sim_t *sim, const char *name);
 void cassie_sim_set_geom_pos(cassie_sim_t *sim, double *pos);
@@ -751,6 +752,53 @@ int cassie_batch_enable_applied_forces(cassie_batch_t *b, int on);
 int cassie_batch_set_trace(cassie_batch_t *b, const int *source, const int *column, int k, int max_ticks);
 int cassie_batch_trace_ticks(const cassie_batch_t *b);
 int cassie_batch_get_trace(cassie_batch_t *b, double *out);
+/* Contact lists for the batch: every environment's MuJoCo contact list (d->contact) and mj_contactForce, as the reference's users read them through
+ * cassie_sim_mjdata and its own queries are built on them (src/cassiemujoco.c:1586-1606, 1781-1898): which geom a foot touched and where, the normal
+ * on a slope, the penetration depth, the friction the solver used, the contact points and frames a contact-aware controller needs.  With contact rows
+ * enabled, every step launch (cassie_sim_step_pd_batch's chunk launches included) and every forward launch (forward_where too: the selected environments
+ * only) fills one row per environment with the contacts of the launch's last sub-step -- the state that sub-step started from, which is what the
+ * reference's queries read after a step -- that entered the solve, in MuJoCo's order, within the capacities of 12 contacts and 48 constraint rows.
+ * Query, set_const, Jacobian, dynamics and inverse launches, resets, set_state, reset_where and snapshots leave the rows alone (they are an output;
+ * a restore followed by forward_where refreshes them).  Row [CASSIE_CON_WIDTH] in the batch precision: CASSIE_CON_HEAD header reals -- [0] contacts
+ * listed, [1] contacts the collision stage found, [2] contacts dropped at the capacities (found - listed; the increment of counters[4]), the rest zero --
+ * then CASSIE_CON_MAX slots of CASSIE_CON_SLOT reals, slot k at CASSIE_CON_HEAD + CASSIE_CON_SLOT * k:
+ *   CASSIE_CON_GEOM1, GEOM2  geom ids in the model's numbering (cassie_batch_id2name(b, "geom", id)); -1 in unused slots
+ *   CASSIE_CON_DIM           condim
+ *   CASSIE_CON_DIST          contact.dist (negative: penetration)
+ *   CASSIE_CON_POS   [3]     contact.pos, world frame
+ *   CASSIE_CON_FRAME [9]     contact.frame, row-major: row 0 the normal, from geom1 to geom2; rows 1 and 2 the tangents
+ *   CASSIE_CON_FORCE [6]     mj_contactForce in the contact frame: normal, two tangential, three torques (zero at condim <= 3).  The force geom2 feels
+ *                            in the world frame is frame' force[0..2]; geom1 feels its negative
+ *   CASSIE_CON_MU            the friction the pyramid used: the pair's mixed friction, from the per-environment friction rows where the batch has them
+ *   CASSIE_CON_EFC           contact.efc_address: the contact's first constraint row (the equality and limit rows come first)
+ * Unused slots are zero apart from the geom ids.  enable_contacts(b, 1) allocates zeroed rows, so that a launch allocates and synchronises nothing;
+ * enable_contacts(b, 0) frees them.  A batch with contact rows runs the F_CL twins of the extended applied-force instances: it carries applied-force
+ * and contact rows (model-valued ones when it has none, dropped again by enable_contacts(b, 0) unless a verb has written them since), and its physics
+ * is bitwise that of the same batch without contact rows.  A batch with a per-tick trace refuses contact rows and a batch with contact rows refuses a
+ * trace.  get_contacts: synchronous host copy [n][CASSIE_CON_WIDTH] doubles.  Device rows: cassie_batch_device_ptr(b, "contacts"),
+ * cassie_batch_row_width(b, "contacts") = CASSIE_CON_WIDTH.  0, or -1 (cassie_b200_last_error says why). */
+#define CASSIE_CON_HEAD 8
+#define CASSIE_CON_SLOT 24
+#define CASSIE_CON_MAX 12
+#define CASSIE_CON_WIDTH 296
+#define CASSIE_CON_GEOM1 0
+#define CASSIE_CON_GEOM2 1
+#define CASSIE_CON_DIM 2
+#define CASSIE_CON_DIST 3
+#define CASSIE_CON_POS 4
+#define CASSIE_CON_FRAME 7
+#define CASSIE_CON_FORCE 16
+#define CASSIE_CON_MU 22
+#define CASSIE_CON_EFC 23
+int cassie_batch_enable_contacts(cassie_batch_t *b, int on);
+int cassie_batch_get_contacts(cassie_batch_t *b, double *out);
+/* Names of the compiled model's objects, as mj_name2id / mj_id2name give them (the reference's cassie_sim_mj_name2id, src/cassiemujoco.c:2194-2246):
+ * type "body" (or "xbody"), "joint", "geom", "site" or "camera".  name2id: the id, or -1 for an unknown or empty name; id2name: the name, or NULL for
+ * an id out of range or an unnamed object (the string lives as long as the batch).  Both return -1 / NULL with a recorded error for mj_name2id's other
+ * kinds (actuators, equalities, meshes, ...: the compiled model keeps no names of them) and for an unknown type.  cassie_sim_mj_name2id is the same
+ * lookup on a cassie_sim_t. */
+int cassie_batch_name2id(const cassie_batch_t *b, const char *type, const char *name);
+const char *cassie_batch_id2name(const cassie_batch_t *b, const char *type, int id);
 /* The controller-stage state of every environment, as the reference's cassie_sim_t holds it: the torque delay line torque_delay [n][10][6] (slot 0
  * newest), the drive encoders' integer FIR taps drive_filter [n][10][9], the joint encoders' IIR filters joint_x [n][6][4] and joint_y [n][6][3].
  * NULL parts are skipped; set changes masked environments only (mask NULL: all).  They are state: reset, snapshots and cassie_sim_copy carry them. */
@@ -759,7 +807,7 @@ int cassie_batch_set_actuator_state(cassie_batch_t *b, const double *torque_dela
                                     const unsigned char *mask);
 
 /* zero-copy access for a PyTorch / DLPack caller: device pointer of a state array ("qpos" [n][36], "qvel" [n][32],
- * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232], "trace" [n][T * k], "inv_qacc" [n][32] ([n][40]), "inv" [n][96]; the inverse rows are allocated by the request) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
+ * "pd" [n][52], "obs" [n][112], "xfrc" [n][8], "aux" [n][64], "frames" [n][count * 20], "acc" [n][40 + 8 count], "actuators" [n][40], "mechanics" [n][192], "contact" [n][256], "applied" [n][232], "trace" [n][T * k], "contacts" [n][296], "inv_qacc" [n][32] ([n][40]), "inv" [n][96]; the inverse rows are allocated by the request) in the batch precision, "terrain" [n] int32; the stream all work is enqueued on
  * (cudaStream_t). */
 void *cassie_batch_device_ptr(cassie_batch_t *b, const char *field);
 void cassie_batch_set_stream(cassie_batch_t *b, void *cuda_stream);
