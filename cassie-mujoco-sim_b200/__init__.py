@@ -26,8 +26,11 @@ DYN_WIDTH, DYN_COLS = 2144, 40
 # the ray's end point when none), static geom slot (-1: none), pad
 RAY_HEADING, RAY_ROOT, RAY_WORLD, RAY_MAX, RAY_SLOT = 0, 1, 2, 1024, 4
 RAY_FRAMES = dict(heading=RAY_HEADING, root=RAY_ROOT, world=RAY_WORLD)
-# depth camera (include/cassie_b200.h CASSIE_CAM_*): largest image side
+# depth cameras (include/cassie_b200.h CASSIE_CAM_*): largest image side, cameras per set, reals per per-environment mount slot (pos[3], quat[4],
+# fovy in degrees)
 CAM_MAXDIM = 256
+CAM_MAX = 4
+CAMENV_SLOT = 8
 DYN = dict(M=slice(0, 1600), bias=slice(1600, 1640), J_eq=slice(1640, 2120), eq_err=slice(2120, 2132), rcm=slice(2132, 2135))
 # inverse row (include/cassie_b200.h CASSIE_INV_*): qfrc_inverse [40], qfrc_constraint [40] (column = dof as in DYN), then the row count, the contacts with
 # rows and the contacts dropped at the capacities, as reals; padded to 96.  The input rows ('inv_qacc') are qvel-wide, column = dof
@@ -1023,7 +1026,93 @@ class CassieBatch:
             rc = self.L.cassie_batch_set_camera_mount(self.h, body.encode(), self._dp(p), self._dp(q), float(fovy), int(width), int(height), float(zfar))
         if rc != 0:
             raise RuntimeError(_last_error())
-        self._cam_hw = (int(height), int(width)) if width else None
+        self._cam_shape = (int(height), int(width)) if width else None
+
+    def _cam_lib(self):
+        L = self.L
+        if not getattr(L, '_cam_bound', False):
+            vp, dp, ip = C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int)
+            L.cassie_batch_set_cameras.argtypes = [vp, C.c_int, ip, dp, dp, dp, C.c_int, C.c_int, C.c_double]
+            L.cassie_batch_model_camera.argtypes = [vp, C.c_char_p, ip, dp, dp, dp]
+            L.cassie_batch_ncameras.argtypes = [vp]
+            L.cassie_batch_set_env_cameras.argtypes = [vp, dp, dp, dp, vp]
+            L.cassie_batch_get_env_cameras.argtypes = [vp, dp, dp, dp]
+            L.cassie_batch_clear_env_cameras.argtypes = [vp]
+            L.cassie_batch_enable_camera_geoms.argtypes = [vp, C.c_int]
+            L.cassie_batch_get_camera_geoms.argtypes = [vp, ip]
+            L._cam_bound = True
+        return L
+
+    def model_camera(self, name):
+        """(body id, pos [3], quat [4], fovy) of a fixed <camera> of the model, e.g. 'egocentric' of cassie_depth.xml"""
+        body, pos, quat, fovy = C.c_int(), np.zeros(3), np.zeros(4), C.c_double()
+        if self._cam_lib().cassie_batch_model_camera(self.h, name.encode(), C.byref(body), self._dp(pos), self._dp(quat), C.byref(fovy)) != 0:
+            raise RuntimeError(_last_error())
+        return body.value, pos, quat, fovy.value
+
+    def set_cameras(self, cams, width=64, height=64, zfar=5.0):
+        """a set of up to CAM_MAX cameras rendered in one launch, sharing one image size and zfar.  Each entry of cams is a model camera name or
+        (body, pos, quat, fovy): body a name or an id, pos / quat in the body frame, fovy the full vertical angle in degrees.  An empty list drops the
+        set.  depth() and torch_view('depth') are then [n, k, height, width].  Drops the depth, geom-id and per-environment mount rows: views taken
+        before it must not be used after it."""
+        L = self._cam_lib()
+        k = len(cams)
+        body, pos, quat, fovy = np.zeros(k, dtype=np.int32), np.zeros((k, 3)), np.zeros((k, 4)), np.zeros(k)
+        for i, c in enumerate(cams):
+            if isinstance(c, str):
+                body[i], pos[i], quat[i], fovy[i] = self.model_camera(c)
+                continue
+            b, p, q, f = c
+            body[i] = self.name2id('body', b) if isinstance(b, str) else int(b)
+            pos[i], quat[i], fovy[i] = p, q, f
+        if L.cassie_batch_set_cameras(self.h, k, body.ctypes.data_as(C.POINTER(C.c_int)), self._dp(pos), self._dp(quat), self._dp(fovy),
+                                      int(width), int(height), float(zfar)) != 0:
+            raise RuntimeError(_last_error())
+        self._cam_shape = (k, int(height), int(width)) if k else None
+
+    def ncameras(self):
+        return int(self._cam_lib().cassie_batch_ncameras(self.h))
+
+    def set_env_cameras(self, pos=None, quat=None, fovy=None, mask=None):
+        """each environment's camera mounts: pos [k, 3] or [n, k, 3] and quat [k, 4] or [n, k, 4] in each camera's body frame, fovy [k] or [n, k] in
+        degrees; the body stays the set's.  A part left None is kept; mask [n]: only the selected environments change.  The first call starts every
+        environment from the set's mounts.  A non-finite value, a zero quaternion or a fovy outside (0, 180) raises, and nothing changes.  Resets
+        and snapshot restores leave the rows alone; a new set drops them.  torch_view('camera_env') [n, k, 8] is the device copy, read at the next
+        render."""
+        L, k = self._cam_lib(), self.ncameras()
+        p = self._arr(pos, np.float64, (self.n, k, 3))
+        q = self._arr(quat, np.float64, (self.n, k, 4))
+        f = self._arr(fovy, np.float64, (self.n, k))
+        m = self._arr(mask, np.uint8, (self.n,))
+        ptr = lambda a: None if a is None else self._dp(a)
+        if L.cassie_batch_set_env_cameras(self.h, ptr(p), ptr(q), ptr(f), None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_cameras(self):
+        """(pos [n, k, 3], quat [n, k, 4], fovy [n, k]): the mount every environment's cameras see (the set's without rows)"""
+        L, k = self._cam_lib(), self.ncameras()
+        p, q, f = np.zeros((self.n, k, 3)), np.zeros((self.n, k, 4)), np.zeros((self.n, k))
+        if L.cassie_batch_get_env_cameras(self.h, self._dp(p), self._dp(q), self._dp(f)) != 0:
+            raise RuntimeError(_last_error())
+        return p, q, f
+
+    def clear_env_cameras(self):
+        """back to the set's mounts in every environment"""
+        if self._cam_lib().cassie_batch_clear_env_cameras(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def enable_camera_geoms(self, on=True):
+        """every render also writes the model geom id of each pixel's surface (-1: nothing within zfar); False frees the rows"""
+        if self._cam_lib().cassie_batch_enable_camera_geoms(self.h, 1 if on else 0) != 0:
+            raise RuntimeError(_last_error())
+
+    def camera_geoms(self):
+        """geom ids of the last render, shaped as depth(): [n, k, height, width] (set_cameras) or [n, height, width] (set_camera)"""
+        shape = getattr(self, '_cam_shape', None)
+        out = np.zeros((self.n,) + (shape or (0,)), dtype=np.int32)
+        if shape is None or self._cam_lib().cassie_batch_get_camera_geoms(self.h, out.ctypes.data_as(C.POINTER(C.c_int))) != 0:
+            raise RuntimeError(_last_error() if shape else 'no camera is set (set_camera / set_cameras)')
+        return out
 
     def render_depth(self):
         """enqueue one depth render of every environment on the batch's stream (asynchronous), at the CURRENT state; nothing else is written"""
@@ -1032,8 +1121,9 @@ class CassieBatch:
             raise RuntimeError(_last_error())
 
     def depth(self):
-        """[n, height, width] z-depths (metres, row 0 at the top; zfar where nothing is hit) of the last render_depth()"""
-        hw = getattr(self, '_cam_hw', None)
+        """[n, height, width] (set_camera) or [n, k, height, width] (set_cameras) z-depths (metres, row 0 at the top; zfar where nothing is hit) of
+        the last render_depth()"""
+        hw = getattr(self, '_cam_shape', None)
         out = np.zeros((self.n,) + (hw or (0, 0)))
         self.L.cassie_batch_get_depth.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         if hw is None or self.L.cassie_batch_get_depth(self.h, self._dp(out)) != 0:
@@ -1199,7 +1289,7 @@ class CassieBatch:
 
     def torch_view(self, field):
         """zero-copy torch tensor over a device state array (qpos [n,36], qvel [n,32], pd [n,52], obs [n,112], aux [n,64], frames [n, nframes * 20],
-        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width],
+        frame_jac [n, 240], dyn [n, DYN_WIDTH] laid out as DYN, rays [n, k * RAY_SLOT], acc [n, acc_width(nframes)] laid out as ACC, depth [n, height, width] (set_camera) or [n, k, height, width] (set_cameras),
         terrain [n] int32: each environment's bank entry, read mod K at the next launch; set_env_hfield first; actuators [n, 40]: lo[10], hi[10], wmax[10]
         in rad/s, delay[10], read at the next launch; set_env_actuators first; mechanics [n, 192]: body_inertia[32][3], armature[32], stiffness[32],
         qpos_spring[32] per main-tree dof (the springs of hinge dofs only are read), read at the next launch; set_env_mechanics first; contact [n, 256]:
@@ -1208,7 +1298,9 @@ class CassieBatch:
         the extra free body 32..37), read at the next launch; set_applied_forces or enable_applied_forces first; trace [n, T, k]: the per-tick trace of
         the last step launch, slot s of every environment, written by step launches only; set_trace first; inv_qacc [n, qvel width]: the qacc of
         compute_inverse(None), column = dof; inv [n, INV_WIDTH] laid out as INV; both allocated by the first request; contacts [n, CON_WIDTH]: the contact
-        lists of the last step / forward launch, a header and CON_MAX slots laid out as CON; enable_contacts first).  set_frames /
+        lists of the last step / forward launch, a header and CON_MAX slots laid out as CON; enable_contacts first; camera_env [n, k, CAMENV_SLOT]: the
+        per-environment camera mounts pos[3], quat[4], fovy in degrees, read at the next render; set_env_cameras first; camera_geom [n, k, height, width]
+        int32 (shaped as depth for set_camera): the geom ids of the last render; enable_camera_geoms and render_depth first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -1218,9 +1310,9 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
-        if field == 'terrain':
+        if field in ('terrain', 'camera_geom'):
             ts = '<i4'
 
         class _Arr:
@@ -1232,7 +1324,9 @@ class CassieBatch:
             return t.view(self.n)
         if field == 'trace':
             return t.view(self.n, *self._trace_shape)
-        return t.view(self.n, *self._cam_hw) if field == 'depth' else t
+        if field == 'camera_env':
+            return t.view(self.n, -1, CAMENV_SLOT)
+        return t.view(self.n, *self._cam_shape) if field in ('depth', 'camera_geom') else t
 
 
 class joint_filter_t(C.Structure):

@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, '_obj')
 LIB = os.path.join(HERE, 'libcassie_b200.so')
 DEPS = [os.path.join(CSRC, f) for f in ('cassie_b200.cu', 'mjcf.cpp', 'step_inst.cu', 'step_kernel.cuh', 'step_core.inl', 'cassie_tree_gen.inc', 'devmodel.h', 'devbuild.h', 'model.h',
-                                        'estimator_host.h', 'legacy_stubs.inc', 'raycast.cu', 'raycast.inl', 'camera.cu', 'camera.inl', 'reset.cu', 'reset.inl')] + [
+                                        'estimator_host.h', 'legacy_stubs.inc', 'raycast.cu', 'raycast.inl', 'camera.cu', 'camera.inl', 'camera_set.cu', 'camera_set.inl', 'reset.cu', 'reset.inl')] + [
     os.path.join(HERE, '..', 'include', 'cassie_b200.h'), os.path.join(HERE, '..', 'include', 'cassie_bus.h')]
 # (tag, real, instance: 0 plain / 1 extended / 2 plain + estimator, feature set): features 1 = extra free body, 2 = height field, 4 = box geoms (csrc/devmodel.h F_*)
 INSTANCES = [('f00', 'float', 0, 0), ('f10', 'float', 1, 0), ('f02', 'float', 0, 2), ('f12', 'float', 1, 2), ('f04', 'float', 0, 4), ('f14', 'float', 1, 4), ('f05', 'float', 0, 5), ('f15', 'float', 1, 5),
@@ -90,9 +90,9 @@ def _run(cmd, verbose, res=None):
 
 
 def res_path(obj):
-    """the resource report written beside a step instance's, the ray kernel's, the camera kernel's or the restore kernel's object file, or None for the other objects."""
+    """the resource report written beside a step instance's, the ray kernel's, a camera kernel's or the restore kernel's object file, or None for the other objects."""
     name = os.path.basename(obj)
-    return obj[:-2] + '.res' if name.startswith(('step_', 'ray_', 'cam_', 'reset_')) and name.endswith('.o') else None
+    return obj[:-2] + '.res' if name.startswith(('step_', 'ray_', 'cam_', 'camset_', 'reset_')) and name.endswith('.o') else None
 
 
 def build(force=False, verbose=False, out=None):
@@ -109,8 +109,9 @@ def build(force=False, verbose=False, out=None):
     jobs.append([nvcc()] + ARCH + ['-c', os.path.join(CSRC, 'mjcf.cpp'), '-o', os.path.join(OBJ, 'mjcf.o')])
     for real in ('float', 'double'):   # the ray kernel, one object per precision; its report is kept as ray_<real>.res (tests/test_raycast_resources.py)
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DRAY_REAL=' + real, '-c', os.path.join(CSRC, 'raycast.cu'), '-o', os.path.join(OBJ, 'ray_%s.o' % real)])
-    for real in ('float', 'double'):   # the camera kernel, likewise; its report is kept as cam_<real>.res (tests/test_camera_resources.py)
+    for real in ('float', 'double'):   # the camera kernels, likewise; their reports are kept as cam_<real>.res and camset_<real>.res (tests/test_camera_resources.py, test_camera_set_resources.py)
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DCAM_REAL=' + real, '-c', os.path.join(CSRC, 'camera.cu'), '-o', os.path.join(OBJ, 'cam_%s.o' % real)])
+        jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DCAMSET_REAL=' + real, '-c', os.path.join(CSRC, 'camera_set.cu'), '-o', os.path.join(OBJ, 'camset_%s.o' % real)])
     for real in ('float', 'double'):   # the restore kernel, likewise; its report is kept as reset_<real>.res (tests/test_reset_resources.py)
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DRESET_REAL=' + real, '-c', os.path.join(CSRC, 'reset.cu'), '-o', os.path.join(OBJ, 'reset_%s.o' % real)])
     with ThreadPoolExecutor(max_workers=max(2, min(len(jobs), (os.cpu_count() or 4)))) as ex:

@@ -21,7 +21,7 @@
 #include "estimator_host.h"
 #include "step_kernel.cuh"
 #include "raycast.inl"
-#include "camera.inl"
+#include "camera_set.inl"
 #include "reset.inl"
 
 // the step-kernel instances live in their own translation units (step_inst.cu, one compilation per instance)
@@ -47,6 +47,7 @@ namespace cassie {
 
 template <typename real> cudaError_t launch_raycast(const RayArgs<real> &A, int device, cudaStream_t stream);   // raycast.cu
 template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int device, cudaStream_t stream);   // camera.cu
+template <typename real> cudaError_t launch_camera_set(const CamSetArgs<real> &A, int device, cudaStream_t stream);   // camera_set.cu
 template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device, cudaStream_t stream);       // reset.cu
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
@@ -428,13 +429,25 @@ struct BatchBase {
   virtual bool raycast() = 0;                           // one launch (asynchronous) at the current qpos
   virtual bool get_rays(double *out) = 0;               // [n][k][RAY_SLOT] of the last cast
   int nray = 0; bool rays_done = false;                 // rays in the table; a cast was enqueued since the table was set
-  // the depth camera (camera.inl): one per batch, mounted on a body; a set is checked before anything changes, width 0 drops it.  The rows
-  // [n][height][width] are allocated by the first render after a set and are a query result, not state
-  struct Camera { int body = -1, width = 0, height = 0; double pos[3] = {0, 0, 0}, quat[4] = {1, 0, 0, 0}, fovy = 45, zfar = 1; } cam;
-  bool depth_done = false;                              // a render was enqueued since the camera was set
-  virtual bool set_camera(int body, const double *pos, const double *quat, double fovy, int width, int height, double zfar, const char *verb) = 0;
+  // the depth cameras (camera.inl, camera_set.inl): a set of k <= CAM_MAX cameras with one image size and zfar, each mounted on a body; a set is checked as a whole
+  // before anything changes, k = 0 drops it, and every set drops the depth, geom-id and per-environment mount rows.  The depth and geom-id rows
+  // [n][k][height][width] are allocated by the first render after a set and are a query result, not state.  The mount rows [n][k][CAMENV_SLOT] are a
+  // model input: allocated by set_env_cameras (holding the set's mounts), left alone by resets and snapshots
+  struct Cameras { int k = 0, width = 0, height = 0, body[CAM_MAX] = {}; double pos[CAM_MAX][3] = {}, quat[CAM_MAX][4] = {}, fovy[CAM_MAX] = {}, zfar = 1; } cam;
+  bool depth_done = false, geoms_done = false;          // a render was enqueued since the set (since the geom-id rows were enabled)
+  bool cam_geoms = false;                               // renders write geom-id rows (cassie_batch_enable_camera_geoms)
+  // k cameras: body [k], pos [k][3], quat [k][4] (normalised here), fovy [k]; indexed: refusals name the camera ("camera i: ...")
+  virtual bool set_cameras(int k, const int *body, const double *pos, const double *quat, const double *fovy, int width, int height, double zfar,
+                           const char *verb, bool indexed) = 0;
   virtual bool render_depth() = 0;                      // one launch (asynchronous) at the current qpos
-  virtual bool get_depth(double *out) = 0;              // [n][height][width] of the last render
+  virtual bool get_depth(double *out) = 0;              // [n][k][height][width] of the last render
+  // per-environment mounts: pos [n][k][3], quat [n][k][4], fovy [n][k], each may be null (kept); only masked environments change; checked as a whole
+  // before anything changes
+  virtual bool set_env_cameras(const double *pos, const double *quat, const double *fovy, const unsigned char *mask) = 0;
+  virtual bool get_env_cameras(double *pos, double *quat, double *fovy) = 0;
+  virtual bool clear_env_cameras() = 0;
+  virtual bool enable_camera_geoms(bool on) = 0;
+  virtual bool get_camera_geoms(int *out) = 0;          // [n][k][height][width] model geom ids of the last render, -1 where nothing is hit
   std::vector<int> frame_list;                          // (kind, id) per frame of the current frame table
   int nsub_override = 0;                                // > 0: physics sub-steps per control tick of the next launches (cassie_sim_step_pd_no2khz)
   bool sync() { CUDA_OK(cudaStreamSynchronize(stream)); return true; }
@@ -464,6 +477,10 @@ template <typename real> struct Batch : BatchBase {
   float *d_hfield = nullptr; unsigned char *d_mask = nullptr; DevModel<real> h_model_copy{}; int geom_dev[256]; void *d_row = nullptr;
   real *d_rtab = nullptr, *d_rays = nullptr;   // ray table (RT_HDR + nray RT_W) and the rows of the last cast
   real *d_depth = nullptr;                     // depth rows of the last render
+  int *d_camgeom = nullptr;                    // geom-id rows of the last render (with cam_geoms)
+  real *d_camenv = nullptr;                    // per-environment camera mounts [n][k][CAMENV_SLOT], allocated by the first cassie_batch_set_env_cameras
+  std::vector<double> ce_host;                 // [n][k][CAMENV_SLOT] the mounts every environment sees while d_camenv exists (in double: what get returns)
+  int *d_gtab = nullptr;                       // [MGT] the model geom of each device geom (-1: none): contact lists and camera geom ids, built on first use
   real *d_genv = nullptr;                  // A.genv: [n][GEOM_ENV_W] per-environment static-geom placement, allocated by the first per-environment placement
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   int *d_terrain = nullptr;                // A.terrain: [n] per-environment bank entries, allocated by the first per-environment terrain (F_TR instances)
@@ -488,7 +505,7 @@ template <typename real> struct Batch : BatchBase {
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.cl.geom); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -1009,6 +1026,13 @@ template <typename real> struct Batch : BatchBase {
       CUDA_OK(cudaMemcpy(d_mech, src->d_mech, sizeof(real) * n * MECH_W, cudaMemcpyDeviceToDevice));
       A.mech = d_mech;
     }
+    if (src->d_camenv && src->cam.k == cam.k) {   // the per-environment camera mounts, when the two batches hold as many cameras
+      ce_host = src->ce_host;
+      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
+      const size_t w = (size_t)n * cam.k * CAMENV_SLOT;
+      if (!d_camenv) CUDA_OK(cudaMalloc(&d_camenv, sizeof(real) * w));
+      CUDA_OK(cudaMemcpy(d_camenv, src->d_camenv, sizeof(real) * w, cudaMemcpyDeviceToDevice));
+    } else if (!clear_env_cameras()) return false;
     if (src->d_ct) {   // likewise the contact rows (the mechanics rows came just now)
       ct_host = src->ct_host; ct_mech = src->ct_mech; xf_ct = src->xf_ct;
       CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
@@ -1636,19 +1660,24 @@ template <typename real> struct Batch : BatchBase {
     if (on && A.trace.rows) { set_err("cassie_batch_enable_contacts: the batch has a per-tick trace (cassie_batch_set_trace); a trace and contact lists do not combine"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (on && !A.cl.rows) {
-      if (!chain_twin_rows()) return false;
-      int tab[MGT]; for (int k = 0; k < MGT; k++) tab[k] = -1;   // device geom -> model geom
-      for (int g = 0; g < hm.ngeom && g < 256; g++) if (geom_dev[g] >= 0 && geom_dev[g] < MGT) tab[geom_dev[g]] = g;
-      int *geom = nullptr; real *rows = nullptr;
-      CUDA_OK(cudaMalloc(&geom, sizeof tab)); CUDA_OK(cudaMemcpy(geom, tab, sizeof tab, cudaMemcpyHostToDevice));
+      if (!chain_twin_rows() || !geom_table()) return false;
+      real *rows = nullptr;
       CUDA_OK(cudaMalloc(&rows, sizeof(real) * n * CON_W)); CUDA_OK(cudaMemset(rows, 0, sizeof(real) * n * CON_W));
-      A.cl.rows = rows; A.cl.geom = geom;
+      A.cl.rows = rows; A.cl.geom = d_gtab;
     }
     if (!on && A.cl.rows) {
       CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight writes the rows
-      CUDA_OK(cudaFree(A.cl.rows)); CUDA_OK(cudaFree((void *)A.cl.geom)); A.cl = ContactListArgs<real>{};
+      CUDA_OK(cudaFree(A.cl.rows)); A.cl = ContactListArgs<real>{};   // (the geom table stays with the batch)
       if (tc_app) { tc_app = false; return enable_applied_forces(false); }   // back to the instances that ran before
     }
+    return true;
+  }
+  bool geom_table() {   // d_gtab: device geom -> model geom, for the contact lists and the camera geom ids
+    if (d_gtab) return true;
+    int tab[MGT]; for (int k = 0; k < MGT; k++) tab[k] = -1;
+    for (int g = 0; g < hm.ngeom && g < 256; g++) if (geom_dev[g] >= 0 && geom_dev[g] < MGT) tab[geom_dev[g]] = g;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMalloc(&d_gtab, sizeof tab)); CUDA_OK(cudaMemcpy(d_gtab, tab, sizeof tab, cudaMemcpyHostToDevice));
     return true;
   }
   bool get_contacts(double *out) override {
@@ -1844,37 +1873,146 @@ template <typename real> struct Batch : BatchBase {
     if (!out) { set_err("cassie_batch_get_rays: out is required"); return false; }
     return d2h(d_rays, nray * RAY_SLOT, nray * RAY_SLOT, 0, out);
   }
-  bool set_camera(int body, const double *pos, const double *quat, double fovy, int width, int height, double zfar, const char *verb) override {
-    Camera c; std::string err;
-    if (width != 0) {
-      if (body < 0 || body >= hm.nbody) { set_err(std::string(verb) + ": unknown body"); return false; }
-      if (!camera_check(pos, quat, fovy, width, height, zfar, c.quat, err)) { set_err(std::string(verb) + ": " + err); return false; }
-      c.body = body; c.width = width; c.height = height; c.fovy = fovy; c.zfar = zfar;
-      for (int i = 0; i < 3; i++) c.pos[i] = pos[i];
+  bool set_cameras(int k, const int *body, const double *pos, const double *quat, const double *fovy, int width, int height, double zfar, const char *verb,
+                   bool indexed) override {
+    Cameras c; std::string err;
+    if (k < 0 || k > CAM_MAX) { set_err(std::string(verb) + ": between 0 and " + std::to_string(CAM_MAX) + " cameras"); return false; }
+    if (k > 0 && (!body || !pos || !quat || !fovy)) { set_err(std::string(verb) + ": body, pos, quat and fovy are required"); return false; }
+    for (int i = 0; i < k; i++) {
+      const std::string at = std::string(verb) + (indexed ? ": camera " + std::to_string(i) : "");
+      if (body[i] < 0 || body[i] >= hm.nbody) { set_err(at + ": unknown body"); return false; }
+      if (!camera_check(pos + 3 * i, quat + 4 * i, fovy[i], width, height, zfar, c.quat[i], err)) { set_err(at + ": " + err); return false; }
+      c.body[i] = body[i]; c.fovy[i] = fovy[i];
+      for (int j = 0; j < 3; j++) c.pos[i][j] = pos[3 * i + j];
     }
+    if (k > 0) { c.k = k; c.width = width; c.height = height; c.zfar = zfar; }
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
-    CUDA_OK(cudaFree(d_depth)); d_depth = nullptr; depth_done = false;
+    CUDA_OK(cudaFree(d_depth)); CUDA_OK(cudaFree(d_camgeom)); CUDA_OK(cudaFree(d_camenv)); d_depth = nullptr; d_camgeom = nullptr; d_camenv = nullptr;
+    ce_host.clear(); depth_done = geoms_done = false;
     cam = c;
     return true;
   }
   bool render_depth() override {
-    if (!cam.width) { set_err("cassie_batch_render_depth: no camera is set (cassie_batch_set_camera)"); return false; }
+    if (!cam.k) { set_err("cassie_batch_render_depth: no camera is set (cassie_batch_set_camera)"); return false; }
     CUDA_OK(cudaSetDevice(device));
-    if (!d_depth) CUDA_OK(cudaMalloc(&d_depth, sizeof(real) * n * cam.width * cam.height));
-    CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = d_bpos;
-    C.body = cam.body; C.width = cam.width; C.height = cam.height; C.tan_half = (real)std::tan(cam.fovy * M_PI / 360); C.zfar = (real)cam.zfar;
-    for (int i = 0; i < 3; i++) C.pos[i] = (real)cam.pos[i];
-    for (int i = 0; i < 4; i++) C.quat[i] = (real)cam.quat[i];
-    C.out = d_depth; C.n = n;
-    CUDA_OK(launch_camera<real>(C, device, stream));
-    launches++; depth_done = true;
+    const size_t px = (size_t)n * cam.k * cam.width * cam.height;
+    if (!d_depth) CUDA_OK(cudaMalloc(&d_depth, sizeof(real) * px));
+    if (cam_geoms && !d_camgeom) { if (!geom_table()) return false; CUDA_OK(cudaMalloc(&d_camgeom, sizeof(int) * px)); }
+    CamMount<real> mt[CAM_MAX];
+    for (int c = 0; c < cam.k; c++) {
+      mt[c].body = cam.body[c]; mt[c].tan_half = (real)std::tan(cam.fovy[c] * M_PI / 360);
+      for (int i = 0; i < 3; i++) mt[c].pos[i] = (real)cam.pos[c][i];
+      for (int i = 0; i < 4; i++) mt[c].quat[i] = (real)cam.quat[c][i];
+    }
+    if (cam.k == 1 && !d_camenv && !cam_geoms) {   // one camera, nothing per environment: the one-camera kernel (DESIGN.md section 5)
+      CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = d_bpos;
+      C.body = mt[0].body; C.width = cam.width; C.height = cam.height; C.tan_half = mt[0].tan_half; C.zfar = (real)cam.zfar;
+      for (int i = 0; i < 3; i++) C.pos[i] = mt[0].pos[i];
+      for (int i = 0; i < 4; i++) C.quat[i] = mt[0].quat[i];
+      C.out = d_depth; C.n = n;
+      CUDA_OK(launch_camera<real>(C, device, stream));
+    } else {
+      CamSetArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = d_bpos;
+      C.k = cam.k; C.width = cam.width; C.height = cam.height; C.zfar = (real)cam.zfar;
+      for (int c = 0; c < CAM_MAX; c++) C.cam[c] = mt[c < cam.k ? c : 0];
+      C.out = d_depth; C.n = n; C.cenv = d_camenv; C.geom = cam_geoms ? d_camgeom : nullptr; C.gtab = d_gtab;
+      CUDA_OK(launch_camera_set<real>(C, device, stream));
+    }
+    launches++; depth_done = true; geoms_done = cam_geoms;
     return true;
   }
   bool get_depth(double *out) override {
     if (!depth_done) { set_err("cassie_batch_get_depth: no render since the camera was set (cassie_batch_render_depth)"); return false; }
     if (!out) { set_err("cassie_batch_get_depth: out is required"); return false; }
-    const int w = cam.width * cam.height;
+    const int w = cam.k * cam.width * cam.height;
     return d2h(d_depth, w, w, 0, out);
+  }
+  bool enable_camera_geoms(bool on) override {
+    if (on == cam_geoms) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a render in flight writes the rows
+    CUDA_OK(cudaFree(d_camgeom)); d_camgeom = nullptr;
+    cam_geoms = on; geoms_done = false;
+    return true;
+  }
+  bool get_camera_geoms(int *out) override {
+    if (!geoms_done) { set_err("cassie_batch_get_camera_geoms: no render with geom ids since the cameras were set or geom ids enabled (cassie_batch_enable_camera_geoms, cassie_batch_render_depth)"); return false; }
+    if (!out) { set_err("cassie_batch_get_camera_geoms: out is required"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemcpyAsync(out, d_camgeom, sizeof(int) * n * cam.k * cam.width * cam.height, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  // ---- per-environment camera mounts (extrinsics and field-of-view randomisation): the pose in each camera's body frame and its fovy, per
+  // environment; the body stays the set's.  As with the actuator rows, the device rows are what the kernel reads, the mirror keeps the doubles the verb
+  // was last given, and get reports a value the row still holds as the verb stored it as the verb was given it
+  void model_camenv(int c, double *v) const { for (int i = 0; i < 3; i++) v[CE_POS + i] = cam.pos[c][i]; for (int i = 0; i < 4; i++) v[CE_QUAT + i] = cam.quat[c][i]; v[CE_FOVY] = cam.fovy[c]; }
+  bool pull_camenv(std::vector<real> &all) {
+    const size_t w = (size_t)n * cam.k * CAMENV_SLOT;
+    all.assign(w, real(0));
+    if (!d_camenv) return true;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemcpyAsync(all.data(), d_camenv, sizeof(real) * w, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  bool set_env_cameras(const double *pos, const double *quat, const double *fovy, const unsigned char *mask) override {
+    const std::string verb = "cassie_batch_set_env_cameras";
+    const int k = cam.k;
+    if (!k) { set_err(verb + ": no cameras are set (cassie_batch_set_cameras)"); return false; }
+    for (int e = 0; e < n; e++) {   // every masked value is checked before anything changes
+      if (mask && !mask[e]) continue;
+      for (int c = 0; c < k; c++) {
+        const size_t i = (size_t)e * k + c; const std::string at = verb + ": environment " + std::to_string(e) + ", camera " + std::to_string(c) + ": ";
+        if (pos && !std::isfinite(pos[3 * i] + pos[3 * i + 1] + pos[3 * i + 2])) { set_err(at + "pos must be finite"); return false; }
+        if (quat) {
+          const double *q = quat + 4 * i, nq = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+          if (!(nq > 0) || !std::isfinite(nq)) { set_err(at + "quat must be finite and non-zero"); return false; }
+        }
+        if (fovy && !(fovy[i] > 0 && fovy[i] < 180)) { set_err(at + "fovy must be in (0, 180) degrees"); return false; }
+      }
+    }
+    std::vector<real> all;
+    if (!d_camenv) {   // the first call: every environment starts from the set's mounts
+      ce_host.resize((size_t)n * k * CAMENV_SLOT); all.resize(ce_host.size());
+      for (int e = 0; e < n; e++) for (int c = 0; c < k; c++) model_camenv(c, &ce_host[((size_t)e * k + c) * CAMENV_SLOT]);
+      for (size_t i = 0; i < all.size(); i++) all[i] = (real)ce_host[i];
+    } else if (!pull_camenv(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      for (int c = 0; c < k; c++) {
+        const size_t i = (size_t)e * k + c; double *h = &ce_host[i * CAMENV_SLOT]; real *r = &all[i * CAMENV_SLOT];
+        if (pos) for (int j = 0; j < 3; j++) { h[CE_POS + j] = pos[3 * i + j]; r[CE_POS + j] = (real)h[CE_POS + j]; }
+        if (quat) for (int j = 0; j < 4; j++) { h[CE_QUAT + j] = quat[4 * i + j]; r[CE_QUAT + j] = (real)h[CE_QUAT + j]; }
+        if (fovy) { h[CE_FOVY] = fovy[i]; r[CE_FOVY] = (real)h[CE_FOVY]; }
+      }
+    }
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a render in flight reads the rows
+    if (!d_camenv) CUDA_OK(cudaMalloc(&d_camenv, sizeof(real) * all.size()));
+    CUDA_OK(cudaMemcpy(d_camenv, all.data(), sizeof(real) * all.size(), cudaMemcpyHostToDevice));
+    return true;
+  }
+  bool get_env_cameras(double *pos, double *quat, double *fovy) override {
+    const int k = cam.k;
+    if (!k) { set_err("cassie_batch_get_env_cameras: no cameras are set (cassie_batch_set_cameras)"); return false; }
+    std::vector<real> all;
+    if (!pull_camenv(all)) return false;
+    for (int e = 0; e < n; e++) for (int c = 0; c < k; c++) {
+      const size_t i = (size_t)e * k + c; double v[CAMENV_SLOT];
+      model_camenv(c, v);
+      if (d_camenv) for (int f = 0; f < CAMENV_SLOT; f++) {
+        const double h = ce_host[i * CAMENV_SLOT + f]; const real dv = all[i * CAMENV_SLOT + f];
+        v[f] = dv == (real)h ? h : (double)dv;
+      }
+      if (pos) for (int j = 0; j < 3; j++) pos[3 * i + j] = v[CE_POS + j];
+      if (quat) for (int j = 0; j < 4; j++) quat[4 * i + j] = v[CE_QUAT + j];
+      if (fovy) fovy[i] = v[CE_FOVY];
+    }
+    return true;
+  }
+  bool clear_env_cameras() override {   // back to the set's mounts
+    ce_host.clear();
+    if (!d_camenv) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_camenv)); d_camenv = nullptr;
+    return true;
   }
   // open-loop sinusoidal gait on the motor-PD targets (BASELINE config 5 "random PD gaits"): evaluated in the kernel every control tick, so
   // multi-tick launches follow it without a host round trip; installing it restarts the tick clock
@@ -1985,7 +2123,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "camera_env")) return d_camenv; if (!strcmp(f, "camera_geom")) return d_camgeom; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
     if (!strcmp(f, "applied")) return d_app;
     if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
@@ -2015,7 +2153,7 @@ template <typename real> struct Batch : BatchBase {
 
 // ====================================================================== C-ABI
 using namespace cassie;
-static_assert(CASSIE_CAM_MAXDIM == CAM_MAXDIM, "camera image size");
+static_assert(CASSIE_CAM_MAXDIM == CAM_MAXDIM && CASSIE_CAM_MAX == CAM_MAX && CASSIE_CAMENV_SLOT == CAMENV_SLOT, "camera set and rows");
 static_assert(CASSIE_RAY_MAX == RAY_MAX && CASSIE_RAY_SLOT == RAY_SLOT && CASSIE_RAY_HEADING == RAY_HEADING && CASSIE_RAY_ROOT == RAY_ROOT && CASSIE_RAY_WORLD == RAY_WORLD, "ray table and rows");
 static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == FJ_COLS, "frame Jacobian row layout");
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
@@ -2101,7 +2239,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "pd")) return PD_W; if (!strcmp(field, "obs")) return OBS_W; if (!strcmp(field, "xfrc")) return XFRC_W; if (!strcmp(field, "aux")) return AUX_W;
   if (!strcmp(field, "frames")) return (int)(b->impl->frame_list.size() / 2) * FRAME_W; if (!strcmp(field, "frame_jac")) return FRAME_JAC_W;
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
-  if (!strcmp(field, "depth")) return b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
+  if (!strcmp(field, "depth") || !strcmp(field, "camera_geom")) return b->impl->cam.k * b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "camera_env")) return b->impl->cam.k * CAMENV_SLOT; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "trace")) return b->impl->trace_width();
   if (!strcmp(field, "contacts")) return CON_W;
   if (!strcmp(field, "inv_qacc")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN; if (!strcmp(field, "inv")) return INV_W;
@@ -2599,23 +2737,48 @@ int cassie_batch_set_rays(cassie_batch_t *b, const int *frame, const double *ori
 int cassie_batch_nrays(const cassie_batch_t *b) { return b->impl->nray; }
 int cassie_batch_raycast(cassie_batch_t *b) { return b->impl->raycast() ? 0 : -1; }
 int cassie_batch_get_rays(cassie_batch_t *b, double *out) { return b->impl->get_rays(out) ? 0 : -1; }
-int cassie_batch_set_camera(cassie_batch_t *b, const char *camera, int width, int height, double zfar) {
-  const HostModel &hm = b->impl->hm;
-  if (width == 0) return b->impl->set_camera(-1, nullptr, nullptr, 0, 0, 0, 0, "cassie_batch_set_camera") ? 0 : -1;
+// the index of a fixed <camera> of the model, or -1 with the error recorded under `verb`
+static int fixed_camera(const HostModel &hm, const char *camera, const char *verb) {
   const int k = camera ? hm.camera_id(camera) : -1;
   if (k < 0) {
     std::string names; for (const std::string &c : hm.names_camera) names += (names.empty() ? "" : ", ") + c;
-    set_err("cassie_batch_set_camera: unknown camera '" + std::string(camera ? camera : "") + "' (the model's cameras: " + (names.empty() ? "none" : names) + ")"); return -1;
+    set_err(std::string(verb) + ": unknown camera '" + std::string(camera ? camera : "") + "' (the model's cameras: " + (names.empty() ? "none" : names) + ")"); return -1;
   }
-  if (hm.camera_mode[k] != CAM_FIXED) { set_err("cassie_batch_set_camera: camera '" + std::string(camera) + "' is not a fixed camera (track / target modes are not rendered)"); return -1; }
-  return b->impl->set_camera(hm.camera_body[k], &hm.camera_pos[3 * k], &hm.camera_quat[4 * k], hm.camera_fovy[k], width, height, zfar, "cassie_batch_set_camera") ? 0 : -1;
+  if (hm.camera_mode[k] != CAM_FIXED) { set_err(std::string(verb) + ": camera '" + std::string(camera) + "' is not a fixed camera (track / target modes are not rendered)"); return -1; }
+  return k;
+}
+int cassie_batch_set_camera(cassie_batch_t *b, const char *camera, int width, int height, double zfar) {
+  const HostModel &hm = b->impl->hm;
+  if (width == 0) return b->impl->set_cameras(0, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, "cassie_batch_set_camera", false) ? 0 : -1;
+  const int k = fixed_camera(hm, camera, "cassie_batch_set_camera");
+  if (k < 0) return -1;
+  return b->impl->set_cameras(1, &hm.camera_body[k], &hm.camera_pos[3 * k], &hm.camera_quat[4 * k], &hm.camera_fovy[k], width, height, zfar, "cassie_batch_set_camera", false) ? 0 : -1;
 }
 int cassie_batch_set_camera_mount(cassie_batch_t *b, const char *body, const double pos[3], const double quat[4], double fovy, int width, int height, double zfar) {
-  if (width == 0) return b->impl->set_camera(-1, nullptr, nullptr, 0, 0, 0, 0, "cassie_batch_set_camera_mount") ? 0 : -1;
+  if (width == 0) return b->impl->set_cameras(0, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, "cassie_batch_set_camera_mount", false) ? 0 : -1;
   const int id = body ? b->impl->hm.body_id(body) : -1;
   if (id < 0) { set_err("cassie_batch_set_camera_mount: unknown body '" + std::string(body ? body : "") + "'"); return -1; }
-  return b->impl->set_camera(id, pos, quat, fovy, width, height, zfar, "cassie_batch_set_camera_mount") ? 0 : -1;
+  return b->impl->set_cameras(1, &id, pos, quat, &fovy, width, height, zfar, "cassie_batch_set_camera_mount", false) ? 0 : -1;
 }
+int cassie_batch_set_cameras(cassie_batch_t *b, int k, const int *body, const double *pos, const double *quat, const double *fovy, int width, int height, double zfar) {
+  return b->impl->set_cameras(k, body, pos, quat, fovy, width, height, zfar, "cassie_batch_set_cameras", true) ? 0 : -1;
+}
+int cassie_batch_model_camera(cassie_batch_t *b, const char *camera, int *body, double pos[3], double quat[4], double *fovy) {
+  const HostModel &hm = b->impl->hm;
+  const int k = fixed_camera(hm, camera, "cassie_batch_model_camera");
+  if (k < 0) return -1;
+  if (body) *body = hm.camera_body[k];
+  if (pos) for (int i = 0; i < 3; i++) pos[i] = hm.camera_pos[3 * k + i];
+  if (quat) for (int i = 0; i < 4; i++) quat[i] = hm.camera_quat[4 * k + i];
+  if (fovy) *fovy = hm.camera_fovy[k];
+  return 0;
+}
+int cassie_batch_ncameras(const cassie_batch_t *b) { return b->impl->cam.k; }
+int cassie_batch_set_env_cameras(cassie_batch_t *b, const double *pos, const double *quat, const double *fovy, const unsigned char *mask) { return b->impl->set_env_cameras(pos, quat, fovy, mask) ? 0 : -1; }
+int cassie_batch_get_env_cameras(cassie_batch_t *b, double *pos, double *quat, double *fovy) { return b->impl->get_env_cameras(pos, quat, fovy) ? 0 : -1; }
+int cassie_batch_clear_env_cameras(cassie_batch_t *b) { return b->impl->clear_env_cameras() ? 0 : -1; }
+int cassie_batch_enable_camera_geoms(cassie_batch_t *b, int on) { return b->impl->enable_camera_geoms(on != 0) ? 0 : -1; }
+int cassie_batch_get_camera_geoms(cassie_batch_t *b, int *out) { return b->impl->get_camera_geoms(out) ? 0 : -1; }
 int cassie_batch_render_depth(cassie_batch_t *b) { return b->impl->render_depth() ? 0 : -1; }
 int cassie_batch_get_depth(cassie_batch_t *b, double *out) { return b->impl->get_depth(out) ? 0 : -1; }
 int cassie_batch_dynamics(cassie_batch_t *b) { return b->impl->dynamics() ? 0 : -1; }

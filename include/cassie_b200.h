@@ -250,9 +250,10 @@ int cassie_batch_set_rays(cassie_batch_t *b, const int *frame, const double *ori
 int cassie_batch_nrays(const cassie_batch_t *b);
 int cassie_batch_raycast(cassie_batch_t *b);
 int cassie_batch_get_rays(cassie_batch_t *b, double *out);
-/* Depth camera: one camera per batch, mounted on a body, rendered at the CURRENT qpos of every environment as a depth image -- the perception signal
- * of the reference's CassieVis draw_depth (an offscreen OpenGL render, one environment at a time), here one kernel launch for the batch.
- * The camera looks along its -z axis, +y is image up, fovy is the full vertical angle (degrees).  Pixel (r, c) of a width x height image is taken at
+/* Depth cameras: a set of up to CASSIE_CAM_MAX cameras per batch, each mounted on a body, rendered at the CURRENT qpos of every environment as depth
+ * images -- the perception signal of the reference's CassieVis draw_depth (an offscreen OpenGL render, one environment at a time), here one kernel
+ * launch for the batch and every camera of the set (the body poses are composed once per environment for all of them).
+ * A camera looks along its -z axis, +y is image up, fovy is the full vertical angle (degrees).  Pixel (r, c) of a width x height image is taken at
  * its centre, row 0 at the TOP; its value is the z-depth (distance along the optical axis, metres) of the first hit in (0, zfar], and zfar where
  * nothing is hit within zfar.  (The reference's mjr_readPixels buffer is bottom row first and holds OpenGL's non-linear depth; the values here are
  * linear metres.)  What is seen: the static collision geoms with the ray rules (each environment's own placement and terrain), and the moving
@@ -262,17 +263,47 @@ int cassie_batch_get_rays(cassie_batch_t *b, double *out);
  * camera the caller mounts on a named body, pos / quat in the body frame (quat is normalised).  Either returns 0, or -1 with nothing changed
  * (cassie_b200_last_error) for an unknown camera or body (the message lists the model's cameras), a camera that is not fixed, fovy outside
  * (0, 180), width or height outside 1 .. CASSIE_CAM_MAXDIM, zfar <= 0 or not finite, a zero or non-finite quaternion.  width = 0 drops the
- * camera.  Every successful set drops the rows: a device pointer taken before it is no longer valid.
- * cassie_batch_render_depth: one launch on the batch stream (asynchronous); it writes nothing but the rows [n][height][width] in the batch precision
- * (allocated by the first render after a set; snapshots, resets and cassie_sim_copy leave them alone).
- * cassie_batch_get_depth: synchronous copy [n][height][width] doubles; -1 before the first render after a set.  Device rows:
- * cassie_batch_device_ptr(b, "depth"), row width height x width. */
+ * camera.  Either is a set of one camera.  Every successful set drops the depth, geom-id and per-environment mount rows: a device pointer taken
+ * before it is no longer valid.
+ * cassie_batch_set_cameras: k cameras sharing one image size and zfar; body [k] in the model's numbering (cassie_batch_name2id(b, "body", ..)),
+ * pos [k][3], quat [k][4] (normalised), fovy [k].  Each is checked as set_camera_mount checks its mount; a refusal returns -1 with nothing changed
+ * and names the camera ("camera i: ...").  k = 0 drops the set.  cassie_batch_model_camera: the mount of a fixed <camera> of the model (body,
+ * pos, quat as the model has them, fovy); -1 for an unknown or non-fixed camera.  cassie_batch_ncameras: k of the current set (0: none).
+ * cassie_batch_render_depth: one launch on the batch stream (asynchronous); it writes nothing but the rows [n][k][height][width] in the batch
+ * precision, and the geom-id rows when enabled (allocated by the first render after a set; snapshots, resets and cassie_sim_copy leave them alone).
+ * cassie_batch_get_depth: synchronous copy [n][k][height][width] doubles; -1 before the first render after a set.  Device rows:
+ * cassie_batch_device_ptr(b, "depth"), row width k x height x width (for k = 1 the layout of a one-camera batch).
+ * Per-environment mounts (extrinsics and field-of-view randomisation): cassie_batch_set_env_cameras gives environment e's camera c its own pose in
+ * the camera's body frame and its own fovy: pos [n][k][3], quat [n][k][4], fovy [n][k]; any part may be NULL (kept); mask [n] (NULL: all)
+ * selects the environments that change.  The first call starts every environment from the set's mounts.  A non-finite value, a zero quaternion or
+ * a fovy outside (0, 180) returns -1 with nothing changed; the error names the environment, the camera and the field.  get reports what every
+ * environment sees, with or without rows; clear returns to the set's mounts.  Device rows: cassie_batch_device_ptr(b, "camera_env")
+ * [n][k][CASSIE_CAMENV_SLOT] in the batch precision: pos[3], quat[4], fovy in degrees, read at the next render.  The kernel normalises the
+ * quaternion and forms tan(fovy / 2) itself, so rows written on the device need no host call; a slot with a non-finite value, a zero quaternion or a
+ * fovy outside (0, 180) renders nothing (zfar and geom -1 on every pixel of that camera).  The rows are a model input: resets, reset_where,
+ * set_state and snapshot restores leave them alone, cassie_sim_copy copies them (between sets of as many cameras; otherwise it drops the
+ * destination's).  The body of each camera is the set's in every environment.
+ * Geom ids: cassie_batch_enable_camera_geoms(b, 1) makes every render also write int32 rows [n][k][height][width]
+ * (cassie_batch_device_ptr(b, "camera_geom")): the model geom id (cassie_batch_id2name(b, "geom", id)) of the surface that set the pixel's depth,
+ * -1 where nothing lies within zfar; on a tie the static geom, then the lower device index.  0 frees them.  cassie_batch_get_camera_geoms copies
+ * them; -1 before the first render with geom ids after a set or an enable. */
 #define CASSIE_CAM_MAXDIM 256
+#define CASSIE_CAM_MAX 4
+#define CASSIE_CAMENV_SLOT 8
 int cassie_batch_set_camera(cassie_batch_t *b, const char *camera, int width, int height, double zfar);
 int cassie_batch_set_camera_mount(cassie_batch_t *b, const char *body, const double pos[3], const double quat[4], double fovy,
                                   int width, int height, double zfar);
+int cassie_batch_set_cameras(cassie_batch_t *b, int k, const int *body, const double *pos, const double *quat, const double *fovy, int width, int height,
+                             double zfar);
+int cassie_batch_model_camera(cassie_batch_t *b, const char *camera, int *body, double pos[3], double quat[4], double *fovy);
+int cassie_batch_ncameras(const cassie_batch_t *b);
 int cassie_batch_render_depth(cassie_batch_t *b);
 int cassie_batch_get_depth(cassie_batch_t *b, double *out);
+int cassie_batch_set_env_cameras(cassie_batch_t *b, const double *pos, const double *quat, const double *fovy, const unsigned char *mask);
+int cassie_batch_get_env_cameras(cassie_batch_t *b, double *pos, double *quat, double *fovy);
+int cassie_batch_clear_env_cameras(cassie_batch_t *b);
+int cassie_batch_enable_camera_geoms(cassie_batch_t *b, int on);
+int cassie_batch_get_camera_geoms(cassie_batch_t *b, int *out);
 /* include/cassiemujoco.h:61-73 (src/cassiemujoco.c:1072-1093): model (per-environment constants, height field, timestep) + full dynamic state */
 cassie_sim_t *cassie_sim_duplicate(const cassie_sim_t *src);
 void cassie_sim_copy(cassie_sim_t *dst, const cassie_sim_t *src);
