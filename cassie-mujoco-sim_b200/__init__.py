@@ -733,6 +733,63 @@ class CassieBatch:
         if self._applied_lib().cassie_batch_enable_applied_forces(self.h, 1 if on else 0) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- sensor models drawn in the step kernel (encoder offsets and noise, IMU mount, bias and noise: sim-to-real randomisation)
+    def _sensor_lib(self):
+        L = self.L
+        if not getattr(L, '_sensor_bound', False):
+            vp, dp, up = C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_ulonglong)
+            L.cassie_batch_set_env_sensors.argtypes = [vp, dp, dp, dp, dp, dp, vp]
+            L.cassie_batch_get_env_sensors.argtypes = [vp, dp, dp, dp, dp, dp]
+            L.cassie_batch_clear_env_sensors.argtypes = [vp]
+            L.cassie_batch_seed_sensors.argtypes = [vp, C.c_ulonglong, vp]
+            L.cassie_batch_get_sensor_rng.argtypes = [vp, up, up]
+            for n in ('set_env_sensors', 'get_env_sensors', 'clear_env_sensors', 'seed_sensors', 'get_sensor_rng'):
+                getattr(L, 'cassie_batch_' + n).restype = C.c_int
+            L._sensor_bound = True
+        return L
+
+    _SENSOR_SHAPES = (('enc_offset', (16,)), ('enc_noise', (16,)), ('imu_quat', (4,)), ('imu_bias', (6,)), ('imu_noise', (9,)))
+
+    def set_env_sensors(self, enc_offset=None, enc_noise=None, imu_quat=None, imu_bias=None, imu_noise=None, mask=None):
+        """each environment's sensor model, applied every tick to what the controller, the safety layer, the encoder filters and the estimator measure:
+        enc_offset / enc_noise [16] or [n, 16] -- offset and noise std of the encoders in cassie_out order (10 drives, 6 joints), output radians --,
+        imu_quat [4] or [n, 4] -- the IMU mount q_m (w x y z, normalised on write): orientation q (x) q_m, rates and accelerations R_m' v --, imu_bias [6]
+        or [n, 6] -- gyro, accelerometer --, imu_noise [9] or [n, 9] -- std of the orientation (rad), gyro, accelerometer.  A part left None is kept;
+        mask [n]: only the selected environments change.  A non-finite value, a negative std or a zero quaternion raises, and nothing changes.  Reset and
+        snapshot restore leave the rows alone.  The first call seeds the generator as seed_sensors(0)."""
+        L = self._sensor_lib()
+        a = [self._arr(v, np.float64, (self.n,) + sh) for v, (_, sh) in zip((enc_offset, enc_noise, imu_quat, imu_bias, imu_noise), self._SENSOR_SHAPES)]
+        m = self._arr(mask, np.uint8, (self.n,))
+        if L.cassie_batch_set_env_sensors(self.h, *[None if v is None else self._dp(v) for v in a], None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def env_sensors(self):
+        """dict of enc_offset [n, 16], enc_noise [n, 16], imu_quat [n, 4], imu_bias [n, 6], imu_noise [n, 9]: what the rows hold (the zero model without rows)"""
+        L = self._sensor_lib()
+        out = [np.zeros((self.n,) + sh) for _, sh in self._SENSOR_SHAPES]
+        if L.cassie_batch_get_env_sensors(self.h, *[self._dp(v) for v in out]) != 0:
+            raise RuntimeError(_last_error())
+        return dict(zip([k for k, _ in self._SENSOR_SHAPES], out))
+
+    def clear_env_sensors(self):
+        """back to perfect sensors and the kernel instances that ran before"""
+        if self._sensor_lib().cassie_batch_clear_env_sensors(self.h) != 0:
+            raise RuntimeError(_last_error())
+
+    def seed_sensors(self, seed, mask=None):
+        """environment i draws from key seed + i, counter 0 (mask [n]: only the selected environments); set_env_sensors first"""
+        m = self._arr(mask, np.uint8, (self.n,))
+        if self._sensor_lib().cassie_batch_seed_sensors(self.h, C.c_ulonglong(int(seed) & (2 ** 64 - 1)), None if m is None else m.ctypes.data_as(C.c_void_p)) != 0:
+            raise RuntimeError(_last_error())
+
+    def sensor_rng(self):
+        """(key [n], counter [n]) uint64: the generator each environment draws from; step launches advance the counter by their tick count"""
+        key, ctr = np.zeros(self.n, dtype=np.uint64), np.zeros(self.n, dtype=np.uint64)
+        up = C.POINTER(C.c_ulonglong)
+        if self._sensor_lib().cassie_batch_get_sensor_rng(self.h, key.ctypes.data_as(up), ctr.ctypes.data_as(up)) != 0:
+            raise RuntimeError(_last_error())
+        return key, ctr
+
     # ---- per-tick traces of multi-tick launches
     def _trace_lib(self):
         L = self.L
@@ -1300,7 +1357,8 @@ class CassieBatch:
         compute_inverse(None), column = dof; inv [n, INV_WIDTH] laid out as INV; both allocated by the first request; contacts [n, CON_WIDTH]: the contact
         lists of the last step / forward launch, a header and CON_MAX slots laid out as CON; enable_contacts first; camera_env [n, k, CAMENV_SLOT]: the
         per-environment camera mounts pos[3], quat[4], fovy in degrees, read at the next render; set_env_cameras first; camera_geom [n, k, height, width]
-        int32 (shaped as depth for set_camera): the geom ids of the last render; enable_camera_geoms and render_depth first).  set_frames /
+        int32 (shaped as depth for set_camera): the geom ids of the last render; enable_camera_geoms and render_depth first; sensors [n, 52] laid out as
+        SN, read at the next launch; sensor_rng [n, 4] int32: key lo, hi, counter lo, hi; set_env_sensors first for both).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -1310,9 +1368,9 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first; sensors, sensor_rng: set_env_sensors first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
-        if field in ('terrain', 'camera_geom'):
+        if field in ('terrain', 'camera_geom', 'sensor_rng'):
             ts = '<i4'
 
         class _Arr:

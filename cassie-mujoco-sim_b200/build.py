@@ -69,6 +69,13 @@ TRACE_INSTANCES = [('f1fc4', 'float', 1, 4036), ('f1fd7', 'float', 1, 4055), ('d
 # twins read; tag = precision, kind, features in hex
 CONTACT_LIST_INSTANCES = [('f117d7', 'float', 1, 6103), ('d117d7', 'double', 1, 6103), ('f117df', 'float', 1, 6111), ('d117df', 'double', 1, 6111),
                           ('f117ff', 'float', 1, 6143), ('d117ff', 'double', 1, 6143)]
+# sensor models (feature 8192 = F_SN; cassie_batch_set_env_sensors): encoder offsets and noise, IMU mount, bias and noise applied to the controller stage's
+# copy of the sensordata every tick.  The plain twins f02404 / f22404 (F_SN | F_XF | F_BOX) run where f04 / f24 / f0404 / f2404 would, with zeroed applied
+# rows when the batch has none; any other batch with sensor rows runs the F_SN twin of the F_XF chain twin its rule picks (f17c4, f17d7 / d17d7, f17df /
+# d17df, f17ff / d17ff), with the model-valued applied, contact, mechanics, actuator and offset rows the chain twins read; tag = precision, kind, features in hex
+SENSOR_INSTANCES = [('f02404', 'float', 0, 9220), ('f22404', 'float', 2, 9220),
+                    ('f127c4', 'float', 1, 10180), ('f127d7', 'float', 1, 10199), ('d127d7', 'double', 1, 10199), ('f127df', 'float', 1, 10207), ('d127df', 'double', 1, 10207),
+                    ('f127ff', 'float', 1, 10239), ('d127ff', 'double', 1, 10239)]
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC,-fopenmp'] + os.environ.get('CASSIE_B200_NVCC_EXTRA', '').split()   # extra flags for A/B builds
 
 
@@ -102,7 +109,7 @@ def build(force=False, verbose=False, out=None):
     os.makedirs(OBJ, exist_ok=True)
     ptx = ['-Xptxas', '-v'] if verbose else []
     jobs = []
-    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES + APPLIED_INSTANCES + TRACE_INSTANCES + CONTACT_LIST_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
+    for tag, real, dr, feat in INSTANCES + ENV_GEOM_INSTANCES + FRAME_INSTANCES + TERRAIN_INSTANCES + BODY_POS_INSTANCES + ACTUATOR_INSTANCES + MECHANICS_INSTANCES + CONTACT_INSTANCES + APPLIED_INSTANCES + TRACE_INSTANCES + CONTACT_LIST_INSTANCES + SENSOR_INSTANCES:   # always -Xptxas -v: tests/test_step_resources.py reads the spill counts from csrc/_obj/step_<tag>.res
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DINST_REAL=' + real, '-DINST_DR=%d' % dr, '-DINST_FEAT=%d' % feat, '-DINST_TAG=' + tag, '-c', os.path.join(CSRC, 'step_inst.cu'),
                                            '-o', os.path.join(OBJ, 'step_%s.o' % tag)])
     jobs.append([nvcc()] + ARCH + ptx + ['-c', os.path.join(CSRC, 'cassie_b200.cu'), '-o', os.path.join(OBJ, 'cassie_b200.o')])

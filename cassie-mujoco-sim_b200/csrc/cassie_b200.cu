@@ -41,6 +41,8 @@ CASSIE_STEP_ENTRY(f0404) CASSIE_STEP_ENTRY(f2404)
 CASSIE_STEP_ENTRY(f17c4) CASSIE_STEP_ENTRY(f17d7) CASSIE_STEP_ENTRY(d17d7) CASSIE_STEP_ENTRY(f17df) CASSIE_STEP_ENTRY(d17df) CASSIE_STEP_ENTRY(f17ff) CASSIE_STEP_ENTRY(d17ff)
 CASSIE_STEP_ENTRY(f1fc4) CASSIE_STEP_ENTRY(f1fd7) CASSIE_STEP_ENTRY(d1fd7) CASSIE_STEP_ENTRY(f1fdf) CASSIE_STEP_ENTRY(d1fdf) CASSIE_STEP_ENTRY(f1fff) CASSIE_STEP_ENTRY(d1fff)
 CASSIE_STEP_ENTRY(f117d7) CASSIE_STEP_ENTRY(d117d7) CASSIE_STEP_ENTRY(f117df) CASSIE_STEP_ENTRY(d117df) CASSIE_STEP_ENTRY(f117ff) CASSIE_STEP_ENTRY(d117ff)
+CASSIE_STEP_ENTRY(f02404) CASSIE_STEP_ENTRY(f22404)
+CASSIE_STEP_ENTRY(f127c4) CASSIE_STEP_ENTRY(f127d7) CASSIE_STEP_ENTRY(d127d7) CASSIE_STEP_ENTRY(f127df) CASSIE_STEP_ENTRY(d127df) CASSIE_STEP_ENTRY(f127ff) CASSIE_STEP_ENTRY(d127ff)
 #undef CASSIE_STEP_ENTRY
 
 namespace cassie {
@@ -52,6 +54,21 @@ template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device
 
 // the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
 template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
+  if (feat & F_SN) {   // sensor models: the F_SN twins of the F_XF instances, by their rule (a batch with sensor rows always has applied rows); none with a
+                       // trace or contact lists
+    if (feat & (F_TC | F_CL)) return nullptr;
+    const bool dbl = std::is_same<real, double>::value;
+    if (inst != 1) {   // null: the batch runs the extended kind (step_range)
+      if (dbl || (feat & ~(F_XF | F_SN)) != F_BOX) return nullptr;
+      if (compiled_feat) *compiled_feat = F_BOX | F_XF | F_SN;
+      return inst == 2 ? cassie_step_entry_f22404() : cassie_step_entry_f02404();
+    }
+    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN; return dbl ? cassie_step_entry_d127ff() : cassie_step_entry_f127ff(); }
+    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN; return dbl ? cassie_step_entry_d127df() : cassie_step_entry_f127df(); }
+    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN; return cassie_step_entry_f127c4(); }
+    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN;
+    return dbl ? cassie_step_entry_d127d7() : cassie_step_entry_f127d7();
+  }
   if (feat & F_CL) {   // contact lists: the F_CL twins of the F_FR chain twins (a batch with contact lists always has applied rows)
     if (inst != 1) return nullptr;
     const bool dbl = std::is_same<real, double>::value;
@@ -406,6 +423,14 @@ struct BatchBase {
   // get copies [n][CON_W]
   virtual bool enable_contacts(bool on) = 0;
   virtual bool get_contacts(double *out) = 0;
+  // sensor models (F_SN instances; a model input): encoder offset [n][16] and std [n][16], IMU mount [n][4], bias [n][6] (gyro, accelerometer) and std
+  // [n][9] (orientation, gyro, accelerometer); null parts are kept, only masked environments change, checked as a whole before anything changes.  The
+  // generator rows: key seed + i and counter 0 for the masked environments; get returns key and counter [n] each
+  virtual bool set_env_sensors(const double *enc_offset, const double *enc_noise, const double *imu_quat, const double *imu_bias, const double *imu_noise, const unsigned char *mask) = 0;
+  virtual bool get_env_sensors(double *enc_offset, double *enc_noise, double *imu_quat, double *imu_bias, double *imu_noise) = 0;
+  virtual bool clear_env_sensors() = 0;
+  virtual bool seed_sensors(unsigned long long seed, const unsigned char *mask) = 0;
+  virtual bool get_sensor_rng(unsigned long long *seed, unsigned long long *counter) = 0;
   // the controller-stage state of every environment (views of the cst / dfilt rows): delay line [n][10][6], drive FIR taps [n][10][9], joint IIR
   // filters x [n][6][4] and y [n][6][3]; null parts are skipped, set changes masked environments only
   virtual bool get_actuator_state(double *torque_delay, int *drive_filter, double *joint_x, double *joint_y) = 0;
@@ -499,13 +524,14 @@ template <typename real> struct Batch : BatchBase {
   bool ct_mech = false;                    // the mechanics rows were allocated by the contact setter (model values), and no mechanics call has written them since
   real *d_app = nullptr;                   // A.applied: [n][APPLIED_W] per-environment applied forces (state), allocated by the first applied-force verb (F_XF instances)
   bool xf_ct = false;                      // the contact rows were allocated for the chain twin (model values), and no contact call has written them since
-  bool tc_app = false;                     // the applied-force rows were allocated for the trace instances (zero), and no applied-force verb has written them since
+  bool tc_app = false;                     // the applied-force rows were allocated for the trace, contact-list or sensor instances (zero), and no applied-force verb has
+                                           // written them since
   int tc_ticks = 0;                        // slots the last step launch wrote into the trace rows (A.trace: [n][T][k], allocated by cassie_batch_set_trace)
   Snap *bank = nullptr;                    // the reset bank (cassie_batch_set_reset_bank): a snapshot of k entries
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
+    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -580,9 +606,12 @@ template <typename real> struct Batch : BatchBase {
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), (int)cfg[ext].smem));   // and their F_CT twins
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), (int)cfg[ext].smem));   // and their F_XF twins
             CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_TC), (int)cfg[ext].smem));   // and their F_TC twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_CL), (int)cfg[ext].smem)); }   // and their F_CL twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_CL), (int)cfg[ext].smem));   // and their F_CL twins
+            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_SN), (int)cfg[ext].smem)); }   // and their F_SN twins
         if (ext != 1 && step_entry<real>(ext, feat | F_XF))   // the plain F_XF twins (applied forces), where this model runs f04 / f24
           CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF), (int)cfg[ext].smem));
+        if (ext != 1 && step_entry<real>(ext, feat | F_XF | F_SN))   // and their F_SN twins (sensor models)
+          CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF | F_SN), (int)cfg[ext].smem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
@@ -1040,6 +1069,12 @@ template <typename real> struct Batch : BatchBase {
       CUDA_OK(cudaMemcpy(d_ct, src->d_ct, sizeof(real) * n * CONTACT_W, cudaMemcpyDeviceToDevice));
       A.contact = d_ct;
     }
+    if (src->A.sn.rows) {   // the sensor models and the generator rows: a copy draws what its source would
+      if (!A.sn.rows && !alloc_sensors()) return false;
+      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
+      CUDA_OK(cudaMemcpy((void *)A.sn.rows, src->A.sn.rows, sizeof(real) * n * SN_W, cudaMemcpyDeviceToDevice));
+      CUDA_OK(cudaMemcpy(A.sn.rng, src->A.sn.rng, sizeof(int) * n * SR_W, cudaMemcpyDeviceToDevice));
+    } else if (!clear_env_sensors()) return false;
     if (src->d_hfield) {
       const size_t cells = (size_t)hm.hfield_nrow[0] * hm.hfield_ncol[0] * src->A.n_terrain;
       std::vector<float> tmp(cells); CUDA_OK(cudaMemcpy(tmp.data(), src->d_hfield, sizeof(float) * cells, cudaMemcpyDeviceToHost));
@@ -1616,6 +1651,7 @@ template <typename real> struct Batch : BatchBase {
     const std::string verb = "cassie_batch_set_trace: ";
     if (legacy) { set_err(verb + "the batch belongs to a cassie_sim_t"); return false; }
     if (k > 0 && A.cl.rows) { set_err(verb + "the batch has contact lists (cassie_batch_enable_contacts); a trace and contact lists do not combine"); return false; }
+    if (k > 0 && A.sn.rows) { set_err(verb + "the batch has sensor models (cassie_batch_set_env_sensors); a trace and sensor models do not combine"); return false; }
     if (k < 0 || k > TRACE_MAX) { set_err(verb + "between 0 and " + std::to_string(TRACE_MAX) + " columns"); return false; }
     std::vector<int> codes((size_t)k);
     int need = 0;
@@ -1658,6 +1694,7 @@ template <typename real> struct Batch : BatchBase {
   // written them since
   bool enable_contacts(bool on) override {
     if (on && A.trace.rows) { set_err("cassie_batch_enable_contacts: the batch has a per-tick trace (cassie_batch_set_trace); a trace and contact lists do not combine"); return false; }
+    if (on && A.sn.rows) { set_err("cassie_batch_enable_contacts: the batch has sensor models (cassie_batch_set_env_sensors); contact lists and sensor models do not combine"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (on && !A.cl.rows) {
       if (!chain_twin_rows() || !geom_table()) return false;
@@ -1669,6 +1706,99 @@ template <typename real> struct Batch : BatchBase {
       CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight writes the rows
       CUDA_OK(cudaFree(A.cl.rows)); A.cl = ContactListArgs<real>{};   // (the geom table stays with the batch)
       if (tc_app) { tc_app = false; return enable_applied_forces(false); }   // back to the instances that ran before
+    }
+    return true;
+  }
+  // ---- sensor models: a model input like the actuator rows, read by the controller stage of every step tick.  The device rows are what the environments
+  // run with (a write through the device pointer takes effect at the next launch), so the verbs read them back and keep no mirror.  The sensor
+  // instances are the F_SN twins of the applied-force instances, so the batch carries applied-force rows (zero when it has none: tc_app)
+  bool alloc_sensors() {   // zero rows with the identity mount, generator rows seeded as seed_sensors(0, all)
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    std::vector<real> rows((size_t)n * SN_W, real(0)); std::vector<int> rng((size_t)n * SR_W, 0);
+    for (int e = 0; e < n; e++) { rows[(size_t)e * SN_W + SN_QUAT] = 1; rng[(size_t)e * SR_W] = e; }
+    real *r = nullptr; int *g = nullptr;
+    CUDA_OK(cudaMalloc(&r, sizeof(real) * n * SN_W)); CUDA_OK(cudaMalloc(&g, sizeof(int) * n * SR_W));
+    A.sn.rows = r; A.sn.rng = g;
+    CUDA_OK(cudaMemcpy(r, rows.data(), sizeof(real) * n * SN_W, cudaMemcpyHostToDevice)); CUDA_OK(cudaMemcpy(g, rng.data(), sizeof(int) * n * SR_W, cudaMemcpyHostToDevice));
+    if (!d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }
+    return true;
+  }
+  bool set_env_sensors(const double *enc_offset, const double *enc_noise, const double *imu_quat, const double *imu_bias, const double *imu_noise, const unsigned char *mask) override {
+    const std::string verb = "cassie_batch_set_env_sensors: ";
+    if (A.trace.rows) { set_err(verb + "the batch has a per-tick trace (cassie_batch_set_trace); sensor models and a trace do not combine"); return false; }
+    if (A.cl.rows) { set_err(verb + "the batch has contact lists (cassie_batch_enable_contacts); sensor models and contact lists do not combine"); return false; }
+    static const char *const bias_name[2] = {"gyro bias", "accelerometer bias"}, *const std_name[3] = {"orientation noise", "gyro noise", "accelerometer noise"};
+    for (int e = 0; e < n; e++) {   // every masked value first
+      if (mask && !mask[e]) continue;
+      const std::string env = verb + "environment " + std::to_string(e) + ", ";
+      for (int c = 0; c < 16; c++) {
+        if (enc_offset && !std::isfinite(enc_offset[(size_t)e * 16 + c])) { set_err(env + "encoder " + std::to_string(c) + ": the offset is not finite"); return false; }
+        if (enc_noise && !(std::isfinite(enc_noise[(size_t)e * 16 + c]) && enc_noise[(size_t)e * 16 + c] >= 0)) { set_err(env + "encoder " + std::to_string(c) + ": the noise std must be finite and >= 0"); return false; }
+      }
+      if (imu_quat) {
+        const double *q = imu_quat + (size_t)e * 4; double nn = 0;
+        for (int k = 0; k < 4; k++) { if (!std::isfinite(q[k])) { set_err(env + "IMU mount: quaternion component " + std::to_string(k) + " is not finite"); return false; } nn += q[k] * q[k]; }
+        if (!(nn > 0)) { set_err(env + "IMU mount: the quaternion is zero"); return false; }
+      }
+      for (int c = 0; imu_bias && c < 6; c++) if (!std::isfinite(imu_bias[(size_t)e * 6 + c])) { set_err(env + bias_name[c / 3] + " " + "xyz"[c % 3] + ": not finite"); return false; }
+      for (int c = 0; imu_noise && c < 9; c++) { const double v = imu_noise[(size_t)e * 9 + c]; if (!(std::isfinite(v) && v >= 0)) { set_err(env + std_name[c / 3] + " " + "xyz"[c % 3] + ": the std must be finite and >= 0"); return false; } }
+    }
+    if (!A.sn.rows && !alloc_sensors()) return false;   // the first call: the zero model
+    std::vector<real> all((size_t)n * SN_W);
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    CUDA_OK(cudaMemcpy(all.data(), A.sn.rows, sizeof(real) * n * SN_W, cudaMemcpyDeviceToHost));   // unmasked environments keep what their rows hold
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      real *r = &all[(size_t)e * SN_W];
+      for (int c = 0; c < 16; c++) { if (enc_offset) r[SN_ENC_OFF + c] = (real)enc_offset[(size_t)e * 16 + c]; if (enc_noise) r[SN_ENC_STD + c] = (real)enc_noise[(size_t)e * 16 + c]; }
+      if (imu_quat) { const double *q = imu_quat + (size_t)e * 4; const double nn = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]); for (int k = 0; k < 4; k++) r[SN_QUAT + k] = (real)(q[k] / nn); }
+      for (int k = 0; imu_bias && k < 3; k++) { r[SN_GYRO_BIAS + k] = (real)imu_bias[(size_t)e * 6 + k]; r[SN_ACC_BIAS + k] = (real)imu_bias[(size_t)e * 6 + 3 + k]; }
+      for (int k = 0; imu_noise && k < 3; k++) { r[SN_ORI_STD + k] = (real)imu_noise[(size_t)e * 9 + k]; r[SN_GYRO_STD + k] = (real)imu_noise[(size_t)e * 9 + 3 + k]; r[SN_ACC_STD + k] = (real)imu_noise[(size_t)e * 9 + 6 + k]; }
+    }
+    CUDA_OK(cudaMemcpy((void *)A.sn.rows, all.data(), sizeof(real) * n * SN_W, cudaMemcpyHostToDevice));
+    return true;
+  }
+  bool get_env_sensors(double *enc_offset, double *enc_noise, double *imu_quat, double *imu_bias, double *imu_noise) override {   // the zero model without rows
+    std::vector<real> all((size_t)n * SN_W, real(0));
+    if (A.sn.rows) { CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaMemcpyAsync(all.data(), A.sn.rows, sizeof(real) * n * SN_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
+    else for (int e = 0; e < n; e++) all[(size_t)e * SN_W + SN_QUAT] = 1;
+    for (int e = 0; e < n; e++) {
+      const real *r = &all[(size_t)e * SN_W];
+      for (int c = 0; c < 16; c++) { if (enc_offset) enc_offset[(size_t)e * 16 + c] = (double)r[SN_ENC_OFF + c]; if (enc_noise) enc_noise[(size_t)e * 16 + c] = (double)r[SN_ENC_STD + c]; }
+      for (int k = 0; imu_quat && k < 4; k++) imu_quat[(size_t)e * 4 + k] = (double)r[SN_QUAT + k];
+      for (int k = 0; imu_bias && k < 3; k++) { imu_bias[(size_t)e * 6 + k] = (double)r[SN_GYRO_BIAS + k]; imu_bias[(size_t)e * 6 + 3 + k] = (double)r[SN_ACC_BIAS + k]; }
+      for (int k = 0; imu_noise && k < 3; k++) { imu_noise[(size_t)e * 9 + k] = (double)r[SN_ORI_STD + k]; imu_noise[(size_t)e * 9 + 3 + k] = (double)r[SN_GYRO_STD + k]; imu_noise[(size_t)e * 9 + 6 + k] = (double)r[SN_ACC_STD + k]; }
+    }
+    return true;
+  }
+  bool clear_env_sensors() override {   // back to the instances that ran before
+    if (!A.sn.rows) return true;
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree((void *)A.sn.rows)); CUDA_OK(cudaFree(A.sn.rng)); A.sn = SensorArgs<real>{};
+    if (tc_app) { tc_app = false; return enable_applied_forces(false); }
+    return true;
+  }
+  bool seed_sensors(unsigned long long seed, const unsigned char *mask) override {
+    if (!A.sn.rows) { set_err("cassie_batch_seed_sensors: no sensor models (cassie_batch_set_env_sensors)"); return false; }
+    std::vector<int> g((size_t)n * SR_W);
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaMemcpy(g.data(), A.sn.rng, sizeof(int) * n * SR_W, cudaMemcpyDeviceToHost));
+    for (int e = 0; e < n; e++) {
+      if (mask && !mask[e]) continue;
+      const unsigned long long k = seed + (unsigned long long)e;
+      g[(size_t)e * SR_W] = (int)(uint32_t)k; g[(size_t)e * SR_W + 1] = (int)(uint32_t)(k >> 32); g[(size_t)e * SR_W + 2] = 0; g[(size_t)e * SR_W + 3] = 0;
+    }
+    CUDA_OK(cudaMemcpy(A.sn.rng, g.data(), sizeof(int) * n * SR_W, cudaMemcpyHostToDevice));
+    return true;
+  }
+  bool get_sensor_rng(unsigned long long *seed, unsigned long long *counter) override {
+    if (!A.sn.rows) { set_err("cassie_batch_get_sensor_rng: no sensor models (cassie_batch_set_env_sensors)"); return false; }
+    std::vector<int> g((size_t)n * SR_W);
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaMemcpyAsync(g.data(), A.sn.rng, sizeof(int) * n * SR_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    for (int e = 0; e < n; e++) {
+      const uint32_t *w = reinterpret_cast<const uint32_t *>(&g[(size_t)e * SR_W]);
+      if (seed) seed[e] = (unsigned long long)w[0] | ((unsigned long long)w[1] << 32);
+      if (counter) counter[e] = (unsigned long long)w[2] | ((unsigned long long)w[3] << 32);
     }
     return true;
   }
@@ -2033,7 +2163,7 @@ template <typename real> struct Batch : BatchBase {
     // the in-kernel estimator alone: the plain instance with the estimator stage
     int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || A.trace.rows || A.cl.rows || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
     // applied forces: a plain twin where f04 / f24 would run, else the chain twin
-    if (A.applied && ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF)) ext = 1;
+    if (A.applied && ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF | (A.sn.rows ? F_SN : 0))) ext = 1;
     return ext;
   }
   bool step_range(int nticks, int mode, int env0, int count, cudaStream_t on) {   // the launch covers environments [env0, env0 + count)
@@ -2045,6 +2175,7 @@ template <typename real> struct Batch : BatchBase {
     A.nsub = nsub_override;
     const int ext = launch_kind(mode);
     if ((A.trace.rows || A.cl.rows) && !chain_twin_rows()) return false;   // only after a verb dropped the rows set_trace / enable_contacts allocated
+    if (A.sn.rows && !d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }   // likewise the applied rows of set_env_sensors
     if (A.applied && ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }   // the chain twin reads contact rows (the model's values when none were set)
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
@@ -2054,7 +2185,7 @@ template <typename real> struct Batch : BatchBase {
     // mode 6: the caller's qacc reaches the lanes through the warm-start load (mode 6 writes no state back); the forward's stage dump, sensor data and
     // counters go to the launch's scratch rows, for inverse_row; no aux or frame rows
     if (mode == 6) { La.qacc_ws = d_iq; La.dbg = d_idbg; La.cst = d_icst; La.counters = d_icnt; La.aux = nullptr; La.nfr = 0; }
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | (A.cl.rows ? F_CL : 0) | ((A.frames || A.acc || A.cl.rows || mode == 5 || mode == 6) ? F_FR : 0);   // frame, acceleration, dynamics and inverse rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | (A.cl.rows ? F_CL : 0) | (A.sn.rows ? F_SN : 0) | ((A.frames || A.acc || A.cl.rows || mode == 5 || mode == 6) ? F_FR : 0);   // frame, acceleration, dynamics and inverse rows: the extended F_FR instance (set_const launches too: they write no frames)
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
       CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
@@ -2128,6 +2259,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
     if (!strcmp(f, "contacts")) return A.cl.rows;
+    if (!strcmp(f, "sensors")) return (void *)A.sn.rows; if (!strcmp(f, "sensor_rng")) return A.sn.rng;
 #ifdef CASSIE_STAGE_CLOCKS
     if (!strcmp(f, "stage_clocks")) return A.qM;   // [n][2 NM_MAX] reals, words 0.. the stage clocks of the last step sub-step (step_core.inl STAGE_CLOCK)
 #endif
@@ -2160,6 +2292,7 @@ static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_
 static_assert(CASSIE_INV_WIDTH == INV_W && CASSIE_INV_COLS == IV_COLS && CASSIE_INV_QFRC == IV_QFRC && CASSIE_INV_QFRCC == IV_QFRCC && CASSIE_INV_NEFC == IV_NEFC && CASSIE_INV_NCON == IV_NCON && CASSIE_INV_DROPPED == IV_DROPPED, "inverse row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
 static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
+static_assert(CASSIE_SENSOR_WIDTH == SN_W && CASSIE_SN_ENC_OFF == SN_ENC_OFF && CASSIE_SN_ENC_STD == SN_ENC_STD && CASSIE_SN_QUAT == SN_QUAT && CASSIE_SN_ORI_STD == SN_ORI_STD && CASSIE_SN_GYRO_BIAS == SN_GYRO_BIAS && CASSIE_SN_GYRO_STD == SN_GYRO_STD && CASSIE_SN_ACC_BIAS == SN_ACC_BIAS && CASSIE_SN_ACC_STD == SN_ACC_STD, "sensor row layout");
 static_assert(CASSIE_CON_WIDTH == CON_W && CASSIE_CON_MAX == MAXCON && CASSIE_CON_HEAD == CON_HEAD && CASSIE_CON_SLOT == CON_SLOT && CASSIE_CON_GEOM1 == CN_GEOM1 && CASSIE_CON_GEOM2 == CN_GEOM2 &&
               CASSIE_CON_DIM == CN_DIM && CASSIE_CON_DIST == CN_DIST && CASSIE_CON_POS == CN_POS && CASSIE_CON_FRAME == CN_FRAME && CASSIE_CON_FORCE == CN_FORCE && CASSIE_CON_MU == CN_MU &&
               CASSIE_CON_EFC == CN_EFC, "contact-list row layout");
@@ -2242,6 +2375,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "depth") || !strcmp(field, "camera_geom")) return b->impl->cam.k * b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "camera_env")) return b->impl->cam.k * CAMENV_SLOT; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "trace")) return b->impl->trace_width();
   if (!strcmp(field, "contacts")) return CON_W;
+  if (!strcmp(field, "sensors")) return SN_W; if (!strcmp(field, "sensor_rng")) return SR_W;
   if (!strcmp(field, "inv_qacc")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN; if (!strcmp(field, "inv")) return INV_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
 }
@@ -2706,6 +2840,13 @@ int cassie_batch_get_trace(cassie_batch_t *b, double *out) { return b->impl->get
 // contact lists of step and forward launches; see include/cassie_b200.h
 int cassie_batch_enable_contacts(cassie_batch_t *b, int on) { return b->impl->enable_contacts(on != 0) ? 0 : -1; }
 int cassie_batch_get_contacts(cassie_batch_t *b, double *out) { return b->impl->get_contacts(out) ? 0 : -1; }
+// sensor models drawn in the step kernel; see include/cassie_b200.h
+int cassie_batch_set_env_sensors(cassie_batch_t *b, const double *enc_offset, const double *enc_noise, const double *imu_quat, const double *imu_bias, const double *imu_noise, const unsigned char *mask) {
+  return b->impl->set_env_sensors(enc_offset, enc_noise, imu_quat, imu_bias, imu_noise, mask) ? 0 : -1; }
+int cassie_batch_get_env_sensors(cassie_batch_t *b, double *enc_offset, double *enc_noise, double *imu_quat, double *imu_bias, double *imu_noise) { return b->impl->get_env_sensors(enc_offset, enc_noise, imu_quat, imu_bias, imu_noise) ? 0 : -1; }
+int cassie_batch_clear_env_sensors(cassie_batch_t *b) { return b->impl->clear_env_sensors() ? 0 : -1; }
+int cassie_batch_seed_sensors(cassie_batch_t *b, unsigned long long seed, const unsigned char *mask) { return b->impl->seed_sensors(seed, mask) ? 0 : -1; }
+int cassie_batch_get_sensor_rng(cassie_batch_t *b, unsigned long long *seed, unsigned long long *counter) { return b->impl->get_sensor_rng(seed, counter) ? 0 : -1; }
 // names of the compiled model's objects (mj_name2id / mj_id2name for the kinds it keeps names of); see include/cassie_b200.h
 int cassie_batch_name2id(const cassie_batch_t *b, const char *type, const char *name) {
   const std::vector<std::string> *t = name_table(b->impl->hm, type, "cassie_batch_name2id");

@@ -41,6 +41,7 @@ constexpr int F_CT = 512; // per-environment contact softness: each contact row 
 constexpr int F_XF = 1024; // per-environment applied forces: xfrc_applied / qfrc_applied from an APPLIED_W row (plain F_BOX twins, and extended with F_BP | F_AC | F_MC | F_CT)
 constexpr int F_TC = 2048; // per-tick trace: every tick of a step launch stores the traced columns into a TRACE row slot (the F_XF chain twins' twins only)
 constexpr int F_CL = 4096; // contact lists: the last sub-step of a step / forward launch stores its contacts into a CON_W row (the F_FR chain twins' twins only)
+constexpr int F_SN = 8192; // sensor models: encoder offsets and noise, IMU mount, bias and noise from an SN_W row, drawn every tick (the F_XF twins' twins only)
 
 CASSIE_HD inline int pair_g1(uint32_t c) { return (int)(c & 63u); }
 CASSIE_HD inline int pair_g2(uint32_t c) { return (int)((c >> 6) & 63u); }
@@ -220,6 +221,14 @@ constexpr int TRACE_MAX = 64;   // columns
 constexpr int CON_HEAD = 8, CON_SLOT = 24, CON_W = CON_HEAD + MAXCON * CON_SLOT;
 constexpr int CN_GEOM1 = 0, CN_GEOM2 = 1, CN_DIM = 2, CN_DIST = 3, CN_POS = 4, CN_FRAME = 7, CN_FORCE = 16, CN_MU = 22, CN_EFC = 23;
 static_assert(CON_W == 296 && CON_HEAD % 4 == 0 && CON_SLOT % 4 == 0, "contact-list row layout");
+// sensor models (optional, cassie_batch_set_env_sensors; F_SN instances): per environment the offset and noise std of the 16 encoders in cassie_out order
+// (10 drives, then 6 joints; output radians), the IMU mount quaternion (w x y z, applied as q (x) q_m), and the orientation noise std (rad, a small rotation
+// on the right), the gyro bias and noise std, the accelerometer bias and noise std.  A model input like the CE rows.  The generator rows [n][SR_W] are int32:
+// the Philox key (seed lo, hi) and the tick counter (lo, hi), which step launches advance by their tick count; resets and snapshots leave both alone.
+constexpr int SN_W = 52;
+constexpr int SN_ENC_OFF = 0, SN_ENC_STD = 16, SN_QUAT = 32, SN_ORI_STD = 36, SN_GYRO_BIAS = 39, SN_GYRO_STD = 42, SN_ACC_BIAS = 45, SN_ACC_STD = 48;
+constexpr int SN_NCH = 25;   // noise channels: 16 encoders, orientation 3, gyro 3, accelerometer 3 (channel c: word c % 4 of Philox block c / 4)
+constexpr int SR_W = 4;
 
 // frames (optional, cassie_batch_set_frames): per environment a row [count][FRAME_W] describing named bodies / sites as the reference's queries see them
 // after mj_step / mj_forward (src/cassiemujoco.c:1242-1252, 1543-1553, 1752-1809): poses of the state the last sub-step started from, velocities and

@@ -34,6 +34,7 @@ template <typename real> struct EnvArrays {
                                               // dbg, cst and counters are scratch rows
   ContactListArgs<real> cl;                   // [n][CON_W] contact-list rows and the device-to-model geom ids [MGT] (F_CL instances); last, so that
                                               // the model block (DevModel, which with 16 warps fills the shared memory) does not grow
+  SensorArgs<real> sn;                        // [n][SN_W] sensor-model rows and [n][SR_W] generator rows (F_SN instances)
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -125,9 +126,11 @@ __global__ void __launch_bounds__(512) cassie_step_kernel(const DevModel<real> *
     if (FEAT & F_XF) E.env = env;   // and the applied-force rows, at the bias sum, the applied dof forces and the extra body's acceleration, from A.applied
     if (FEAT & F_TC) E.env = env;   // and the trace rows, after every tick, from A.trace
     if (FEAT & F_CL) E.env = env;   // and the contact-list rows, in the last sub-step, from A.cl
+    if (FEAT & F_SN) E.env = env;   // and the sensor-model and generator rows, at the controller stage, from A.sn
     step_env<real, INST == 1, FEAT, INST >= 1>(cm, sm, E, qvel, qacc_ws, xqvel, xqacc_ws, nticks, mode, (FEAT & F_BP) ? A.bpos : (const real *)0, (FEAT & F_AC) ? A.act : (const real *)0,
                                                (FEAT & F_MC) ? A.mech : (const real *)0, (FEAT & F_CT) ? A.contact : (const real *)0, (FEAT & F_XF) ? A.applied : (const real *)0,
-                                               (FEAT & F_TC) ? A.trace : TraceArgs<real>{}, (FEAT & F_CL) ? A.cl : ContactListArgs<real>{});
+                                               (FEAT & F_TC) ? A.trace : TraceArgs<real>{}, (FEAT & F_CL) ? A.cl : ContactListArgs<real>{},
+                                               (FEAT & F_SN) ? A.sn : SensorArgs<real>{});
     __syncwarp();
     if (mode >= 2) {   // query / set_const / frame Jacobian / dynamics / inverse: only the aux row / the constant row / the Jacobian row / the dynamics row / the inverse row is written
       if constexpr ((FEAT & F_FR) != 0) {   // from what mode 5's / mode 6's sub-step left in shared memory (mode 6: and in its scratch rows)

@@ -823,6 +823,44 @@ int cassie_batch_get_trace(cassie_batch_t *b, double *out);
 #define CASSIE_CON_EFC 23
 int cassie_batch_enable_contacts(cassie_batch_t *b, int on);
 int cassie_batch_get_contacts(cassie_batch_t *b, double *out);
+/* Sensor models, drawn in the step kernel: what the controller, the safety layer, the encoder filters and the estimator of every step tick measure.
+ * Each tick the controller stage takes last step's sensordata and measures:
+ *   encoder c (cassie_out order: 10 drives, then 6 joints)   true + offset[c] + n_c (output radians; a drive's motor-side value moves by gear times
+ *                                                            that), then the encoder's quantisation and filters as before
+ *   IMU orientation                                          q (x) q_m (x) normalise(1, (n_16, n_17, n_18) / 2)
+ *   gyro / accelerometer                                     R_m' v + bias + (n_19..21) / (n_22..24), clamped at the model's sensor cutoffs
+ *   magnetometer                                             R_m' m
+ * where q_m is the environment's IMU mount quaternion.  MuJoCo's sensordata (rows, aux, frames, rays, cameras) keeps the true values.  Noise: channel c
+ * takes 64-bit word c % 4 of the Philox-4x64-10 block with key (seed, 0) and counter (t, c / 4, 0, 0), t = the environment's counter + the tick of the
+ * launch; n = std * C * (u0 + u1 + u2 + u3 - 131070) over the word's four 16-bit parts, C = 1 / sqrt((65536^2 - 1) / 3): zero mean, unit variance
+ * times std, kurtosis 2.7, tails cut at 3.46 std (Irwin-Hall with four terms; integer operations and correctly rounded multiplies, so every build
+ * draws the same bits).  Step launches advance the counter by their tick count; other launches, resets, reset_where and snapshots leave it alone, so
+ * a new episode never replays old noise.  To replay a stretch, save and restore the counter (device rows "sensor_rng").
+ * set_env_sensors: enc_offset [n][16], enc_noise [n][16] (std), imu_quat [n][4] (w x y z, normalised on write), imu_bias [n][6] (gyro, accelerometer),
+ * imu_noise [n][9] (std of orientation in rad, gyro, accelerometer); NULL keeps a part, only masked environments change.  The first call allocates
+ * the zero model (zeros, identity mount; bitwise the batch without rows) and generator rows as seed_sensors(b, 0, NULL) seeds them.  A non-finite
+ * value, a negative std or a zero quaternion is refused with nothing changed, and the error names the environment, channel and field.  The rows are a
+ * model input: resets and snapshot restores leave them alone, cassie_sim_copy copies them and the generator rows, cassie_sim_step_pd_batch honours
+ * them.  A batch with rows runs the F_SN twins of the applied-force instances (carrying zero applied-force rows when it has none) and refuses a
+ * per-tick trace or contact lists, as they refuse it.  get: NULL parts are skipped; the zero model without rows.  clear: drops the rows, back to the
+ * instances that ran before.  seed_sensors: environment i gets key seed + i and counter 0 (masked environments only).  get_sensor_rng: key and
+ * counter [n] each.  Device rows: cassie_batch_device_ptr(b, "sensors") [n][CASSIE_SENSOR_WIDTH] in the batch precision, laid out as CASSIE_SN_*, and
+ * "sensor_rng" [n][4] int32 (key lo, hi, counter lo, hi); a write takes effect at the next launch.  0, or -1 (cassie_b200_last_error says why). */
+#define CASSIE_SENSOR_WIDTH 52
+#define CASSIE_SN_ENC_OFF 0
+#define CASSIE_SN_ENC_STD 16
+#define CASSIE_SN_QUAT 32
+#define CASSIE_SN_ORI_STD 36
+#define CASSIE_SN_GYRO_BIAS 39
+#define CASSIE_SN_GYRO_STD 42
+#define CASSIE_SN_ACC_BIAS 45
+#define CASSIE_SN_ACC_STD 48
+int cassie_batch_set_env_sensors(cassie_batch_t *b, const double *enc_offset, const double *enc_noise, const double *imu_quat, const double *imu_bias,
+                                 const double *imu_noise, const unsigned char *mask);
+int cassie_batch_get_env_sensors(cassie_batch_t *b, double *enc_offset, double *enc_noise, double *imu_quat, double *imu_bias, double *imu_noise);
+int cassie_batch_clear_env_sensors(cassie_batch_t *b);
+int cassie_batch_seed_sensors(cassie_batch_t *b, unsigned long long seed, const unsigned char *mask);
+int cassie_batch_get_sensor_rng(cassie_batch_t *b, unsigned long long *seed, unsigned long long *counter);
 /* Names of the compiled model's objects, as mj_name2id / mj_id2name give them (the reference's cassie_sim_mj_name2id, src/cassiemujoco.c:2194-2246):
  * type "body" (or "xbody"), "joint", "geom", "site" or "camera".  name2id: the id, or -1 for an unknown or empty name; id2name: the name, or NULL for
  * an id out of range or an unnamed object (the string lives as long as the batch).  Both return -1 / NULL with a recorded error for mj_name2id's other
