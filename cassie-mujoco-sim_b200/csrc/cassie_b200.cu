@@ -20,30 +20,15 @@
 #include "devbuild.h"
 #include "estimator_host.h"
 #include "step_kernel.cuh"
+#include "step_select.h"
 #include "raycast.inl"
 #include "camera_set.inl"
 #include "reset.inl"
 
-// the step-kernel instances live in their own translation units (step_inst.cu, one compilation per instance)
-#define CASSIE_STEP_ENTRY(tag) extern "C" const void *cassie_step_entry_##tag(void);
-CASSIE_STEP_ENTRY(f00) CASSIE_STEP_ENTRY(f10) CASSIE_STEP_ENTRY(f02) CASSIE_STEP_ENTRY(f12) CASSIE_STEP_ENTRY(f04) CASSIE_STEP_ENTRY(f14) CASSIE_STEP_ENTRY(f05) CASSIE_STEP_ENTRY(f15) CASSIE_STEP_ENTRY(f07) CASSIE_STEP_ENTRY(f17)
-CASSIE_STEP_ENTRY(d07) CASSIE_STEP_ENTRY(d17)
-CASSIE_STEP_ENTRY(f20) CASSIE_STEP_ENTRY(f22) CASSIE_STEP_ENTRY(f24) CASSIE_STEP_ENTRY(f25) CASSIE_STEP_ENTRY(f27) CASSIE_STEP_ENTRY(d27)
-CASSIE_STEP_ENTRY(f0c) CASSIE_STEP_ENTRY(f1c) CASSIE_STEP_ENTRY(f2c) CASSIE_STEP_ENTRY(f0f) CASSIE_STEP_ENTRY(f1f) CASSIE_STEP_ENTRY(f2f)
-CASSIE_STEP_ENTRY(d0f) CASSIE_STEP_ENTRY(d1f) CASSIE_STEP_ENTRY(d2f)
-CASSIE_STEP_ENTRY(f114) CASSIE_STEP_ENTRY(f117) CASSIE_STEP_ENTRY(d117) CASSIE_STEP_ENTRY(f11c) CASSIE_STEP_ENTRY(f11f) CASSIE_STEP_ENTRY(d11f)
-CASSIE_STEP_ENTRY(f02f) CASSIE_STEP_ENTRY(f12f) CASSIE_STEP_ENTRY(f22f) CASSIE_STEP_ENTRY(d02f) CASSIE_STEP_ENTRY(d12f) CASSIE_STEP_ENTRY(d22f) CASSIE_STEP_ENTRY(f13f) CASSIE_STEP_ENTRY(d13f)
-CASSIE_STEP_ENTRY(f144) CASSIE_STEP_ENTRY(f157) CASSIE_STEP_ENTRY(d157) CASSIE_STEP_ENTRY(f15f) CASSIE_STEP_ENTRY(d15f) CASSIE_STEP_ENTRY(f17f) CASSIE_STEP_ENTRY(d17f)
-CASSIE_STEP_ENTRY(f1c4) CASSIE_STEP_ENTRY(f1d7) CASSIE_STEP_ENTRY(d1d7) CASSIE_STEP_ENTRY(f1df) CASSIE_STEP_ENTRY(d1df) CASSIE_STEP_ENTRY(f1ff) CASSIE_STEP_ENTRY(d1ff)
-CASSIE_STEP_ENTRY(f11c4) CASSIE_STEP_ENTRY(f11d7) CASSIE_STEP_ENTRY(d11d7) CASSIE_STEP_ENTRY(f11df) CASSIE_STEP_ENTRY(d11df) CASSIE_STEP_ENTRY(f11ff) CASSIE_STEP_ENTRY(d11ff)
-CASSIE_STEP_ENTRY(f13c4) CASSIE_STEP_ENTRY(f13d7) CASSIE_STEP_ENTRY(d13d7) CASSIE_STEP_ENTRY(f13df) CASSIE_STEP_ENTRY(d13df) CASSIE_STEP_ENTRY(f13ff) CASSIE_STEP_ENTRY(d13ff)
-CASSIE_STEP_ENTRY(f0404) CASSIE_STEP_ENTRY(f2404)
-CASSIE_STEP_ENTRY(f17c4) CASSIE_STEP_ENTRY(f17d7) CASSIE_STEP_ENTRY(d17d7) CASSIE_STEP_ENTRY(f17df) CASSIE_STEP_ENTRY(d17df) CASSIE_STEP_ENTRY(f17ff) CASSIE_STEP_ENTRY(d17ff)
-CASSIE_STEP_ENTRY(f1fc4) CASSIE_STEP_ENTRY(f1fd7) CASSIE_STEP_ENTRY(d1fd7) CASSIE_STEP_ENTRY(f1fdf) CASSIE_STEP_ENTRY(d1fdf) CASSIE_STEP_ENTRY(f1fff) CASSIE_STEP_ENTRY(d1fff)
-CASSIE_STEP_ENTRY(f117d7) CASSIE_STEP_ENTRY(d117d7) CASSIE_STEP_ENTRY(f117df) CASSIE_STEP_ENTRY(d117df) CASSIE_STEP_ENTRY(f117ff) CASSIE_STEP_ENTRY(d117ff)
-CASSIE_STEP_ENTRY(f02404) CASSIE_STEP_ENTRY(f22404)
-CASSIE_STEP_ENTRY(f127c4) CASSIE_STEP_ENTRY(f127d7) CASSIE_STEP_ENTRY(d127d7) CASSIE_STEP_ENTRY(f127df) CASSIE_STEP_ENTRY(d127df) CASSIE_STEP_ENTRY(f127ff) CASSIE_STEP_ENTRY(d127ff)
-#undef CASSIE_STEP_ENTRY
+// the step-kernel instances live in their own translation units (step_inst.cu, one compilation per line of step_instances.inc)
+#define STEP_INSTANCE(tag) extern "C" const void *cassie_step_entry_##tag(void);
+#include "step_instances.inc"
+#undef STEP_INSTANCE
 
 namespace cassie {
 
@@ -52,122 +37,14 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 template <typename real> cudaError_t launch_camera_set(const CamSetArgs<real> &A, int device, cudaStream_t stream);   // camera_set.cu
 template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device, cudaStream_t stream);       // reset.cu
 
-// the instance for (precision, plain / extended, model features): the smallest compiled feature set that covers the model's
-template <typename real> static const void *step_entry(int inst, int feat, int *compiled_feat = nullptr) {   // inst: 0 plain, 1 extended, 2 plain + estimator
-  if (feat & F_SN) {   // sensor models: the F_SN twins of the F_XF instances, by their rule (a batch with sensor rows always has applied rows); none with a
-                       // trace or contact lists
-    if (feat & (F_TC | F_CL)) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (inst != 1) {   // null: the batch runs the extended kind (step_range)
-      if (dbl || (feat & ~(F_XF | F_SN)) != F_BOX) return nullptr;
-      if (compiled_feat) *compiled_feat = F_BOX | F_XF | F_SN;
-      return inst == 2 ? cassie_step_entry_f22404() : cassie_step_entry_f02404();
-    }
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN; return dbl ? cassie_step_entry_d127ff() : cassie_step_entry_f127ff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN; return dbl ? cassie_step_entry_d127df() : cassie_step_entry_f127df(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN; return cassie_step_entry_f127c4(); }
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_SN;
-    return dbl ? cassie_step_entry_d127d7() : cassie_step_entry_f127d7();
-  }
-  if (feat & F_CL) {   // contact lists: the F_CL twins of the F_FR chain twins (a batch with contact lists always has applied rows)
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_CL; return dbl ? cassie_step_entry_d117ff() : cassie_step_entry_f117ff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_CL; return dbl ? cassie_step_entry_d117df() : cassie_step_entry_f117df(); }
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_CL;
-    return dbl ? cassie_step_entry_d117d7() : cassie_step_entry_f117d7();
-  }
-  if (feat & F_TC) {   // per-tick traces: the F_TC twins of the F_XF chain twins, by their rule (a batch with a trace always has applied rows)
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC; return dbl ? cassie_step_entry_d1fff() : cassie_step_entry_f1fff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC; return dbl ? cassie_step_entry_d1fdf() : cassie_step_entry_f1fdf(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC; return cassie_step_entry_f1fc4(); }
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF | F_TC;
-    return dbl ? cassie_step_entry_d1fd7() : cassie_step_entry_f1fd7();
-  }
-  if (feat & F_XF) {   // per-environment applied forces: the plain twins of f04 / f24 where those would run, else the F_XF twins of the F_CT instances by their rule
-    const bool dbl = std::is_same<real, double>::value;
-    if (inst != 1) {   // null: the batch runs the extended kind (step_range)
-      if (dbl || (feat & ~F_XF) != F_BOX) return nullptr;
-      if (compiled_feat) *compiled_feat = F_BOX | F_XF;
-      return inst == 2 ? cassie_step_entry_f2404() : cassie_step_entry_f0404();
-    }
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF; return dbl ? cassie_step_entry_d17ff() : cassie_step_entry_f17ff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF; return dbl ? cassie_step_entry_d17df() : cassie_step_entry_f17df(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT | F_XF; return cassie_step_entry_f17c4(); }
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT | F_XF;
-    return dbl ? cassie_step_entry_d17d7() : cassie_step_entry_f17d7();
-  }
-  if (feat & F_CT) {   // per-environment contact softness: the F_CT twins of the F_MC instances, by the same rule (a batch with contact rows always has mechanics rows)
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC | F_CT; return dbl ? cassie_step_entry_d13ff() : cassie_step_entry_f13ff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC | F_CT; return dbl ? cassie_step_entry_d13df() : cassie_step_entry_f13df(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC | F_CT)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC | F_CT; return cassie_step_entry_f13c4(); }   // no frame / acceleration / dynamics / Jacobian launch
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC | F_CT;
-    return dbl ? cassie_step_entry_d13d7() : cassie_step_entry_f13d7();
-  }
-  if (feat & F_MC) {   // per-environment mechanics: the F_MC twins of the F_AC instances, by the same rule (a batch with mechanics rows always has actuator rows)
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC | F_MC; return dbl ? cassie_step_entry_d11ff() : cassie_step_entry_f11ff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC | F_MC; return dbl ? cassie_step_entry_d11df() : cassie_step_entry_f11df(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC | F_MC)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC | F_MC; return cassie_step_entry_f11c4(); }   // no frame / acceleration / dynamics / Jacobian launch
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC | F_MC;
-    return dbl ? cassie_step_entry_d11d7() : cassie_step_entry_f11d7();
-  }
-  if (feat & F_AC) {   // per-environment actuators: the F_AC twins of the F_BP instances, by the same rule (a batch with actuator rows always has offset rows)
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP | F_AC; return dbl ? cassie_step_entry_d1ff() : cassie_step_entry_f1ff(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP | F_AC; return dbl ? cassie_step_entry_d1df() : cassie_step_entry_f1df(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP | F_AC)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP | F_AC; return cassie_step_entry_f1c4(); }   // no frame / acceleration / dynamics / Jacobian launch
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP | F_AC;
-    return dbl ? cassie_step_entry_d1d7() : cassie_step_entry_f1d7();
-  }
-  if (feat & F_BP) {   // per-environment body offsets: extended instances only (a batch with offset rows always has constant rows)
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value;
-    if (feat & F_TR) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | F_FR | F_BP; return dbl ? cassie_step_entry_d17f() : cassie_step_entry_f17f(); }
-    if (feat & F_EG) { if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_FR | F_BP; return dbl ? cassie_step_entry_d15f() : cassie_step_entry_f15f(); }
-    if (!dbl && (feat & ~(F_BOX | F_BP)) == 0) { if (compiled_feat) *compiled_feat = F_BOX | F_BP; return cassie_step_entry_f144(); }   // no frame / acceleration / dynamics / Jacobian launch
-    if (compiled_feat) *compiled_feat = F_ALL | F_FR | F_BP;
-    return dbl ? cassie_step_entry_d157() : cassie_step_entry_f157();
-  }
-  if (feat & F_TR) {   // per-environment terrain (always with the per-environment static geoms): F_ALL | F_EG | F_TR, with or without frame rows
-    const bool dbl = std::is_same<real, double>::value, fr = (feat & F_FR) != 0;
-    if (compiled_feat) *compiled_feat = F_ALL | F_EG | F_TR | (fr ? F_FR : 0);
-    if (fr) { if (inst != 1) return nullptr; return dbl ? cassie_step_entry_d13f() : cassie_step_entry_f13f(); }
-    if (dbl) return inst == 1 ? cassie_step_entry_d12f() : (inst == 2 ? cassie_step_entry_d22f() : cassie_step_entry_d02f());
-    return inst == 1 ? cassie_step_entry_f12f() : (inst == 2 ? cassie_step_entry_f22f() : cassie_step_entry_f02f());
-  }
-  if (feat & F_FR) {   // frame rows: extended instances only; F_BOX covers models with at most boxes, F_ALL the rest, each with or without F_EG
-    if (inst != 1) return nullptr;
-    const bool dbl = std::is_same<real, double>::value, eg = (feat & F_EG) != 0, box = !dbl && (feat & ~(F_BOX | F_EG | F_FR)) == 0;
-    if (compiled_feat) *compiled_feat = (box ? F_BOX : F_ALL) | F_FR | (eg ? F_EG : 0);
-    if (dbl) return eg ? cassie_step_entry_d11f() : cassie_step_entry_d117();
-    if (box) return eg ? cassie_step_entry_f11c() : cassie_step_entry_f114();
-    return eg ? cassie_step_entry_f11f() : cassie_step_entry_f117();
-  }
-  if (feat & F_EG) {   // per-environment static-geom rows: F_BOX | F_EG covers models with at most boxes (a floor without boxes too), F_ALL | F_EG the rest
-    const bool box = !std::is_same<real, double>::value && (feat & ~(F_BOX | F_EG)) == 0;
-    if (compiled_feat) *compiled_feat = box ? (F_BOX | F_EG) : (F_ALL | F_EG);
-    if (std::is_same<real, double>::value) return inst == 1 ? cassie_step_entry_d1f() : (inst == 2 ? cassie_step_entry_d2f() : cassie_step_entry_d0f());
-    if (box) return inst == 1 ? cassie_step_entry_f1c() : (inst == 2 ? cassie_step_entry_f2c() : cassie_step_entry_f0c());
-    return inst == 1 ? cassie_step_entry_f1f() : (inst == 2 ? cassie_step_entry_f2f() : cassie_step_entry_f0f());
-  }
-  int f = F_ALL;
-  if (!std::is_same<real, double>::value) { if (feat == 0) f = 0; else if (feat == F_HFIELD) f = F_HFIELD; else if (feat == F_BOX) f = F_BOX; else if ((feat & ~(F_XB | F_BOX)) == 0) f = F_XB | F_BOX; }
-  if (compiled_feat) *compiled_feat = f;
-  if (std::is_same<real, double>::value) return inst == 1 ? cassie_step_entry_d17() : (inst == 2 ? cassie_step_entry_d27() : cassie_step_entry_d07());
-  switch (f) {
-    case 0: return inst == 1 ? cassie_step_entry_f10() : (inst == 2 ? cassie_step_entry_f20() : cassie_step_entry_f00());
-    case F_HFIELD: return inst == 1 ? cassie_step_entry_f12() : (inst == 2 ? cassie_step_entry_f22() : cassie_step_entry_f02());
-    case F_BOX: return inst == 1 ? cassie_step_entry_f14() : (inst == 2 ? cassie_step_entry_f24() : cassie_step_entry_f04());
-    case F_XB | F_BOX: return inst == 1 ? cassie_step_entry_f15() : (inst == 2 ? cassie_step_entry_f25() : cassie_step_entry_f05());
-    default: return inst == 1 ? cassie_step_entry_f17() : (inst == 2 ? cassie_step_entry_f27() : cassie_step_entry_f07());
-  }
+static constexpr StepInstance STEP_INSTANCES[] = {
+#define STEP_INSTANCE(tag) step_instance(#tag, cassie_step_entry_##tag),
+#include "step_instances.inc"
+#undef STEP_INSTANCE
+};
+
+template <typename real> static StepChoice select_step(int kind, int feat) {
+  return step_select(STEP_INSTANCES, (int)(sizeof STEP_INSTANCES / sizeof STEP_INSTANCES[0]), std::is_same<real, double>::value, kind, feat);
 }
 
 // cassie_sim_centroid_inertia (src/cassiemujoco.c:1647-1687) from one dynamics row: m = M[0][0], I_p = M[3:6, 3:6], r = the row's centre-of-mass offset
@@ -591,28 +468,13 @@ template <typename real> struct Batch : BatchBase {
       }
       cfg[ext].wpb = k_sel; cfg[ext].smem = model_bytes<real>() + (size_t)k_sel * wb;
       int per_sm = 0;
-      { const void *entry = step_entry<real>(ext, feat);
-        CUDA_OK(raise_smem_limit(entry, (int)cfg[ext].smem));
-        CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_EG), (int)cfg[ext].smem));   // same scratch, same shape
-        if (ext == 1) for (int fe : {feat | F_FR, feat | F_EG | F_FR}) CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe), (int)cfg[ext].smem));
-        if (hm.nhfield == 1) {   // per-environment terrain: F_ALL | F_EG | F_TR (the scratch of F_ALL)
-          CUDA_OK(raise_smem_limit(step_entry<real>(ext, F_ALL | F_EG | F_TR), (int)cfg[ext].smem));
-          if (ext == 1) CUDA_OK(raise_smem_limit(step_entry<real>(ext, F_ALL | F_EG | F_TR | F_FR), (int)cfg[ext].smem)); }
-        if (ext == 1)   // per-environment body offsets: every instance step_entry routes F_BP launches to (the extended scratch)
-          for (int fe : {feat | F_BP, feat | F_BP | F_FR, feat | F_EG | F_BP, F_ALL | F_EG | F_TR | F_BP}) {   // and their F_AC twins (per-environment actuators)
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe), (int)cfg[ext].smem));
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC), (int)cfg[ext].smem));
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC), (int)cfg[ext].smem));   // and their F_MC twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT), (int)cfg[ext].smem));   // and their F_CT twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF), (int)cfg[ext].smem));   // and their F_XF twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_TC), (int)cfg[ext].smem));   // and their F_TC twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_CL), (int)cfg[ext].smem));   // and their F_CL twins
-            CUDA_OK(raise_smem_limit(step_entry<real>(ext, fe | F_AC | F_MC | F_CT | F_XF | F_SN), (int)cfg[ext].smem)); }   // and their F_SN twins
-        if (ext != 1 && step_entry<real>(ext, feat | F_XF))   // the plain F_XF twins (applied forces), where this model runs f04 / f24
-          CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF), (int)cfg[ext].smem));
-        if (ext != 1 && step_entry<real>(ext, feat | F_XF | F_SN))   // and their F_SN twins (sensor models)
-          CUDA_OK(raise_smem_limit(step_entry<real>(ext, feat | F_XF | F_SN), (int)cfg[ext].smem));
-        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, entry, 32 * k_sel, cfg[ext].smem)); }
+      // every instance a launch of this kind can run for this model (the same scratch, the same shape): the one picked for the model's features
+      // plus the optional features of each instance of the kind
+      for (const StepInstance &si : STEP_INSTANCES) if (si.dbl == std::is_same<real, double>::value && si.kind == ext) {
+        const StepChoice s = select_step<real>(ext, feat | (si.feat & ~F_ALL));
+        if (s.kind == ext && s.index >= 0) CUDA_OK(raise_smem_limit(STEP_INSTANCES[s.index].entry(), (int)cfg[ext].smem));
+      }
+      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, STEP_INSTANCES[select_step<real>(ext, feat).index].entry(), 32 * k_sel, cfg[ext].smem));
       cfg[ext].resident_ctas = per_sm * sms < 1 ? 1 : per_sm * sms;
     }
     wpb = cfg[0].wpb;
@@ -2157,14 +2019,18 @@ template <typename real> struct Batch : BatchBase {
     return true;
   }
   bool step(int nticks, int mode) override { return step_range(nticks, mode, 0, n, stream); }
+  // the features a launch of `mode` asks for (devmodel.h F_*): the model's and one per kind of per-environment rows the batch holds; frame,
+  // acceleration, dynamics and inverse rows: an F_FR instance (set_const launches too: they write no frames)
+  int launch_feat(int mode) const {
+    return (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) |
+           (A.trace.rows ? F_TC : 0) | (A.cl.rows ? F_CL : 0) | (A.sn.rows ? F_SN : 0) | ((A.frames || A.acc || A.cl.rows || mode == 5 || mode == 6) ? F_FR : 0);
+  }
   // the instance kind a launch of `mode` runs: 0 plain, 1 extended, 2 plain + estimator
   int launch_kind(int mode) {
     // per-environment model constants / derived-quantity rows / task-space PD / set_const: extended instance (its own scratch size and launch shape);
     // the in-kernel estimator alone: the plain instance with the estimator stage
-    int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || A.trace.rows || A.cl.rows || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
-    // applied forces: a plain twin where f04 / f24 would run, else the chain twin
-    if (A.applied && ext != 1 && !step_entry<real>(ext, feat | (A.genv ? F_EG : 0) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | F_XF | (A.sn.rows ? F_SN : 0))) ext = 1;
-    return ext;
+    const int ext = (A.cenv || A.aux || A.task || A.frames || A.acc || A.trace.rows || A.cl.rows || (A.dbg && !DBG_IN_ALL_INSTANCES) || mode >= 3) ? 1 : (A.est ? 2 : 0);   // debug batches: the stage dumps live in the extended instance
+    return select_step<real>(ext, launch_feat(mode)).kind;   // applied forces: a plain twin where f04 / f24 would run, else the extended kind
   }
   bool step_range(int nticks, int mode, int env0, int count, cudaStream_t on) {   // the launch covers environments [env0, env0 + count)
     CUDA_OK(cudaSetDevice(device));
@@ -2185,9 +2051,10 @@ template <typename real> struct Batch : BatchBase {
     // mode 6: the caller's qacc reaches the lanes through the warm-start load (mode 6 writes no state back); the forward's stage dump, sensor data and
     // counters go to the launch's scratch rows, for inverse_row; no aux or frame rows
     if (mode == 6) { La.qacc_ws = d_iq; La.dbg = d_idbg; La.cst = d_icst; La.counters = d_icnt; La.aux = nullptr; La.nfr = 0; }
-    const int lf = (A.genv ? feat | F_EG : feat) | (A.terrain ? F_TR : 0) | (A.bpos ? F_BP : 0) | (A.act ? F_AC : 0) | (A.mech ? F_MC : 0) | (A.contact ? F_CT : 0) | (A.applied ? F_XF : 0) | (A.trace.rows ? F_TC : 0) | (A.cl.rows ? F_CL : 0) | (A.sn.rows ? F_SN : 0) | ((A.frames || A.acc || A.cl.rows || mode == 5 || mode == 6) ? F_FR : 0);   // frame, acceleration, dynamics and inverse rows: the extended F_FR instance (set_const launches too: they write no frames)
+    const StepChoice inst = select_step<real>(ext, launch_feat(mode));   // with the rows provisioned above
+    if (inst.kind != ext || inst.index < 0) { set_err("no step-kernel instance is compiled for this batch's rows"); return false; }
     { const DevModel<real> *dm = d_model; void *args[4] = {(void *)&dm, (void *)&La, (void *)&nticks, (void *)&mode};
-      CUDA_OK(cudaLaunchKernel(step_entry<real>(ext, lf), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
+      CUDA_OK(cudaLaunchKernel(STEP_INSTANCES[inst.index].entry(), dim3(grid), dim3(32 * c.wpb), args, c.smem, on)); }
     launches++;
     if (mode == 0 && A.trace.rows) tc_ticks = nticks < A.trace.T ? nticks : A.trace.T;
     CUDA_OK(cudaGetLastError());
