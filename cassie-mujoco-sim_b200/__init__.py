@@ -1315,6 +1315,31 @@ class CassieBatch:
         if L.cassie_batch_forward_where(self.h, C.c_void_p(self._mask_ptr(mask, 'mask'))) != 0:
             raise RuntimeError(_last_error())
 
+    # ---- loop closure: qpos and qvel projected onto the legs' connect equalities (rules in include/cassie_b200.h, DESIGN.md section 3)
+    LOOP_TOL = {FP64: 1e-12, FP32: 1e-6}   # metres: fp32 kinematics reaches ~5e-7 at best, so 1e-6 converges in 2-4 steps from 0.05 rad of noise
+
+    def close_loops(self, mask=None, max_iter=20, tol=None):
+        """close the loops of the environments with mask[e] set (CUDA bool / uint8 tensor [n]; None: every environment): the rod, tarsus, crank and
+        plantar-rod coordinates are moved until max |p1 - p2| <= tol (None: LOOP_TOL of the precision) or max_iter damped Gauss-Newton steps, and their
+        velocities projected so that J qvel ~ 0; everything else is held bitwise.  An environment that does not converge keeps qpos and qvel.  One
+        launch on the batch's stream, capturable in a CUDA graph after the first call (which allocates the status rows), with reset_where's stream
+        rule.  It writes qpos, qvel and loop_status() only: follow it with forward_where(mask) to refresh the observation, sensors and frames"""
+        L = self.L
+        L.cassie_batch_close_loops.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double]
+        mp = None if mask is None else C.c_void_p(self._mask_ptr(mask, 'mask'))
+        if L.cassie_batch_close_loops(self.h, mp, int(max_iter), float(self.LOOP_TOL[self.precision] if tol is None else tol)) != 0:
+            raise RuntimeError(_last_error())
+
+    def loop_status(self):
+        """the status rows of the last close_loops, as numpy arrays [n]: residual (max |p1 - p2| in metres after the launch; for a failure, that of the
+        unchanged pose), iterations (0: already closed, -1: not converged) and vel_residual (max |J qvel| after the launch); environments outside the
+        last mask keep the values of their last selection (zero before it)"""
+        out = dict(residual=np.zeros(self.n), iterations=np.zeros(self.n, dtype=np.int32), vel_residual=np.zeros(self.n))
+        self.L.cassie_batch_get_loop_status.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_double)]
+        if self.L.cassie_batch_get_loop_status(self.h, self._dp(out['residual']), out['iterations'].ctypes.data_as(C.POINTER(C.c_int)), self._dp(out['vel_residual'])) != 0:
+            raise RuntimeError(_last_error())
+        return out
+
     def set_timestep(self, dt):
         self.L.cassie_batch_set_timestep.argtypes = [C.c_void_p, C.c_double]
         if self.L.cassie_batch_set_timestep(self.h, float(dt)) != 0:
@@ -1358,7 +1383,8 @@ class CassieBatch:
         lists of the last step / forward launch, a header and CON_MAX slots laid out as CON; enable_contacts first; camera_env [n, k, CAMENV_SLOT]: the
         per-environment camera mounts pos[3], quat[4], fovy in degrees, read at the next render; set_env_cameras first; camera_geom [n, k, height, width]
         int32 (shaped as depth for set_camera): the geom ids of the last render; enable_camera_geoms and render_depth first; sensors [n, 52] laid out as
-        SN, read at the next launch; sensor_rng [n, 4] int32: key lo, hi, counter lo, hi; set_env_sensors first for both).  set_frames /
+        SN, read at the next launch; sensor_rng [n, 4] int32: key lo, hi, counter lo, hi; set_env_sensors first for both; loops [n, 4]: the status
+        rows of close_loops -- residual, iterations, max |J qvel|, pad; close_loops first).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -1368,7 +1394,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first; sensors, sensor_rng: set_env_sensors first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first; sensors, sensor_rng: set_env_sensors first; loops: close_loops first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field in ('terrain', 'camera_geom', 'sensor_rng'):
             ts = '<i4'

@@ -24,6 +24,7 @@
 #include "raycast.inl"
 #include "camera_set.inl"
 #include "reset.inl"
+#include "loops.inl"
 
 // the step-kernel instances live in their own translation units (step_inst.cu, one compilation per line of step_instances.inc)
 #define STEP_INSTANCE(tag) extern "C" const void *cassie_step_entry_##tag(void);
@@ -36,6 +37,7 @@ template <typename real> cudaError_t launch_raycast(const RayArgs<real> &A, int 
 template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int device, cudaStream_t stream);   // camera.cu
 template <typename real> cudaError_t launch_camera_set(const CamSetArgs<real> &A, int device, cudaStream_t stream);   // camera_set.cu
 template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device, cudaStream_t stream);       // reset.cu
+template <typename real> cudaError_t launch_loops(const LoopArgs<real> &A, int device, cudaStream_t stream);   // loops.cu
 
 static constexpr StepInstance STEP_INSTANCES[] = {
 #define STEP_INSTANCE(tag) step_instance(#tag, cassie_step_entry_##tag),
@@ -251,6 +253,10 @@ struct BatchBase {
   // device-masked restore from the bank and device-masked mj_forward: enqueued on the batch's stream, no host synchronisation, copy or allocation
   virtual bool reset_where(const void *d_mask, const void *d_entry) = 0;
   virtual bool forward_where(const void *d_mask) = 0;
+  // loop closure (loops.inl): the selected environments' qpos and qvel projected onto the connect equalities, one launch on the batch's stream; the
+  // first call allocates the status rows [n][LOOP_SLOT].  get_loop_status copies them; any pointer may be null
+  virtual bool close_loops(const void *d_mask, int max_iter, double tol) = 0;
+  virtual bool get_loop_status(double *residual, int *iterations, double *vel_residual) = 0;
   bool legacy = false;   // the batch of a cassie_sim_t: its host mirrors are pushed before every launch, so device-side resets are refused
   virtual bool copy_model_from(BatchBase *src) = 0;     // per-environment constants, height fields, timestep (mj_copyModel in cassie_sim_copy, :1083-1091)
   virtual bool rebuild_model() = 0;                     // after hm was edited (timestep, hold / release): rebuild and upload the constant block
@@ -405,10 +411,11 @@ template <typename real> struct Batch : BatchBase {
                                            // written them since
   int tc_ticks = 0;                        // slots the last step launch wrote into the trace rows (A.trace: [n][T][k], allocated by cassie_batch_set_trace)
   Snap *bank = nullptr;                    // the reset bank (cassie_batch_set_reset_bank): a snapshot of k entries
+  real *d_loops = nullptr;                 // [n][LOOP_SLOT] status rows of cassie_batch_close_loops, allocated (zero) by its first call
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
+    cudaFree(d_loops); cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -870,6 +877,36 @@ template <typename real> struct Batch : BatchBase {
       set_err(std::string(verb) + ": this batch gets model-valued contact rows at its first extended launch; run cassie_batch_step or cassie_batch_forward once first"); return false; }
     A.mask = (const unsigned char *)d_mask; const bool ok = step(0, 1); A.mask = nullptr;
     return ok;
+  }
+  bool close_loops(const void *d_mask, int max_iter, double tol) override {
+    const std::string verb = "cassie_batch_close_loops";
+    if (d_mask && !device_rows(d_mask, verb.c_str(), "the mask")) return false;
+    if (max_iter < 1 || max_iter > LOOP_MAX_ITER) { set_err(verb + ": max_iter must be between 1 and " + std::to_string(LOOP_MAX_ITER)); return false; }
+    if (!(tol > 0) || !std::isfinite(tol)) { set_err(verb + ": tol must be finite and > 0"); return false; }
+    if (legacy) { set_err(verb + ": the batch belongs to a cassie_sim_t, whose host mirrors would overwrite the closed state"); return false; }
+    LoopArgs<real> L; std::string err;
+    if (!loop_table(hm, L.T, err)) { set_err(verb + ": " + err); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    if (!d_loops) { CUDA_OK(cudaMalloc(&d_loops, sizeof(real) * n * LOOP_SLOT)); CUDA_OK(cudaMemsetAsync(d_loops, 0, sizeof(real) * n * LOOP_SLOT, stream)); }
+    if (L.T.nrow == 0) return true;   // no connect equality: nothing to close
+    L.model = d_model; L.qpos = A.qpos; L.qpos_w = QW; L.qvel = A.qvel; L.qvel_w = VW; L.bpos = d_bpos; L.status = d_loops;
+    L.mask = (const unsigned char *)d_mask; L.n = n; L.max_iter = max_iter; L.tol = (real)tol;
+    CUDA_OK(launch_loops<real>(L, device, stream));
+    launches++;
+    return true;
+  }
+  bool get_loop_status(double *residual, int *iterations, double *vel_residual) override {
+    if (!d_loops) { set_err("cassie_batch_get_loop_status: no cassie_batch_close_loops call yet"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    h_tmp.resize((size_t)n * LOOP_SLOT);
+    CUDA_OK(cudaMemcpyAsync(h_tmp.data(), d_loops, sizeof(real) * n * LOOP_SLOT, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    for (int e = 0; e < n; e++) {
+      const real *r = &h_tmp[(size_t)e * LOOP_SLOT];
+      if (residual) residual[e] = (double)r[0];
+      if (iterations) iterations[e] = (int)r[1];
+      if (vel_residual) vel_residual[e] = (double)r[2];
+    }
+    return true;
   }
   bool rebuild_model() override {
     CUDA_OK(cudaSetDevice(device));
@@ -2122,7 +2159,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "camera_env")) return d_camenv; if (!strcmp(f, "camera_geom")) return d_camgeom; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
-    if (!strcmp(f, "applied")) return d_app;
+    if (!strcmp(f, "applied")) return d_app; if (!strcmp(f, "loops")) return d_loops;
     if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
     if (!strcmp(f, "contacts")) return A.cl.rows;
@@ -2158,6 +2195,7 @@ static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == 
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
 static_assert(CASSIE_INV_WIDTH == INV_W && CASSIE_INV_COLS == IV_COLS && CASSIE_INV_QFRC == IV_QFRC && CASSIE_INV_QFRCC == IV_QFRCC && CASSIE_INV_NEFC == IV_NEFC && CASSIE_INV_NCON == IV_NCON && CASSIE_INV_DROPPED == IV_DROPPED, "inverse row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
+static_assert(CASSIE_LOOP_SLOT == LOOP_SLOT && CASSIE_LOOP_MAX_ITER == LOOP_MAX_ITER && CASSIE_LOOP_RESIDUAL == 0 && CASSIE_LOOP_ITERATIONS == 1 && CASSIE_LOOP_VEL_RESIDUAL == 2, "loop status rows");
 static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
 static_assert(CASSIE_SENSOR_WIDTH == SN_W && CASSIE_SN_ENC_OFF == SN_ENC_OFF && CASSIE_SN_ENC_STD == SN_ENC_STD && CASSIE_SN_QUAT == SN_QUAT && CASSIE_SN_ORI_STD == SN_ORI_STD && CASSIE_SN_GYRO_BIAS == SN_GYRO_BIAS && CASSIE_SN_GYRO_STD == SN_GYRO_STD && CASSIE_SN_ACC_BIAS == SN_ACC_BIAS && CASSIE_SN_ACC_STD == SN_ACC_STD, "sensor row layout");
 static_assert(CASSIE_CON_WIDTH == CON_W && CASSIE_CON_MAX == MAXCON && CASSIE_CON_HEAD == CON_HEAD && CASSIE_CON_SLOT == CON_SLOT && CASSIE_CON_GEOM1 == CN_GEOM1 && CASSIE_CON_GEOM2 == CN_GEOM2 &&
@@ -2241,7 +2279,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
   if (!strcmp(field, "depth") || !strcmp(field, "camera_geom")) return b->impl->cam.k * b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "camera_env")) return b->impl->cam.k * CAMENV_SLOT; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "trace")) return b->impl->trace_width();
-  if (!strcmp(field, "contacts")) return CON_W;
+  if (!strcmp(field, "contacts")) return CON_W; if (!strcmp(field, "loops")) return LOOP_SLOT;
   if (!strcmp(field, "sensors")) return SN_W; if (!strcmp(field, "sensor_rng")) return SR_W;
   if (!strcmp(field, "inv_qacc")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN; if (!strcmp(field, "inv")) return INV_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
@@ -2911,6 +2949,8 @@ int cassie_batch_set_state(cassie_batch_t *b, const void *state, const unsigned 
 int cassie_batch_set_reset_bank(cassie_batch_t *b, const void *state, const int *envs, int k) { return b->impl->set_reset_bank((const Snap *)state, envs, k) ? 0 : -1; }
 int cassie_batch_reset_bank_size(const cassie_batch_t *b) { return b->impl->reset_bank_size(); }
 int cassie_batch_reset_where(cassie_batch_t *b, const void *d_mask, const void *d_entry) { return b->impl->reset_where(d_mask, d_entry) ? 0 : -1; }
+int cassie_batch_close_loops(cassie_batch_t *b, const void *d_mask, int max_iter, double tol) { return b->impl->close_loops(d_mask, max_iter, tol) ? 0 : -1; }
+int cassie_batch_get_loop_status(cassie_batch_t *b, double *residual, int *iterations, double *vel_residual) { return b->impl->get_loop_status(residual, iterations, vel_residual) ? 0 : -1; }
 int cassie_batch_forward_where(cassie_batch_t *b, const void *d_mask) { return b->impl->forward_where(d_mask) ? 0 : -1; }
 #include "legacy_stubs.inc"
 }  // extern "C"

@@ -606,6 +606,44 @@ int cassie_batch_set_reset_bank(cassie_batch_t *b, const void *state, const int 
 int cassie_batch_reset_bank_size(const cassie_batch_t *b);
 int cassie_batch_reset_where(cassie_batch_t *b, const void *d_mask, const void *d_entry);
 int cassie_batch_forward_where(cassie_batch_t *b, const void *d_mask);
+/* Loop closure (new): each selected environment's qpos and qvel projected onto the model's connect equalities, for start states that did not come from
+ * the simulator (noise on qpos, retargeted motions, poses from motor angles, body offsets inside a loop), which would otherwise start with open loops that
+ * the constraint rows pull shut over the first ticks.
+ *
+ * Loop-closure rules that are ours:
+ * - Equations: every connect equality, with MuJoCo's definition p1 = xpos[b1] + xmat[b1] eq_data[0..2], p2 = xpos[b2] + xmat[b2] eq_data[3..5], residual
+ *   r = p1 - p2 (4 x 3 rows for the Cassie models).  A model without connect equalities makes the call a no-op that returns 0.
+ * - Free coordinates: every main-tree joint that is not on the root body (the root body's joints -- a free joint, or the pelvis's three slides and ball
+ *   -- place the tree in the world), drives no actuator and has zero jnt_stiffness in the model table.  For the Cassie models: the achilles-rod ball,
+ *   tarsus, foot crank and plantar rod of each leg.  Every other coordinate (pelvis, motors including the foot, shin and heel springs, the extra free
+ *   body) is held bitwise.
+ * - Positions: the free ball joints' quaternions are normalised, then damped Gauss-Newton steps dq_f = -J_f' (J_f J_f' + lambda I)^-1 r run, J_f being the
+ *   translational Jacobian difference of the anchor points in the free columns; a ball joint turns by its step through the step integrator's quaternion
+ *   update.  They stop when max |r| <= tol or after max_iter steps.  lambda = 1e-10 m^2 in fp64, 1e-6 m^2 in fp32: the rows of a planar loop (a Cassie
+ *   leg's plantar-rod loop) are rank-deficient, so J_f J_f' is singular; lambda sits above its rounding and far below its smallest non-zero eigenvalue
+ *   (~1.2e-3 m^2 for Cassie).
+ * - Velocities, at the closed pose: qvel_f <- qvel_f - J_f' (J_f J_f' + lambda I)^-1 (J qvel), so that J qvel ~ 0 (up to lambda / 1.2e-3 of it in the
+ *   weakest direction); held velocities are unchanged.
+ * - Per-environment body offsets (cassie_batch_set_env_body_pos) move the anchors and are honoured; no other per-environment row enters.
+ * - An environment that is not within tol after max_iter steps keeps its qpos and qvel bitwise and reports -1 iterations; one already within tol keeps
+ *   its qpos bitwise (0 iterations) and still has its velocity projected.  Unselected environments, their status rows included, are not touched.
+ * - The launch writes qpos, qvel and the status rows only: follow it with cassie_batch_forward_where(mask) to refresh sensordata, aux, frames and the
+ *   observation, as after cassie_batch_reset_where plus noise.
+ *
+ * cassie_batch_close_loops: d_mask is device uint8[n] (a torch.bool tensor as it is), NULL for every environment.  One launch on the batch's stream: no
+ * host synchronisation, copy or allocation, so it can be captured in a CUDA graph -- except the first call, which allocates and zeroes the status rows
+ * (make it before a capture).  -1, with nothing enqueued, for a mask that is not device or managed memory of the batch's device, max_iter outside
+ * 1..CASSIE_LOOP_MAX_ITER, a tol that is not finite and > 0, a connect equality on the extra free body, or the batch of a cassie_sim_t.
+ * cassie_batch_device_ptr(b, "loops"): the status rows [n][CASSIE_LOOP_SLOT] in the batch precision: the residual max |p1 - p2| after the launch (metres;
+ * for a failure, that of the unchanged pose), the iterations used (0: already closed, -1: not converged), max |J qvel| after the launch, a pad.
+ * cassie_batch_get_loop_status: their synchronous host copy, [n] each; any pointer may be NULL.  -1 before the first cassie_batch_close_loops. */
+#define CASSIE_LOOP_SLOT 4
+#define CASSIE_LOOP_MAX_ITER 200
+#define CASSIE_LOOP_RESIDUAL 0
+#define CASSIE_LOOP_ITERATIONS 1
+#define CASSIE_LOOP_VEL_RESIDUAL 2
+int cassie_batch_close_loops(cassie_batch_t *b, const void *d_mask, int max_iter, double tol);
+int cassie_batch_get_loop_status(cassie_batch_t *b, double *residual, int *iterations, double *vel_residual);
 /* batched cassie_sim_apply_force / cassie_sim_clear_forces: xfrc [n][6]; one (wrench, body) slot per env, added to the applied-force rows
  * (cassie_batch_set_applied_forces) when the batch has them; clear_forces empties the slot and zeroes the rows' xfrc_applied, keeping qfrc_applied */
 int cassie_batch_apply_force(cassie_batch_t *b, const double *xfrc, const char *body_name);
