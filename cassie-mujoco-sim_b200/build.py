@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, '_obj')
 LIB = os.path.join(HERE, 'libcassie_b200.so')
 DEPS = [os.path.join(CSRC, f) for f in ('cassie_b200.cu', 'mjcf.cpp', 'step_inst.cu', 'step_kernel.cuh', 'step_core.inl', 'cassie_tree_gen.inc', 'devmodel.h', 'devbuild.h', 'model.h',
-                                        'estimator_host.h', 'legacy_stubs.inc', 'step_instances.inc', 'step_select.h', 'raycast.cu', 'raycast.inl', 'camera.cu', 'camera.inl', 'camera_set.cu', 'camera_set.inl', 'reset.cu', 'reset.inl', 'loops.cu', 'loops.inl')] + [
+                                        'estimator_host.h', 'legacy_stubs.inc', 'step_instances.inc', 'step_select.h', 'env_rows.h', 'raycast.cu', 'raycast.inl', 'camera.cu', 'camera.inl', 'camera_set.cu', 'camera_set.inl', 'reset.cu', 'reset.inl', 'loops.cu', 'loops.inl')] + [
     os.path.join(HERE, '..', 'include', 'cassie_b200.h'), os.path.join(HERE, '..', 'include', 'cassie_bus.h')]
 # (tag, real, kind: 0 plain / 1 extended / 2 plain + estimator, feature bits csrc/devmodel.h F_*) of every step instance, from the tags of
 # csrc/step_instances.inc: <f|d><kind digit><feature bits in hex>

@@ -21,6 +21,7 @@
 #include "estimator_host.h"
 #include "step_kernel.cuh"
 #include "step_select.h"
+#include "env_rows.h"
 #include "raycast.inl"
 #include "camera_set.inl"
 #include "reset.inl"
@@ -393,31 +394,22 @@ template <typename real> struct Batch : BatchBase {
   std::vector<double> ge_host[MGS];        // per static slot touched by a per-environment placement: [n][10] pos 3, quat 4, size 3 in the geom's body frame
   int *d_terrain = nullptr;                // A.terrain: [n] per-environment bank entries, allocated by the first per-environment terrain (F_TR instances)
   std::vector<double> hf_host;             // [n][7] height-field position (in its body frame) 3, size 4 per environment; empty: the shared ones
-  real *d_bpos = nullptr;                  // A.bpos: [n][BP_W] per-environment body offsets, allocated by the first cassie_batch_set_env_body_pos (F_BP instances)
-  std::vector<double> bp_host;             // [n][nbody][3] the offsets every environment sees while d_bpos exists (in double: what get returns)
-  bool bp_cenv = false;                    // the constant rows were allocated by the body-offset setter, and no model-row setter has written them since
-  real *d_act = nullptr;                   // A.act: [n][ACT_W] per-environment actuators, allocated by the first cassie_batch_set_env_actuators (F_AC instances)
-  std::vector<double> ac_host;             // [n][nu][4] lo, hi, rpm, delay every environment sees while d_act exists (in double: what get returns)
-  bool ac_bpos = false;                    // the offset rows were allocated by the actuator setter (model values), and no body-offset call has written them since
-  real *d_mech = nullptr;                  // A.mech: [n][MECH_W] per-environment mechanics, allocated by the first cassie_batch_set_env_mechanics (F_MC instances)
-  std::vector<double> mc_host;             // [n][mech_host_w()] inertia, armature, stiffness, springref every environment sees while d_mech exists (in double)
-  bool mc_act = false;                     // the actuator rows were allocated by the mechanics setter (model values), and no actuator call has written them since
-  real *d_ct = nullptr;                    // A.contact: [n][CONTACT_W] per-environment contact softness, allocated by the first cassie_batch_set_env_contact (F_CT instances)
-  std::vector<double> ct_host;             // [n][ngeom][8] solref, solimp, solmix every environment sees while d_ct exists (in double: what get returns)
-  bool ct_mech = false;                    // the mechanics rows were allocated by the contact setter (model values), and no mechanics call has written them since
-  real *d_app = nullptr;                   // A.applied: [n][APPLIED_W] per-environment applied forces (state), allocated by the first applied-force verb (F_XF instances)
-  bool xf_ct = false;                      // the contact rows were allocated for the chain twin (model values), and no contact call has written them since
-  bool tc_app = false;                     // the applied-force rows were allocated for the trace, contact-list or sensor instances (zero), and no applied-force verb has
-                                           // written them since
+  // the per-environment row blocks of env_rows.h: constant rows, body offsets, actuators, mechanics, contact softness, applied forces.  Each is [n][width]
+  // reals held in its EnvArrays field; lent: the RowBlock bits of blocks lent for another one (env_rows.h)
+  unsigned lent = 0;
+  std::vector<double> bp_host;             // [n][nbody][3] the offsets every environment sees while A.bpos exists (in double: what get returns)
+  std::vector<double> ac_host;             // [n][nu][4] lo, hi, rpm, delay every environment sees while A.act exists (in double: what get returns)
+  std::vector<double> mc_host;             // [n][mech_host_w()] inertia, armature, stiffness, springref every environment sees while A.mech exists (in double)
+  std::vector<double> ct_host;             // [n][ngeom][8] solref, solimp, solmix every environment sees while A.contact exists (in double: what get returns)
   int tc_ticks = 0;                        // slots the last step launch wrote into the trace rows (A.trace: [n][T][k], allocated by cassie_batch_set_trace)
   Snap *bank = nullptr;                    // the reset bank (cassie_batch_set_reset_bank): a snapshot of k entries
   real *d_loops = nullptr;                 // [n][LOOP_SLOT] status rows of cassie_batch_close_loops, allocated (zero) by its first call
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_loops); cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); cudaFree(d_bpos); cudaFree(d_act); cudaFree(d_mech); cudaFree(d_ct); cudaFree(d_app); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
+    cudaFree(d_loops); cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); for (int b = 0; b <= R_APP; b++) cudaFree(row(b)); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
-    cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.cenv); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
+    cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
     if (pin_pd) cudaFreeHost(pin_pd); if (pin_obs) cudaFreeHost(pin_obs); if (d_hfield) cudaFree(d_hfield);
     if (own_stream && stream) cudaStreamDestroy(stream);
@@ -495,7 +487,7 @@ template <typename real> struct Batch : BatchBase {
       std::vector<real> buf((size_t)n * CST_W); std::vector<int> ibuf((size_t)n * DFILT_W, 0);
       auto fill = [&](real *dst, const std::vector<real> &row, int w) -> bool { for (int e = 0; e < n; e++) memcpy(&buf[(size_t)e * w], row.data(), sizeof(real) * w); CUDA_OK(cudaMemcpyAsync(dst, buf.data(), sizeof(real) * n * w, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream)); return true; };
       if (!fill(A.qpos, qpos, QW) || !fill(A.qvel, qvel, VW) || !fill(A.qacc_ws, qa, VW) || !fill(A.cst, cst, CST_W) || !fill(A.xfrc, xf, XFRC_W)) return false;
-      if (d_app) CUDA_OK(cudaMemsetAsync(d_app, 0, sizeof(real) * n * APPLIED_W, stream));   // applied forces are state, as in mjData
+      if (A.applied) CUDA_OK(cudaMemsetAsync(row(R_APP), 0, sizeof(real) * n * APPLIED_W, stream));   // applied forces are state, as in mjData
       CUDA_OK(cudaMemcpyAsync(A.dfilt, ibuf.data(), sizeof(int) * n * DFILT_W, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream));
       return step(0, 1);
     }
@@ -503,7 +495,7 @@ template <typename real> struct Batch : BatchBase {
     if (!upload_mask(mask)) return false;
     if (!fill_masked(A.qpos, qpos.data(), QW) || !fill_masked(A.qvel, qvel.data(), VW) || !fill_masked(A.qacc_ws, qa.data(), VW) || !fill_masked(A.cst, cst.data(), CST_W) ||
         !fill_masked(A.xfrc, xf.data(), XFRC_W) || !fill_masked(A.dfilt, df.data(), DFILT_W)) return false;
-    if (d_app) { const std::vector<real> zero(APPLIED_W, real(0)); if (!fill_masked(d_app, zero.data(), APPLIED_W)) return false; }
+    if (A.applied) { const std::vector<real> zero(APPLIED_W, real(0)); if (!fill_masked(row(R_APP), zero.data(), APPLIED_W)) return false; }
     return step_masked(1);
   }
   bool upload_mask(const unsigned char *mask) {
@@ -529,14 +521,70 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaMemcpyAsync(A.cenv, all.data(), sizeof(real) * n * CE_W, cudaMemcpyHostToDevice, stream)); CUDA_OK(cudaStreamSynchronize(stream));
     return true;
   }
+  // ---- the per-environment row blocks (env_rows.h): which exist, pull, push, drop and copy, and the rule's plans carried out
+  static constexpr int ROW_W[R_APP + 1] = {CE_W, BP_W, ACT_W, MECH_W, CONTACT_W, APPLIED_W};
+  real *row(int b) const { const void *p[R_APP + 1] = {A.cenv, A.bpos, A.act, A.mech, A.contact, A.applied}; return (real *)p[b]; }
+  void publish(int b, real *r) {
+    switch (b) { case R_CENV: A.cenv = r; break; case R_BPOS: A.bpos = r; break; case R_ACT: A.act = r; break; case R_MECH: A.mech = r; break; case R_CT: A.contact = r; break; default: A.applied = r; }
+  }
+  std::vector<double> *mirror(int b) { std::vector<double> *m[R_APP + 1] = {nullptr, &bp_host, &ac_host, &mc_host, &ct_host, nullptr}; return m[b]; }
+  RowState row_state() const {
+    const void *p[R_N] = {A.cenv, A.bpos, A.act, A.mech, A.contact, A.applied, A.trace.rows, A.cl.rows, A.sn.rows};
+    RowState s; s.lent = lent;
+    for (int b = 0; b < R_N; b++) if (p[b]) s.have |= 1u << b;
+    return s;
+  }
+  bool pull(int b, std::vector<real> &all) {   // the device rows (zero without rows)
+    all.assign((size_t)n * ROW_W[b], real(0));
+    if (!row(b)) return true;
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemcpyAsync(all.data(), row(b), sizeof(real) * n * ROW_W[b], cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    return true;
+  }
+  bool alloc_rows(int b) { real *r = nullptr; if (!row(b)) { CUDA_OK(cudaMalloc(&r, sizeof(real) * n * ROW_W[b])); publish(b, r); } return true; }
+  bool push(int b, const std::vector<real> &all) {
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    if (!alloc_rows(b)) return false;
+    CUDA_OK(cudaMemcpy(row(b), all.data(), sizeof(real) * n * ROW_W[b], cudaMemcpyHostToDevice));
+    return b != R_BPOS || put_reach();
+  }
+  bool drop(int b) {
+    if (mirror(b)) mirror(b)->clear();
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
+    CUDA_OK(cudaFree(row(b))); publish(b, nullptr);
+    return b != R_BPOS || rebuild_model();   // the block's robot_reach is the model's again
+  }
+  bool copy_rows(int b, Batch *src) {   // the source's rows as its environments run with them, and its mirror
+    if (mirror(b)) *mirror(b) = *src->mirror(b);
+    CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    if (!alloc_rows(b)) return false;
+    CUDA_OK(cudaMemcpy(row(b), src->row(b), sizeof(real) * n * ROW_W[b], cudaMemcpyDeviceToDevice));
+    return b != R_BPOS || put_reach();
+  }
+  bool put_model(int b) {   // the block's rows holding the model's values (applied forces: zero), allocated where absent
+    std::vector<real> all;
+    switch (b) {
+      case R_CENV: return ensure_cenv();
+      case R_BPOS: model_bpos_rows(); return put_bpos();
+      case R_ACT: model_act_rows(all); break;
+      case R_MECH: model_mech_rows(all); break;
+      case R_CT: model_ct_rows(all); break;
+      default: all.assign((size_t)n * APPLIED_W, real(0));
+    }
+    return push(b, all);
+  }
+  bool run(const RowPlan &p) {
+    for (int i = 0; i < p.n; i++) if (!(p.step[i].op == ROW_DROP ? drop(p.step[i].block) : put_model(p.step[i].block))) return false;
+    return true;
+  }
+  bool rows_rule(void (*rule)(RowState &, RowPlan &, int), int b) { RowState s = row_state(); RowPlan p; rule(s, p, b); lent = s.lent; return run(p); }
   int cenv_slot(const char *what, int i, int &width) const { return cassie::cenv_slot(hm, h_model_copy.nv, geom_dev, what, i, width); }
   bool set_model_rows(const char *what, const double *rows, int width) override {
     int w = 0; cenv_slot(what, 0, w);
     if (w < 0 || w != width) { set_err(std::string("set_model_rows: unknown array or wrong width for ") + what); return false; }
     if (!strcmp(what, "body_ipos") && h_model_copy.xb >= 0) for (int e = 0; e < n; e++) for (int k = 0; k < 3; k++)
       if (rows[(size_t)e * w + 3 * h_model_copy.xb + k] != hm.body_ipos[3 * h_model_copy.xb + k]) { set_err("body_ipos of the extra free body cannot be changed (its inertial frame must stay its body frame)"); return false; }
-    if (!ensure_cenv()) return false;
-    bp_cenv = false;
+    if (!ensure_cenv() || !rows_rule(own, R_CENV)) return false;
     std::vector<real> all((size_t)n * CE_W);
     CUDA_OK(cudaMemcpyAsync(all.data(), A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
     for (int e = 0; e < n; e++) for (int i = 0; i < w; i++) { int ww; const int sl = cenv_slot(what, i, ww); if (sl >= 0) all[(size_t)e * CE_W + sl] = (real)rows[(size_t)e * w + i]; }
@@ -768,11 +816,11 @@ template <typename real> struct Batch : BatchBase {
   // ---- snapshots (the Snap object owns its device memory and knows its own sizes: it may outlive this batch)
   Snap *snap_alloc() override { Snap *k = snap_new(device, n, (int)sizeof(real), QW, VW); if (!k) set_err("snapshot: out of device memory"); return k; }
   bool snap_compatible(const Snap *k) { if (k && k->n == n && k->esz == (int)sizeof(real) && k->qw == QW && k->vw == VW) return true; set_err("snapshot: taken from a batch of another size, precision or model"); return false; }
-  void *snap_src(int r) { void *t[Snap::NROWS] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux, d_app}; return t[r]; }
+  void *snap_src(int r) { void *t[Snap::NROWS] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux, row(R_APP)}; return t[r]; }
   bool snap_get(Snap *k) override {
     if (!snap_compatible(k)) return false;
     CUDA_OK(cudaSetDevice(device));
-    k->has_est = A.est != nullptr; k->has_aux = A.aux != nullptr; k->has_appl = d_app != nullptr;
+    k->has_est = A.est != nullptr; k->has_aux = A.aux != nullptr; k->has_appl = A.applied != nullptr;
     for (int r = 0; r < Snap::NROWS; r++) {
       if (!k->has(r)) continue;
       if (!k->rows[r]) CUDA_OK(cudaMalloc(&k->rows[r], k->bytes(r)));
@@ -789,10 +837,10 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     if (mask && !upload_mask(mask)) return false;
     if (k->has_est && !A.est && !enable_estimator_device(true)) return false;   // optional rows the snapshot has are allocated where the batch lacks them
-    if (k->has_appl && !d_app && !enable_applied_forces(true)) return false;
+    if (k->has_appl && !A.applied && !enable_applied_forces(true)) return false;
     if (mask) return restore_rows(k, d_mask, nullptr) && sync();   // one launch: the snapshot as a bank of n entries, environment e taking entry e
     if (!k->has_est && A.est && !reset_estimator_device(nullptr)) return false;   // the snapshot was taken before the estimator ran: it starts afresh
-    if (!k->has_appl && d_app) CUDA_OK(cudaMemsetAsync(d_app, 0, sizeof(real) * n * APPLIED_W, stream));   // likewise the applied forces: zeroed
+    if (!k->has_appl && A.applied) CUDA_OK(cudaMemsetAsync(row(R_APP), 0, sizeof(real) * n * APPLIED_W, stream));   // likewise the applied forces: zeroed
     for (int r = 0; r < Snap::NROWS; r++) {
       if (!k->has(r) || (r == Snap::R_AUX && !A.aux)) continue;
       CUDA_OK(cudaMemcpyAsync(snap_src(r), k->rows[r], k->bytes(r), cudaMemcpyDeviceToDevice, stream));
@@ -804,7 +852,7 @@ template <typename real> struct Batch : BatchBase {
   // one launch of the restore kernel (reset.cu) from the entries of k into the rows of this batch: environment e, when d_mask[e] is non-zero (null: every
   // environment), takes entry (unsigned)d_entry[e] % k->n (null: e % k->n), by reset_table's rules.  Enqueued only: no synchronisation, copy or allocation
   bool restore_rows(const Snap *k, const unsigned char *dmask, const int *dentry) {
-    void *dst[RR_N] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux, d_app, A.frames, A.acc};
+    void *dst[RR_N] = {A.qpos, A.qvel, A.qacc_ws, A.cst, A.xfrc, A.obs, A.dfilt, A.est, A.aux, row(R_APP), A.frames, A.acc};
     const void *src[RR_N];
     for (int r = 0; r < Snap::NROWS; r++) src[r] = k->has(r) ? k->rows[r] : nullptr;
     src[RR_FRAMES] = k->frames; src[RR_ACC] = k->acc;
@@ -873,7 +921,7 @@ template <typename real> struct Batch : BatchBase {
   bool forward_where(const void *d_mask) override {
     const char *verb = "cassie_batch_forward_where";
     if (!device_rows(d_mask, verb, "the mask")) return false;
-    if (A.applied && !A.contact && launch_kind(1) == 1) {   // step_range would allocate the chain twin's contact rows here
+    if (launch_lends_ext(row_state(), launch_kind(1) == 1)) {   // step_range would lend the chain twin's contact rows here
       set_err(std::string(verb) + ": this batch gets model-valued contact rows at its first extended launch; run cassie_batch_step or cassie_batch_forward once first"); return false; }
     A.mask = (const unsigned char *)d_mask; const bool ok = step(0, 1); A.mask = nullptr;
     return ok;
@@ -889,7 +937,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     if (!d_loops) { CUDA_OK(cudaMalloc(&d_loops, sizeof(real) * n * LOOP_SLOT)); CUDA_OK(cudaMemsetAsync(d_loops, 0, sizeof(real) * n * LOOP_SLOT, stream)); }
     if (L.T.nrow == 0) return true;   // no connect equality: nothing to close
-    L.model = d_model; L.qpos = A.qpos; L.qpos_w = QW; L.qvel = A.qvel; L.qvel_w = VW; L.bpos = d_bpos; L.status = d_loops;
+    L.model = d_model; L.qpos = A.qpos; L.qpos_w = QW; L.qvel = A.qvel; L.qvel_w = VW; L.bpos = A.bpos; L.status = d_loops;
     L.mask = (const unsigned char *)d_mask; L.n = n; L.max_iter = max_iter; L.tol = (real)tol;
     CUDA_OK(launch_loops<real>(L, device, stream));
     launches++;
@@ -912,7 +960,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     DevModel<real> *hmodel = (DevModel<real> *)calloc(1, model_bytes<real>()); std::string err; BuildInfo info;
     if (!build_dev_model(hm, *hmodel, err, &info)) { free(hmodel); set_err(err); return false; }
-    if (d_bpos) hmodel->robot_reach = rows_reach(*hmodel);   // per-environment body offsets: the broad phase's bound covers every row
+    if (A.bpos) hmodel->robot_reach = rows_reach(*hmodel);   // per-environment body offsets: the broad phase's bound covers every row
     CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaMemcpy(d_model, hmodel, model_bytes<real>(), cudaMemcpyHostToDevice));
     h_model_copy = *hmodel; free(hmodel);
@@ -924,12 +972,11 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaSetDevice(device));
     hm = src->hm;
     if (!rebuild_model()) return false;
-    if (!src->d_ct && !clear_env_contact()) return false;   // likewise the contact rows and the mechanics rows their setter allocated
-    if (!src->d_mech && !clear_env_mechanics()) return false;   // likewise the mechanics rows and the actuator rows their setter allocated
-    if (!src->d_act && !clear_env_actuators()) return false;   // likewise the actuator rows and the offset rows their setter allocated
-    if (!src->d_bpos && !clear_env_body_pos()) return false;   // before the constant rows are copied: clearing drops rows the offset setter allocated
-    if (src->A.cenv) { if (!ensure_cenv()) return false; CUDA_OK(cudaMemcpyAsync(A.cenv, src->A.cenv, sizeof(real) * n * CE_W, cudaMemcpyDeviceToDevice, stream)); }
-    else if (A.cenv) { CUDA_OK(cudaStreamSynchronize(stream)); CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; }
+    { RowState st = row_state(); RowPlan p; copy_from(st, p, src->row_state());   // what the source lacks is dropped first, top down
+      if (!run(p)) return false;
+      for (int b = R_CENV; b < R_APP; b++)
+        if (src->row(b) ? !copy_rows(b, src) : row(b) && !drop(b)) return false;   // (the constant rows: the others were dropped above)
+      lent = st.lent; }
     if (!src->d_terrain && !clear_env_hfield()) return false;
     if (src->d_genv) { if (!ensure_genv()) return false; CUDA_OK(cudaMemcpyAsync(d_genv, src->d_genv, sizeof(real) * n * GEOM_ENV_W, cudaMemcpyDeviceToDevice, stream)); }
     else if (!clear_env_geoms()) return false;
@@ -939,21 +986,6 @@ template <typename real> struct Batch : BatchBase {
       CUDA_OK(cudaMemcpyAsync(d_terrain, src->d_terrain, sizeof(int) * n, cudaMemcpyDeviceToDevice, stream));
       hf_host = src->hf_host;
     }
-    if (src->d_bpos) { bp_host = src->bp_host; bp_cenv = src->bp_cenv; if (!put_bpos()) return false; }   // the source's constant rows came above
-    if (src->d_act) {   // the rows as the source's environments run with them (its offset rows came just now)
-      ac_host = src->ac_host; ac_bpos = src->ac_bpos;
-      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
-      if (!d_act) CUDA_OK(cudaMalloc(&d_act, sizeof(real) * n * ACT_W));
-      CUDA_OK(cudaMemcpy(d_act, src->d_act, sizeof(real) * n * ACT_W, cudaMemcpyDeviceToDevice));
-      A.act = d_act;
-    }
-    if (src->d_mech) {   // likewise the mechanics rows (the actuator rows came just now)
-      mc_host = src->mc_host; mc_act = src->mc_act;
-      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
-      if (!d_mech) CUDA_OK(cudaMalloc(&d_mech, sizeof(real) * n * MECH_W));
-      CUDA_OK(cudaMemcpy(d_mech, src->d_mech, sizeof(real) * n * MECH_W, cudaMemcpyDeviceToDevice));
-      A.mech = d_mech;
-    }
     if (src->d_camenv && src->cam.k == cam.k) {   // the per-environment camera mounts, when the two batches hold as many cameras
       ce_host = src->ce_host;
       CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
@@ -961,13 +993,6 @@ template <typename real> struct Batch : BatchBase {
       if (!d_camenv) CUDA_OK(cudaMalloc(&d_camenv, sizeof(real) * w));
       CUDA_OK(cudaMemcpy(d_camenv, src->d_camenv, sizeof(real) * w, cudaMemcpyDeviceToDevice));
     } else if (!clear_env_cameras()) return false;
-    if (src->d_ct) {   // likewise the contact rows (the mechanics rows came just now)
-      ct_host = src->ct_host; ct_mech = src->ct_mech; xf_ct = src->xf_ct;
-      CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
-      if (!d_ct) CUDA_OK(cudaMalloc(&d_ct, sizeof(real) * n * CONTACT_W));
-      CUDA_OK(cudaMemcpy(d_ct, src->d_ct, sizeof(real) * n * CONTACT_W, cudaMemcpyDeviceToDevice));
-      A.contact = d_ct;
-    }
     if (src->A.sn.rows) {   // the sensor models and the generator rows: a copy draws what its source would
       if (!A.sn.rows && !alloc_sensors()) return false;
       CUDA_OK(cudaStreamSynchronize(src->stream)); CUDA_OK(cudaStreamSynchronize(stream));
@@ -1135,12 +1160,11 @@ template <typename real> struct Batch : BatchBase {
     const int nb3 = 3 * hm.nbody;
     std::vector<real> all((size_t)n * BP_W, real(0));
     for (int e = 0; e < n; e++) for (int i = 0; i < nb3; i++) all[(size_t)e * BP_W + i] = (real)bp_host[(size_t)e * nb3 + i];
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows and the block
-    if (!d_bpos) CUDA_OK(cudaMalloc(&d_bpos, sizeof(real) * n * BP_W));
-    CUDA_OK(cudaMemcpy(d_bpos, all.data(), sizeof(real) * n * BP_W, cudaMemcpyHostToDevice));
+    return push(R_BPOS, all);
+  }
+  bool put_reach() {   // after the offset rows changed (a launch in flight reads the block: the caller synchronised)
     h_model_copy.robot_reach = rows_reach(h_model_copy);
     CUDA_OK(cudaMemcpy(&d_model->robot_reach, &h_model_copy.robot_reach, sizeof(real), cudaMemcpyHostToDevice));
-    A.bpos = d_bpos;
     return true;
   }
   bool set_env_body_pos(const double *pos, const unsigned char *mask) override {
@@ -1159,11 +1183,9 @@ template <typename real> struct Batch : BatchBase {
         if (!w.empty()) { set_err(at + "the offset of " + w + " cannot change"); return false; }
       }
     }
-    if (!A.cenv) bp_cenv = true;
-    if (!ensure_cenv()) return false;   // mode 3 (set_const) writes the environment's invweights into its constant row
+    if (!rows_rule(own, R_BPOS)) return false;
     if (bp_host.empty()) { bp_host.resize((size_t)n * nb3); for (int e = 0; e < n; e++) memcpy(&bp_host[(size_t)e * nb3], hm.body_pos.data(), sizeof(double) * nb3); }
     for (int e = 0; e < n; e++) if (!mask || mask[e]) memcpy(&bp_host[(size_t)e * nb3], pos + (size_t)e * nb3, sizeof(double) * nb3);
-    ac_bpos = false;   // the rows are the caller's now, also when the actuator setter allocated them
     return put_bpos();
   }
   bool get_env_body_pos(double *pos) override {
@@ -1172,44 +1194,18 @@ template <typename real> struct Batch : BatchBase {
     for (int e = 0; e < n; e++) memcpy(pos + (size_t)e * nb3, bp_host.empty() ? hm.body_pos.data() : &bp_host[(size_t)e * nb3], sizeof(double) * nb3);
     return true;
   }
-  // back to the model's offsets and the instances that ran before: the block's robot_reach is the model's again, and constant rows the setter
-  // allocated (and no model-row setter wrote since) are dropped.  A batch with actuator rows keeps offset rows, holding the model's values again.
-  bool clear_env_body_pos() override {
-    if (d_act) { model_bpos_rows(); ac_bpos = true; return put_bpos(); }
-    bp_host.clear();
-    if (!d_bpos) return true;
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
-    CUDA_OK(cudaFree(d_bpos)); d_bpos = nullptr; A.bpos = nullptr;
-    if (bp_cenv) { CUDA_OK(cudaFree(A.cenv)); A.cenv = nullptr; bp_cenv = false; }
-    return rebuild_model();
-  }
+  bool clear_env_body_pos() override { return rows_rule(release, R_BPOS); }   // back to the model's offsets and the instances that ran before
   void model_bpos_rows() {   // the mirror of offset rows holding the model's offsets in every environment
     const int nb3 = 3 * hm.nbody;
     bp_host.resize((size_t)n * nb3); for (int e = 0; e < n; e++) memcpy(&bp_host[(size_t)e * nb3], hm.body_pos.data(), sizeof(double) * nb3);
   }
   // ---- per-environment actuators (actuator latency and torque saturation: sim-to-real randomisation): ctrlrange, no-load speed and torque delay per
-  // motor, read by the F_AC instances' motor stage and actuation.  Those instances are the F_AC twins of the F_BP ones, so a batch with actuator rows
-  // carries offset rows too: when it has none, the actuator setter allocates them holding the model's values (and constant rows with them, as the
-  // offset setter does); clear drops them again unless a body-offset call has written them since.
-  // The device rows are what the environments run with: a caller may have written them through the "actuators" device pointer.  The mirror keeps
-  // the doubles the verb was last given, so that get reports them exactly (rpm included) wherever the device still holds what they stored.
+  // motor, read by the F_AC instances' motor stage and actuation.  The device rows are what the environments run with: a caller may have written them
+  // through the "actuators" device pointer.  The mirror keeps the doubles the verb was last given, so that get reports them exactly (rpm included)
+  // wherever the device still holds what they stored.
   static real act_row_value(const double *a, int f) { return f == 2 ? (real)(a[2] * 2 * M_PI / 60) : (real)a[f]; }   // wmax: build_dev_model's expression
   static int act_delay_host(real v) { return (int)(v > real(0) ? (v < real(AC_MAXDELAY) ? v : real(AC_MAXDELAY)) : real(0)); }   // the kernel's act_delay_index
   static constexpr int AC_FIELD[4] = {AC_LO, AC_HI, AC_WMAX, AC_DELAY};
-  bool pull_act(std::vector<real> &all) {   // the device rows (zero without rows)
-    all.assign((size_t)n * ACT_W, real(0));
-    if (!d_act) return true;
-    CUDA_OK(cudaSetDevice(device));
-    CUDA_OK(cudaMemcpyAsync(all.data(), d_act, sizeof(real) * n * ACT_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
-    return true;
-  }
-  bool push_act(const std::vector<real> &all) {
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
-    if (!d_act) CUDA_OK(cudaMalloc(&d_act, sizeof(real) * n * ACT_W));
-    CUDA_OK(cudaMemcpy(d_act, all.data(), sizeof(real) * n * ACT_W, cudaMemcpyHostToDevice));
-    A.act = d_act;
-    return true;
-  }
   void model_act(int i, double *a) const {   // motor i as the model has it: lo, hi (the clamp the block holds), rpm, the reference's delay
     a[0] = (double)h_model_copy.act_ctrl_lo[i]; a[1] = (double)h_model_copy.act_ctrl_hi[i]; a[2] = hm.actuator_user[i]; a[3] = AC_MAXDELAY;
   }
@@ -1227,17 +1223,10 @@ template <typename real> struct Batch : BatchBase {
     if (nu > MU) { set_err(verb + ": the model has more than " + std::to_string(MU) + " actuators"); return false; }
     const std::string why = env_actuators_check(n, nu, ctrlrange, rpm, delay, mask);   // every masked value is checked before anything changes
     if (!why.empty()) { set_err(verb + ": " + why); return false; }
-    if (!d_bpos) {   // the F_AC instances read offset rows: the model's values, dropped again by clear unless a body-offset call writes them
-      if (!A.cenv) bp_cenv = true;
-      if (!ensure_cenv()) return false;
-      model_bpos_rows();
-      if (!put_bpos()) return false;
-      ac_bpos = true;
-    }
-    mc_act = false;   // the rows are the caller's now, also when the mechanics setter allocated them
+    if (!rows_rule(own, R_ACT)) return false;
     std::vector<real> all;
-    if (!d_act) model_act_rows(all);   // the first call: every environment starts from the model's actuators
-    else if (!pull_act(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    if (!A.act) model_act_rows(all);   // the first call: every environment starts from the model's actuators
+    else if (!pull(R_ACT, all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
     for (int e = 0; e < n; e++) {
       if (mask && !mask[e]) continue;
       for (int i = 0; i < nu; i++) {
@@ -1247,19 +1236,19 @@ template <typename real> struct Batch : BatchBase {
         if (delay) { a[3] = delay[k]; r[AC_DELAY + i] = act_row_value(a, 3); }
       }
     }
-    return push_act(all);
+    return push(R_ACT, all);
   }
   // what every environment runs with: a value the device row still holds as the verb stored it is reported as the verb was given it; one written on the
   // device is reported from the row (rpm = wmax * 60 / 2 pi, the delay as the kernel reads it)
   bool get_env_actuators(double *ctrlrange, double *rpm, int *delay) override {
     const int nu = hm.nu;
     std::vector<real> all;
-    if (!pull_act(all)) return false;
+    if (!pull(R_ACT, all)) return false;
     for (int e = 0; e < n; e++) for (int i = 0; i < nu; i++) {
       const size_t k = (size_t)e * nu + i;
       double m[4]; model_act(i, m);
       double v[4] = {m[0], m[1], m[2], m[3]};
-      if (d_act) {
+      if (A.act) {
         const double *a = &ac_host[k * 4];
         for (int f = 0; f < 4; f++) {
           const real dv = all[(size_t)e * ACT_W + AC_FIELD[f] + i];
@@ -1273,21 +1262,10 @@ template <typename real> struct Batch : BatchBase {
     }
     return true;
   }
-  // back to the model's actuators and the instances that ran before.  A batch with mechanics rows keeps actuator rows, holding the model's values again.
-  bool clear_env_actuators() override {
-    if (d_mech) { std::vector<real> all; model_act_rows(all); mc_act = true; return push_act(all); }
-    ac_host.clear();
-    if (!d_act) return true;
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
-    CUDA_OK(cudaFree(d_act)); d_act = nullptr; A.act = nullptr;
-    if (ac_bpos) { ac_bpos = false; return clear_env_body_pos(); }   // (which drops the constant rows too when the offset rows brought them)
-    return true;
-  }
+  bool clear_env_actuators() override { return rows_rule(release, R_ACT); }   // back to the model's actuators and the instances that ran before
   // ---- per-environment mechanics (link inertia, rotor armature, leaf springs: sim-to-real randomisation): MuJoCo's body_inertia, dof_armature and the
-  // jnt_stiffness / qpos_spring of the hinges per environment, read by the F_MC instances' cinert, CRB and passive phases.  Those instances are the F_MC
-  // twins of the F_AC ones, so a batch with mechanics rows carries actuator rows too: when it has none, the setter allocates them holding the model's
-  // values (and offset and constant rows with them, as the actuator setter does); clear drops them again unless an actuator call has written them since.
-  // As with the actuator rows, the device rows are what the environments run with, and the mirror keeps the doubles the verb was last given.
+  // jnt_stiffness / qpos_spring of the hinges per environment, read by the F_MC instances' cinert, CRB and passive phases.  As with the actuator rows,
+  // the device rows are what the environments run with, and the mirror keeps the doubles the verb was last given.
   int mech_host_w() const { return 3 * hm.nbody + hm.nv + 2 * hm.njnt; }   // the mirror per environment: inertia [nbody][3], armature [nv], stiffness [njnt], springref [njnt]
   int mech_slot(int k) const {   // the row slot of mirror entry k, or -1 where the kernel reads the block (the extra free body's dofs, non-hinge springs)
     const int nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
@@ -1302,20 +1280,6 @@ template <typename real> struct Batch : BatchBase {
     if ((k -= nb3) < nv) return hm.dof_armature[k];
     return (k -= nv) < nj ? hm.jnt_stiffness[k] : hm.qpos_spring[hm.jnt_qposadr[k - nj]];
   }
-  bool pull_mech(std::vector<real> &all) {
-    all.assign((size_t)n * MECH_W, real(0));
-    if (!d_mech) return true;
-    CUDA_OK(cudaSetDevice(device));
-    CUDA_OK(cudaMemcpyAsync(all.data(), d_mech, sizeof(real) * n * MECH_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
-    return true;
-  }
-  bool push_mech(const std::vector<real> &all) {
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
-    if (!d_mech) CUDA_OK(cudaMalloc(&d_mech, sizeof(real) * n * MECH_W));
-    CUDA_OK(cudaMemcpy(d_mech, all.data(), sizeof(real) * n * MECH_W, cudaMemcpyHostToDevice));
-    A.mech = d_mech;
-    return true;
-  }
   void model_mech_rows(std::vector<real> &all) {   // the mirror and the rows holding the model's values in every environment (a non-hinge dof's slots too, though the kernel reads the block there)
     const int w = mech_host_w();
     mc_host.resize((size_t)n * w); all.assign((size_t)n * MECH_W, real(0));
@@ -1329,15 +1293,11 @@ template <typename real> struct Batch : BatchBase {
     const std::string verb = "cassie_batch_set_env_mechanics";
     const std::string why = env_mechanics_check(hm, n, h_model_copy.xb, h_model_copy.nv, inertia, armature, stiffness, springref, mask);   // every masked value first
     if (!why.empty()) { set_err(verb + ": " + why); return false; }
-    if (!d_act) {   // the F_MC instances read actuator rows: the model's values, dropped again by clear unless an actuator call writes them
-      if (!set_env_actuators(nullptr, nullptr, nullptr, nullptr)) return false;
-      mc_act = true;
-    }
-    ct_mech = false;   // the rows are the caller's now, also when the contact setter allocated them
+    if (!rows_rule(own, R_MECH)) return false;
     const int w = mech_host_w(), nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
     std::vector<real> all;
-    if (!d_mech) model_mech_rows(all);   // the first call: every environment starts from the model's values
-    else if (!pull_mech(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    if (!A.mech) model_mech_rows(all);   // the first call: every environment starts from the model's values
+    else if (!pull(R_MECH, all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
     const double *part[4] = {inertia, armature, stiffness, springref};
     const int off[5] = {0, nb3, nb3 + nv, nb3 + nv + nj, w};
     for (int e = 0; e < n; e++) {
@@ -1352,14 +1312,14 @@ template <typename real> struct Batch : BatchBase {
         }
       }
     }
-    return push_mech(all);
+    return push(R_MECH, all);
   }
   // what every environment runs with: a value the device row still holds as the verb stored it is reported as the verb was given it, one written on the
   // device from the row; where the kernel reads the block (the extra free body's armature, non-hinge springs), the block's current value
   bool get_env_mechanics(double *inertia, double *armature, double *stiffness, double *springref) override {
     const int w = mech_host_w(), nb3 = 3 * hm.nbody, nv = hm.nv, nj = hm.njnt;
     std::vector<real> all;
-    if (!pull_mech(all)) return false;
+    if (!pull(R_MECH, all)) return false;
     double *part[4] = {inertia, armature, stiffness, springref};
     const int off[5] = {0, nb3, nb3 + nv, nb3 + nv + nj, w};
     for (int e = 0; e < n; e++) for (int p = 0; p < 4; p++) {
@@ -1368,28 +1328,16 @@ template <typename real> struct Batch : BatchBase {
       for (int i = 0; i < cnt; i++) {
         const int k = off[p] + i, sl = mech_slot(k);
         double v = block_mech(k);
-        if (d_mech && sl >= 0) { const real dv = all[(size_t)e * MECH_W + sl]; const double a = mc_host[(size_t)e * w + k]; v = dv == (real)a ? a : (double)dv; }
+        if (A.mech && sl >= 0) { const real dv = all[(size_t)e * MECH_W + sl]; const double a = mc_host[(size_t)e * w + k]; v = dv == (real)a ? a : (double)dv; }
         part[p][(size_t)e * cnt + i] = v;
       }
     }
     return true;
   }
-  // back to the model's values and the instances that ran before (which drops the actuator rows too when this setter brought them).  A batch with contact
-  // rows keeps mechanics rows, holding the model's values again.
-  bool clear_env_mechanics() override {
-    if (d_ct) { std::vector<real> all; model_mech_rows(all); ct_mech = true; return push_mech(all); }
-    mc_host.clear();
-    if (!d_mech) return true;
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
-    CUDA_OK(cudaFree(d_mech)); d_mech = nullptr; A.mech = nullptr;
-    if (mc_act) { mc_act = false; return clear_env_actuators(); }
-    return true;
-  }
+  bool clear_env_mechanics() override { return rows_rule(release, R_MECH); }   // back to the model's values and the instances that ran before
   // ---- per-environment contact softness (ground stiffness, damping and impedance: sim-to-real randomisation): MuJoCo's geom_solref, geom_solimp and
-  // geom_solmix per collision geom and environment, mixed per contact row by the F_CT instances' constraint stage.  Those instances are the F_CT twins of
-  // the F_MC ones, so a batch with contact rows carries mechanics rows too: when it has none, the setter allocates them holding the model's values (and
-  // actuator, offset and constant rows with them, as the mechanics setter does); clear drops them again unless a mechanics call has written them since.
-  // The device rows are what the environments run with, and the mirror keeps the doubles the verb was last given.
+  // geom_solmix per collision geom and environment, mixed per contact row by the F_CT instances' constraint stage.  The device rows are what the
+  // environments run with, and the mirror keeps the doubles the verb was last given.
   int ct_slot(int g) const { return g < 256 && geom_dev[g] >= 0 && geom_dev[g] < MGT ? geom_dev[g] : -1; }   // the device geom of host geom g, or -1: no contact
   static int ct_field(int f) { return f < 2 ? CT_SOLREF + f : (f < 7 ? CT_SOLIMP + f - 2 : CT_SOLMIX); }   // mirror field f (solref 2, solimp 5, solmix 1) -> slot offset
   double model_ct(int g, int f) const { return f < 2 ? hm.geom_solref[2 * g + f] : (f < 7 ? hm.geom_solimp[5 * g + f - 2] : hm.geom_solmix[g]); }
@@ -1404,33 +1352,15 @@ template <typename real> struct Batch : BatchBase {
       }
     }
   }
-  bool pull_ct(std::vector<real> &all) {
-    all.assign((size_t)n * CONTACT_W, real(0));
-    if (!d_ct) return true;
-    CUDA_OK(cudaSetDevice(device));
-    CUDA_OK(cudaMemcpyAsync(all.data(), d_ct, sizeof(real) * n * CONTACT_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
-    return true;
-  }
-  bool push_ct(const std::vector<real> &all) {
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
-    if (!d_ct) CUDA_OK(cudaMalloc(&d_ct, sizeof(real) * n * CONTACT_W));
-    CUDA_OK(cudaMemcpy(d_ct, all.data(), sizeof(real) * n * CONTACT_W, cudaMemcpyHostToDevice));
-    A.contact = d_ct;
-    return true;
-  }
   bool set_env_contact(const double *solref, const double *solimp, const double *solmix, const unsigned char *mask) override {
     const std::string verb = "cassie_batch_set_env_contact";
     const std::string why = env_contact_check(hm, n, geom_dev, solref, solimp, solmix, mask);   // every masked value first
     if (!why.empty()) { set_err(verb + ": " + why); return false; }
-    xf_ct = false;   // the rows are the caller's now, also when the chain twin's launch allocated them
-    if (!d_mech) {   // the F_CT instances read mechanics rows: the model's values, dropped again by clear unless a mechanics call writes them
-      if (!set_env_mechanics(nullptr, nullptr, nullptr, nullptr, nullptr)) return false;
-      ct_mech = true;
-    }
+    if (!rows_rule(own, R_CT)) return false;
     const int ng = hm.ngeom;
     std::vector<real> all;
-    if (!d_ct) model_ct_rows(all);   // the first call: every environment starts from the model's values
-    else if (!pull_ct(all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
+    if (!A.contact) model_ct_rows(all);   // the first call: every environment starts from the model's values
+    else if (!pull(R_CT, all)) return false;   // unmasked environments keep what their rows hold, also when it was written on the device
     const double *part[3] = {solref, solimp, solmix};
     const int off[4] = {0, 2, 7, 8};
     for (int e = 0; e < n; e++) {
@@ -1448,14 +1378,14 @@ template <typename real> struct Batch : BatchBase {
         }
       }
     }
-    return push_ct(all);
+    return push(R_CT, all);
   }
   // what every environment runs with: a value the device row still holds as the verb stored it is reported as the verb was given it, one written on the
   // device from the row; geoms without a collision slot report the model's values
   bool get_env_contact(double *solref, double *solimp, double *solmix) override {
     const int ng = hm.ngeom;
     std::vector<real> all;
-    if (!pull_ct(all)) return false;
+    if (!pull(R_CT, all)) return false;
     double *part[3] = {solref, solimp, solmix};
     const int off[4] = {0, 2, 7, 8};
     for (int e = 0; e < n; e++) for (int g = 0; g < ng; g++) {
@@ -1466,38 +1396,24 @@ template <typename real> struct Batch : BatchBase {
         for (int i = 0; i < cnt; i++) {
           const int f = off[p] + i;
           double v = model_ct(g, f);
-          if (d_ct && s >= 0) { const real dv = all[(size_t)e * CONTACT_W + CT_SLOT * s + ct_field(f)]; const double a = ct_host[((size_t)e * ng + g) * CT_SLOT + f]; v = dv == (real)a ? a : (double)dv; }
+          if (A.contact && s >= 0) { const real dv = all[(size_t)e * CONTACT_W + CT_SLOT * s + ct_field(f)]; const double a = ct_host[((size_t)e * ng + g) * CT_SLOT + f]; v = dv == (real)a ? a : (double)dv; }
           part[p][((size_t)e * ng + g) * cnt + i] = v;
         }
       }
     }
     return true;
   }
-  // back to the model's values and the instances that ran before (which drops the mechanics rows too when this setter brought them)
-  bool clear_env_contact() override {
-    ct_host.clear(); xf_ct = false;
-    if (!d_ct) return true;
-    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
-    CUDA_OK(cudaFree(d_ct)); d_ct = nullptr; A.contact = nullptr;
-    if (ct_mech) { ct_mech = false; return clear_env_mechanics(); }
-    return true;
-  }
+  bool clear_env_contact() override { return rows_rule(release, R_CT); }   // back to the model's values and the instances that ran before
   // ---- per-environment applied forces (pushes on any body, joint-space disturbances): MuJoCo's xfrc_applied and qfrc_applied per environment.  They are
   // state, as in mjData: reset zeroes them, snapshots carry them.  The device rows are what the environments run with (a write through the device
   // pointer takes effect at the next launch), so the verbs read them back and keep no mirror.  A batch with rows runs f0404 / f2404 where f04 / f24
-  // would run, else the chain twins, which read contact rows: step_range allocates those holding the model's values (xf_ct) when the batch has none.
+  // would run, else the chain twins.
   int ap_col(int i) const { const int nvm = h_model_copy.nv; return i < nvm ? i : 32 + (i - nvm); }   // host dof i -> its column in AP_QFRC
   bool enable_applied_forces(bool on) override {
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight reads the rows
-    tc_app = false;   // the rows are the caller's now, also when the trace allocated them
-    if (on) {
-      if (!d_app) { CUDA_OK(cudaMalloc(&d_app, sizeof(real) * n * APPLIED_W)); CUDA_OK(cudaMemset(d_app, 0, sizeof(real) * n * APPLIED_W)); }
-      A.applied = d_app;
-      return true;
-    }
-    if (d_app) { CUDA_OK(cudaFree(d_app)); d_app = nullptr; A.applied = nullptr; }
-    if (xf_ct) return clear_env_contact();   // back to the instances that ran before (clear resets xf_ct)
-    return true;
+    if (on) return rows_rule(own, R_APP) && (A.applied || put_model(R_APP));   // the first call: zeroed rows
+    if (A.applied && !drop(R_APP)) return false;
+    return rows_rule(dropped, R_APP);   // back to the instances that ran before
   }
   bool set_applied_forces(const double *xfrc, const double *qfrc, const unsigned char *mask) override {
     const int nb = hm.nbody, nv = hm.nv;
@@ -1509,22 +1425,20 @@ template <typename real> struct Batch : BatchBase {
       for (int i = 0; qfrc && i < nv; i++) if (!std::isfinite(qfrc[(size_t)e * nv + i])) {
         set_err("cassie_batch_set_applied_forces: environment " + std::to_string(e) + ", dof " + std::to_string(i) + ": qfrc_applied is not finite"); return false; }
     }
-    if (!enable_applied_forces(true)) return false;   // the first call: zeroed rows
-    std::vector<real> all((size_t)n * APPLIED_W);
-    CUDA_OK(cudaMemcpy(all.data(), d_app, sizeof(real) * n * APPLIED_W, cudaMemcpyDeviceToHost));   // unmasked environments keep what their rows hold
+    std::vector<real> all;
+    if (!enable_applied_forces(true) || !pull(R_APP, all)) return false;   // unmasked environments keep what their rows hold
     for (int e = 0; e < n; e++) {
       if (mask && !mask[e]) continue;
       real *r = &all[(size_t)e * APPLIED_W];
       if (xfrc) for (int b = 0; b < nb; b++) for (int k = 0; k < 6; k++) r[AP_XFRC + 6 * b + k] = (real)xfrc[((size_t)e * nb + b) * 6 + k];
       if (qfrc) for (int i = 0; i < nv; i++) r[AP_QFRC + ap_col(i)] = (real)qfrc[(size_t)e * nv + i];
     }
-    CUDA_OK(cudaMemcpy(d_app, all.data(), sizeof(real) * n * APPLIED_W, cudaMemcpyHostToDevice));
-    return true;
+    return push(R_APP, all);
   }
   bool get_applied_forces(double *xfrc, double *qfrc) override {   // what the rows hold; zeros without rows
     const int nb = hm.nbody, nv = hm.nv;
-    std::vector<real> all((size_t)n * APPLIED_W, real(0));
-    if (d_app) { CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaMemcpyAsync(all.data(), d_app, sizeof(real) * n * APPLIED_W, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream)); }
+    std::vector<real> all;
+    if (!pull(R_APP, all)) return false;
     for (int e = 0; e < n; e++) {
       const real *r = &all[(size_t)e * APPLIED_W];
       if (xfrc) for (int b = 0; b < nb; b++) for (int k = 0; k < 6; k++) xfrc[((size_t)e * nb + b) * 6 + k] = (double)r[AP_XFRC + 6 * b + k];
@@ -1533,19 +1447,13 @@ template <typename real> struct Batch : BatchBase {
     return true;
   }
   bool clear_applied_xfrc() override {   // cassie_batch_clear_forces: MuJoCo's xfrc_applied of every environment; qfrc_applied stays (src/cassiemujoco.c:1969-1972)
-    if (!d_app) return true;
+    if (!A.applied) return true;
     CUDA_OK(cudaSetDevice(device));
-    CUDA_OK(cudaMemset2DAsync(d_app + AP_XFRC, sizeof(real) * APPLIED_W, 0, sizeof(real) * AP_QFRC, n, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaMemset2DAsync(row(R_APP) + AP_XFRC, sizeof(real) * APPLIED_W, 0, sizeof(real) * AP_QFRC, n, stream)); CUDA_OK(cudaStreamSynchronize(stream));
     return true;
   }
-  // ---- per-tick trace: the rows are an output, written by step launches only.  The trace instances are the F_TC twins of the chain twins, so a batch
-  // with a trace carries applied-force rows (zero when it has none: tc_app) and, through them, model-valued contact, mechanics, actuator and offset rows
-  // (xf_ct); they are allocated here, so that a step allocates nothing, and dropped again with the trace unless a verb has written them since
-  bool chain_twin_rows() {
-    if (!d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }
-    if (!A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }
-    return true;
-  }
+  // ---- per-tick trace: the rows are an output, written by step launches only.  The trace instances are twins of the extended chain twins: the rows they
+  // need are lent here (env_rows.h), so that a step allocates nothing
   bool set_trace(const int *source, const int *column, int k, int max_ticks) override {
     const std::string verb = "cassie_batch_set_trace: ";
     if (legacy) { set_err(verb + "the batch belongs to a cassie_sim_t"); return false; }
@@ -1571,11 +1479,8 @@ template <typename real> struct Batch : BatchBase {
     }
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight writes the rows
     CUDA_OK(cudaFree(A.trace.rows)); CUDA_OK(cudaFree((void *)A.trace.cols)); A.trace = TraceArgs<real>{}; tc_ticks = 0;
-    if (k == 0) {   // back to the instances that ran before
-      if (tc_app) { tc_app = false; return enable_applied_forces(false); }
-      return true;
-    }
-    if (!chain_twin_rows()) return false;
+    if (k == 0) return rows_rule(dropped, R_TRACE);   // back to the instances that ran before
+    if (!rows_rule(own, R_TRACE)) return false;
     int *cols = nullptr;
     CUDA_OK(cudaMalloc(&cols, sizeof(int) * k)); CUDA_OK(cudaMemcpy(cols, codes.data(), sizeof(int) * k, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMalloc(&A.trace.rows, sizeof(real) * n * max_ticks * k)); CUDA_OK(cudaMemset(A.trace.rows, 0, sizeof(real) * n * max_ticks * k));
@@ -1588,15 +1493,14 @@ template <typename real> struct Batch : BatchBase {
     return d2h(A.trace.rows, A.trace.T * A.trace.k, A.trace.T * A.trace.k, 0, out);
   }
   int trace_ticks() const override { return tc_ticks; }
-  // ---- contact lists: the rows are an output, written by step and forward launches only.  The contact-list instances are the F_CL twins of the F_FR
-  // chain twins, so the batch carries applied-force and contact rows as with a trace (chain_twin_rows), dropped again with the lists unless a verb has
-  // written them since
+  // ---- contact lists: the rows are an output, written by step and forward launches only.  The contact-list instances are twins of the F_FR chain
+  // twins: the rows they need are lent as with a trace
   bool enable_contacts(bool on) override {
     if (on && A.trace.rows) { set_err("cassie_batch_enable_contacts: the batch has a per-tick trace (cassie_batch_set_trace); a trace and contact lists do not combine"); return false; }
     if (on && A.sn.rows) { set_err("cassie_batch_enable_contacts: the batch has sensor models (cassie_batch_set_env_sensors); contact lists and sensor models do not combine"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (on && !A.cl.rows) {
-      if (!chain_twin_rows() || !geom_table()) return false;
+      if (!rows_rule(own, R_CL) || !geom_table()) return false;
       real *rows = nullptr;
       CUDA_OK(cudaMalloc(&rows, sizeof(real) * n * CON_W)); CUDA_OK(cudaMemset(rows, 0, sizeof(real) * n * CON_W));
       A.cl.rows = rows; A.cl.geom = d_gtab;
@@ -1604,13 +1508,13 @@ template <typename real> struct Batch : BatchBase {
     if (!on && A.cl.rows) {
       CUDA_OK(cudaStreamSynchronize(stream));   // a launch in flight writes the rows
       CUDA_OK(cudaFree(A.cl.rows)); A.cl = ContactListArgs<real>{};   // (the geom table stays with the batch)
-      if (tc_app) { tc_app = false; return enable_applied_forces(false); }   // back to the instances that ran before
+      return rows_rule(dropped, R_CL);   // back to the instances that ran before
     }
     return true;
   }
   // ---- sensor models: a model input like the actuator rows, read by the controller stage of every step tick.  The device rows are what the environments
   // run with (a write through the device pointer takes effect at the next launch), so the verbs read them back and keep no mirror.  The sensor
-  // instances are the F_SN twins of the applied-force instances, so the batch carries applied-force rows (zero when it has none: tc_app)
+  // instances are twins of the applied-force instances (env_rows.h)
   bool alloc_sensors() {   // zero rows with the identity mount, generator rows seeded as seed_sensors(0, all)
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     std::vector<real> rows((size_t)n * SN_W, real(0)); std::vector<int> rng((size_t)n * SR_W, 0);
@@ -1619,8 +1523,7 @@ template <typename real> struct Batch : BatchBase {
     CUDA_OK(cudaMalloc(&r, sizeof(real) * n * SN_W)); CUDA_OK(cudaMalloc(&g, sizeof(int) * n * SR_W));
     A.sn.rows = r; A.sn.rng = g;
     CUDA_OK(cudaMemcpy(r, rows.data(), sizeof(real) * n * SN_W, cudaMemcpyHostToDevice)); CUDA_OK(cudaMemcpy(g, rng.data(), sizeof(int) * n * SR_W, cudaMemcpyHostToDevice));
-    if (!d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }
-    return true;
+    return rows_rule(own, R_SN);
   }
   bool set_env_sensors(const double *enc_offset, const double *enc_noise, const double *imu_quat, const double *imu_bias, const double *imu_noise, const unsigned char *mask) override {
     const std::string verb = "cassie_batch_set_env_sensors: ";
@@ -1674,8 +1577,7 @@ template <typename real> struct Batch : BatchBase {
     if (!A.sn.rows) return true;
     CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
     CUDA_OK(cudaFree((void *)A.sn.rows)); CUDA_OK(cudaFree(A.sn.rng)); A.sn = SensorArgs<real>{};
-    if (tc_app) { tc_app = false; return enable_applied_forces(false); }
-    return true;
+    return rows_rule(dropped, R_SN);
   }
   bool seed_sensors(unsigned long long seed, const unsigned char *mask) override {
     if (!A.sn.rows) { set_err("cassie_batch_seed_sensors: no sensor models (cassie_batch_set_env_sensors)"); return false; }
@@ -1891,7 +1793,7 @@ template <typename real> struct Batch : BatchBase {
     if (!nray) { set_err("cassie_batch_raycast: no rays are set (cassie_batch_set_rays)"); return false; }
     CUDA_OK(cudaSetDevice(device));
     if (!d_rays) CUDA_OK(cudaMalloc(&d_rays, sizeof(real) * n * nray * RAY_SLOT));
-    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride; R.terrain = d_terrain; R.bpos = d_bpos;
+    RayArgs<real> R; R.model = d_model; R.qpos = A.qpos; R.qpos_w = QW; R.genv = d_genv; R.hfield = A.hfield; R.n_terrain = A.n_terrain; R.hfield_stride = A.hfield_stride; R.terrain = d_terrain; R.bpos = A.bpos;
     R.tab = d_rtab; R.k = nray; R.out = d_rays; R.n = n;
     CUDA_OK(launch_raycast<real>(R, device, stream));
     launches++; rays_done = true;
@@ -1934,14 +1836,14 @@ template <typename real> struct Batch : BatchBase {
       for (int i = 0; i < 4; i++) mt[c].quat[i] = (real)cam.quat[c][i];
     }
     if (cam.k == 1 && !d_camenv && !cam_geoms) {   // one camera, nothing per environment: the one-camera kernel (DESIGN.md section 5)
-      CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = d_bpos;
+      CamArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = A.bpos;
       C.body = mt[0].body; C.width = cam.width; C.height = cam.height; C.tan_half = mt[0].tan_half; C.zfar = (real)cam.zfar;
       for (int i = 0; i < 3; i++) C.pos[i] = mt[0].pos[i];
       for (int i = 0; i < 4; i++) C.quat[i] = mt[0].quat[i];
       C.out = d_depth; C.n = n;
       CUDA_OK(launch_camera<real>(C, device, stream));
     } else {
-      CamSetArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = d_bpos;
+      CamSetArgs<real> C; C.model = d_model; C.qpos = A.qpos; C.qpos_w = QW; C.genv = d_genv; C.hfield = A.hfield; C.n_terrain = A.n_terrain; C.hfield_stride = A.hfield_stride; C.terrain = d_terrain; C.bpos = A.bpos;
       C.k = cam.k; C.width = cam.width; C.height = cam.height; C.zfar = (real)cam.zfar;
       for (int c = 0; c < CAM_MAX; c++) C.cam[c] = mt[c < cam.k ? c : 0];
       C.out = d_depth; C.n = n; C.cenv = d_camenv; C.geom = cam_geoms ? d_camgeom : nullptr; C.gtab = d_gtab;
@@ -2077,9 +1979,7 @@ template <typename real> struct Batch : BatchBase {
     if (mode == 6 && !d_iq) { set_err("the inverse launch needs its rows (cassie_batch_inverse)"); return false; }
     A.nsub = nsub_override;
     const int ext = launch_kind(mode);
-    if ((A.trace.rows || A.cl.rows) && !chain_twin_rows()) return false;   // only after a verb dropped the rows set_trace / enable_contacts allocated
-    if (A.sn.rows && !d_app) { if (!enable_applied_forces(true)) return false; tc_app = true; }   // likewise the applied rows of set_env_sensors
-    if (A.applied && ext == 1 && !A.contact) { if (!set_env_contact(nullptr, nullptr, nullptr, nullptr)) return false; xf_ct = true; }   // the chain twin reads contact rows (the model's values when none were set)
+    if (!rows_rule(lend_for_launch, ext)) return false;   // rows a verb dropped since their holder's set, and the extended chain twins' contact rows
     A.warp_stride = (int)warp_bytes<real>(A.ystride, ext == 1);
     const LaunchCfg &c = cfg[ext];
     int grid = (count + c.wpb - 1) / c.wpb; if (grid > c.resident_ctas) grid = c.resident_ctas;
@@ -2158,8 +2058,8 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "qpos")) return A.qpos; if (!strcmp(f, "qvel")) return A.qvel; if (!strcmp(f, "pd")) return A.pd; if (!strcmp(f, "obs")) return A.obs;
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
-    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "camera_env")) return d_camenv; if (!strcmp(f, "camera_geom")) return d_camgeom; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return d_act; if (!strcmp(f, "mechanics")) return d_mech; if (!strcmp(f, "contact")) return d_ct;
-    if (!strcmp(f, "applied")) return d_app; if (!strcmp(f, "loops")) return d_loops;
+    if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "camera_env")) return d_camenv; if (!strcmp(f, "camera_geom")) return d_camgeom; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return row(R_ACT); if (!strcmp(f, "mechanics")) return row(R_MECH); if (!strcmp(f, "contact")) return row(R_CT);
+    if (!strcmp(f, "applied")) return row(R_APP); if (!strcmp(f, "loops")) return d_loops;
     if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
     if (!strcmp(f, "contacts")) return A.cl.rows;
