@@ -19,6 +19,8 @@ NU = 10   # motors: every supported model has Cassie's ten (csrc/devmodel.h MU),
 PD_WIDTH, OBS_WIDTH, AUX_WIDTH, EST_WIDTH = 52, 112, 64, 16
 # one frame's slot of a frame row (CASSIE_FRAME_* in include/cassie_b200.h) and the frame kinds of set_frames
 FRAME_WIDTH, FRAME_BODY, FRAME_SITE, FRAME_MAX = 20, 0, 1, 64
+IK_MAX, IK_TARGET_WIDTH, IK_SLOT, IK_WORLD, IK_ROOT = 4, 16, 8, 0, 1   # include/cassie_b200.h CASSIE_IK_*
+IK_STATUS = ('pos_residual', 'ori_residual', 'loop_residual', 'iterations', 'outcome', 'jeq_qvel', 'vel_residual', 'at_bound')
 FRAME = dict(pos=slice(0, 3), quat=slice(3, 7), vel=slice(7, 13), cfrc=slice(13, 19))
 # dynamics row (include/cassie_b200.h CASSIE_DYN_*): M [40][40], bias [40], connect rows [12][40], their errors [12], centre-of-mass offset [3]
 DYN_WIDTH, DYN_COLS = 2144, 40
@@ -1340,6 +1342,53 @@ class CassieBatch:
             raise RuntimeError(_last_error())
         return out
 
+    # ---- inverse kinematics: free coordinates posed to per-environment frame targets (rules in include/cassie_b200.h, DESIGN.md section 3)
+    IK_TOL = {FP64: 1e-10, FP32: 1e-5}    # metres and radians: fp32 kinematics reaches ~1e-6 at best; fp64 reaches 1e-10 in 4-6 steps from a standing pose
+
+    def set_ik(self, names, kinds, frames=None, weights=None):
+        """the target list (at most IK_MAX): body or site names with kinds FRAME_BODY / FRAME_SITE, frames IK_WORLD / IK_ROOT (None: all world), weights
+        [k][6] for the position rows x, y, z and the orientation rows about the target's x, y, z (None: all 1; 0 drops a row).  [] drops the list.  It
+        allocates the target rows torch_view('ik_targets') [n, IK_MAX, 16] (position 3, quaternion 4, linear velocity 3, angular velocity 3, pad) and the
+        status rows torch_view('ik') [n, 8], zero"""
+        names = list(names)
+        k = len(names)
+        kinds = [int(x) for x in kinds]
+        frames = [IK_WORLD] * k if frames is None else [int(x) for x in frames]
+        w = np.ones((k, 6)) if weights is None else np.array(weights, dtype=np.float64).reshape(k, 6)
+        if len(kinds) != k or len(frames) != k:
+            raise ValueError('one kind and one frame per target name')
+        arr = (C.c_char_p * max(1, k))(*[n.encode() for n in names])
+        ks, fs = (C.c_int * max(1, k))(*kinds), (C.c_int * max(1, k))(*frames)
+        w = np.ascontiguousarray(w)
+        self.L.cassie_batch_set_ik.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_int]
+        if self.L.cassie_batch_set_ik(self.h, arr, ks, fs, self._dp(w), k) != 0:
+            raise RuntimeError(_last_error())
+
+    def solve_ik(self, mask=None, max_iter=100, tol=None, velocities=False):
+        """pose the environments with mask[e] set (CUDA bool / uint8 tensor [n]; None: every environment) to their rows of torch_view('ik_targets'):
+        Levenberg-Marquardt steps on the free coordinates (motors and the loops' passive joints) from the current qpos, loops closed and joint ranges
+        held, until every weighted row is within tol (None: IK_TOL of the precision) or the steps stall or max_iter runs out; velocities=True also fits
+        the free qvel to the rows' velocities.  One launch on the batch's stream, capturable in a CUDA graph; it writes qpos, qvel and ik_status() only:
+        follow it with forward_where(mask)"""
+        L = self.L
+        L.cassie_batch_solve_ik.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_double, C.c_int]
+        mp = None if mask is None else C.c_void_p(self._mask_ptr(mask, 'mask'))
+        if L.cassie_batch_solve_ik(self.h, mp, int(max_iter), float(self.IK_TOL[self.precision] if tol is None else tol), 1 if velocities else 0) != 0:
+            raise RuntimeError(_last_error())
+
+    def ik_status(self):
+        """the status rows of the last solve_ik as numpy arrays [n], named as IK_STATUS: pos_residual (m), ori_residual (rad), loop_residual (m),
+        iterations, outcome (1 reached, 2 best effort, -1 kept), jeq_qvel (max |J_eq qvel|), vel_residual, at_bound (free joints at a range bound);
+        environments outside the last mask keep their values (zero before their first selection)"""
+        st = np.zeros((self.n, IK_SLOT))
+        self.L.cassie_batch_get_ik_status.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        if self.L.cassie_batch_get_ik_status(self.h, self._dp(st)) != 0:
+            raise RuntimeError(_last_error())
+        out = {k: st[:, i].copy() for i, k in enumerate(IK_STATUS)}
+        for k in ('iterations', 'outcome', 'at_bound'):
+            out[k] = out[k].astype(np.int32)
+        return out
+
     def set_timestep(self, dt):
         self.L.cassie_batch_set_timestep.argtypes = [C.c_void_p, C.c_double]
         if self.L.cassie_batch_set_timestep(self.h, float(dt)) != 0:
@@ -1384,7 +1433,8 @@ class CassieBatch:
         per-environment camera mounts pos[3], quat[4], fovy in degrees, read at the next render; set_env_cameras first; camera_geom [n, k, height, width]
         int32 (shaped as depth for set_camera): the geom ids of the last render; enable_camera_geoms and render_depth first; sensors [n, 52] laid out as
         SN, read at the next launch; sensor_rng [n, 4] int32: key lo, hi, counter lo, hi; set_env_sensors first for both; loops [n, 4]: the status
-        rows of close_loops -- residual, iterations, max |J qvel|, pad; close_loops first).  set_frames /
+        rows of close_loops -- residual, iterations, max |J qvel|, pad; close_loops first; ik_targets [n, IK_MAX, 16]: the targets of solve_ik, written by
+        the caller; ik [n, 8]: its status rows laid out as IK_STATUS; set_ik first for both).  set_frames /
         set_rays / set_camera reallocate the frame, acceleration, ray and depth rows: a view taken before them must not be used after them.  The dynamics rows stay put once compute_dynamics() has allocated them.
 
         The arrays are written on the batch's stream.  Unless that stream is torch's current stream (set_stream(torch.cuda.current_stream().cuda_stream)),
@@ -1394,7 +1444,7 @@ class CassieBatch:
         width = self.L.cassie_batch_row_width(self.h, field.encode())
         ptr = self.device_ptr(field)
         if width <= 0 or not ptr:
-            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first; sensors, sensor_rng: set_env_sensors first; loops: close_loops first)' % field)
+            raise RuntimeError('no device rows for %r (frames: set_frames first; frame_jac: frame_jacobian first; dyn: compute_dynamics first; rays: raycast first; acc: enable_accelerations first; depth: render_depth first; terrain: set_env_hfield first; actuators: set_env_actuators first; mechanics: set_env_mechanics first; contact: set_env_contact first; applied: enable_applied_forces first; trace: set_trace first; contacts: enable_contacts first; camera_env: set_env_cameras first; camera_geom: enable_camera_geoms and render_depth first; sensors, sensor_rng: set_env_sensors first; loops: close_loops first; ik_targets, ik: set_ik first)' % field)
         dt, isz, ts = (np.float32, 4, '<f4') if self.precision == FP32 else (np.float64, 8, '<f8')
         if field in ('terrain', 'camera_geom', 'sensor_rng'):
             ts = '<i4'
@@ -1410,6 +1460,8 @@ class CassieBatch:
             return t.view(self.n, *self._trace_shape)
         if field == 'camera_env':
             return t.view(self.n, -1, CAMENV_SLOT)
+        if field == 'ik_targets':
+            return t.view(self.n, IK_MAX, IK_TARGET_WIDTH)
         return t.view(self.n, *self._cam_shape) if field in ('depth', 'camera_geom') else t
 
 

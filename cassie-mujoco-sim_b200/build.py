@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, '_obj')
 LIB = os.path.join(HERE, 'libcassie_b200.so')
 DEPS = [os.path.join(CSRC, f) for f in ('cassie_b200.cu', 'mjcf.cpp', 'step_inst.cu', 'step_kernel.cuh', 'step_core.inl', 'cassie_tree_gen.inc', 'devmodel.h', 'devbuild.h', 'model.h',
-                                        'estimator_host.h', 'legacy_stubs.inc', 'step_instances.inc', 'step_select.h', 'env_rows.h', 'raycast.cu', 'raycast.inl', 'camera.cu', 'camera.inl', 'camera_set.cu', 'camera_set.inl', 'reset.cu', 'reset.inl', 'loops.cu', 'loops.inl')] + [
+                                        'estimator_host.h', 'legacy_stubs.inc', 'step_instances.inc', 'step_select.h', 'env_rows.h', 'raycast.cu', 'raycast.inl', 'camera.cu', 'camera.inl', 'camera_set.cu', 'camera_set.inl', 'reset.cu', 'reset.inl', 'loops.cu', 'loops.inl', 'ik.cu', 'ik.inl')] + [
     os.path.join(HERE, '..', 'include', 'cassie_b200.h'), os.path.join(HERE, '..', 'include', 'cassie_bus.h')]
 # (tag, real, kind: 0 plain / 1 extended / 2 plain + estimator, feature bits csrc/devmodel.h F_*) of every step instance, from the tags of
 # csrc/step_instances.inc: <f|d><kind digit><feature bits in hex>
@@ -51,10 +51,10 @@ def _run(cmd, verbose, res=None):
 
 
 def res_path(obj):
-    """the resource report written beside a step instance's, the ray kernel's, a camera kernel's, the restore kernel's or the loop-closure kernel's object
-    file, or None for the other objects."""
+    """the resource report written beside a step instance's, the ray kernel's, a camera kernel's, the restore kernel's, the loop-closure kernel's or the
+    inverse-kinematics kernel's object file, or None for the other objects."""
     name = os.path.basename(obj)
-    return obj[:-2] + '.res' if name.startswith(('step_', 'ray_', 'cam_', 'camset_', 'reset_', 'loops_')) and name.endswith('.o') else None
+    return obj[:-2] + '.res' if name.startswith(('step_', 'ray_', 'cam_', 'camset_', 'reset_', 'loops_', 'ik_')) and name.endswith('.o') else None
 
 
 def build(force=False, verbose=False, out=None):
@@ -78,6 +78,8 @@ def build(force=False, verbose=False, out=None):
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DRESET_REAL=' + real, '-c', os.path.join(CSRC, 'reset.cu'), '-o', os.path.join(OBJ, 'reset_%s.o' % real)])
     for real in ('float', 'double'):   # the loop-closure kernel, likewise; its report is kept as loops_<real>.res (tests/test_loops_resources.py)
         jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DLOOPS_REAL=' + real, '-c', os.path.join(CSRC, 'loops.cu'), '-o', os.path.join(OBJ, 'loops_%s.o' % real)])
+    for real in ('float', 'double'):   # the inverse-kinematics kernel, likewise; its report is kept as ik_<real>.res (tests/test_ik_resources.py)
+        jobs.append([nvcc()] + ARCH + ['-Xptxas', '-v', '-DIK_REAL=' + real, '-c', os.path.join(CSRC, 'ik.cu'), '-o', os.path.join(OBJ, 'ik_%s.o' % real)])
     with ThreadPoolExecutor(max_workers=max(2, min(len(jobs), (os.cpu_count() or 4)))) as ex:
         logs = list(ex.map(lambda c: _run(c, verbose, res_path(c[-1])), jobs))
     if verbose:

@@ -26,6 +26,7 @@
 #include "camera_set.inl"
 #include "reset.inl"
 #include "loops.inl"
+#include "ik.inl"
 
 // the step-kernel instances live in their own translation units (step_inst.cu, one compilation per line of step_instances.inc)
 #define STEP_INSTANCE(tag) extern "C" const void *cassie_step_entry_##tag(void);
@@ -39,6 +40,7 @@ template <typename real> cudaError_t launch_camera(const CamArgs<real> &A, int d
 template <typename real> cudaError_t launch_camera_set(const CamSetArgs<real> &A, int device, cudaStream_t stream);   // camera_set.cu
 template <typename real> cudaError_t launch_reset(const ResetArgs &A, int device, cudaStream_t stream);       // reset.cu
 template <typename real> cudaError_t launch_loops(const LoopArgs<real> &A, int device, cudaStream_t stream);   // loops.cu
+template <typename real> cudaError_t launch_ik(const IkArgs<real> &A, int device, cudaStream_t stream);         // ik.cu
 
 static constexpr StepInstance STEP_INSTANCES[] = {
 #define STEP_INSTANCE(tag) step_instance(#tag, cassie_step_entry_##tag),
@@ -258,6 +260,11 @@ struct BatchBase {
   // first call allocates the status rows [n][LOOP_SLOT].  get_loop_status copies them; any pointer may be null
   virtual bool close_loops(const void *d_mask, int max_iter, double tol) = 0;
   virtual bool get_loop_status(double *residual, int *iterations, double *vel_residual) = 0;
+  // inverse kinematics (ik.inl): set_ik allocates the target and status rows (count 0 frees them); solve_ik is one launch on the batch's stream;
+  // get_ik_status copies the status rows [n][IK_SLOT]
+  virtual bool set_ik(const char *const *names, const int *kinds, const int *frames, const double *weights, int count) = 0;
+  virtual bool solve_ik(const void *d_mask, int max_iter, double tol, int velocities) = 0;
+  virtual bool get_ik_status(double *status) = 0;
   bool legacy = false;   // the batch of a cassie_sim_t: its host mirrors are pushed before every launch, so device-side resets are refused
   virtual bool copy_model_from(BatchBase *src) = 0;     // per-environment constants, height fields, timestep (mj_copyModel in cassie_sim_copy, :1083-1091)
   virtual bool rebuild_model() = 0;                     // after hm was edited (timestep, hold / release): rebuild and upload the constant block
@@ -404,10 +411,13 @@ template <typename real> struct Batch : BatchBase {
   int tc_ticks = 0;                        // slots the last step launch wrote into the trace rows (A.trace: [n][T][k], allocated by cassie_batch_set_trace)
   Snap *bank = nullptr;                    // the reset bank (cassie_batch_set_reset_bank): a snapshot of k entries
   real *d_loops = nullptr;                 // [n][LOOP_SLOT] status rows of cassie_batch_close_loops, allocated (zero) by its first call
+  real *d_ikt = nullptr, *d_ik = nullptr;  // [n][IK_MAX][IK_TW] target rows and [n][IK_SLOT] status rows of the IK target list (cassie_batch_set_ik)
+  int ik_n = 0;                            // the list: its targets' bodies, frames, poses in their bodies and weights
+  std::vector<int> ik_body, ik_frame; std::vector<double> ik_pos, ik_quat, ik_w;
   ~Batch() override {
     snap_delete(bank);
     cudaSetDevice(device);
-    cudaFree(d_loops); cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); for (int b = 0; b <= R_APP; b++) cudaFree(row(b)); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
+    cudaFree(d_ik); cudaFree(d_ikt); cudaFree(d_loops); cudaFree(d_rtab); cudaFree(d_rays); cudaFree(d_depth); cudaFree(d_camgeom); cudaFree(d_camenv); cudaFree(d_gtab); cudaFree(d_genv); cudaFree(d_terrain); for (int b = 0; b <= R_APP; b++) cudaFree(row(b)); cudaFree(A.trace.rows); cudaFree((void *)A.trace.cols); cudaFree(A.cl.rows); cudaFree((void *)A.sn.rows); cudaFree(A.sn.rng); cudaFree(A.frames); cudaFree((void *)A.ftab); cudaFree(A.jac); cudaFree(A.dyn); cudaFree(A.acc); cudaFree(A.inv); cudaFree(d_iq); cudaFree(d_idbg); cudaFree(d_icst); cudaFree(d_icnt);
     cudaFree(d_model); cudaFree(A.qpos); cudaFree(A.qvel); cudaFree(A.qacc_ws); cudaFree(A.cst); cudaFree(A.pd); cudaFree(A.xfrc); cudaFree(A.obs); cudaFree(A.dbg);
     cudaFree(A.dfilt); cudaFree(A.counters); cudaFree(A.qM); cudaFree(A.ticket); cudaFree(A.aux); cudaFree(A.task); cudaFree(A.gait); cudaFree(A.est); if (pin_task) cudaFreeHost(pin_task); cudaFree(d_mask); cudaFree(d_row);
     for (int i = 0; i < AOS_MAXC; i++) { if (aos_done[i]) cudaEventDestroy(aos_done[i]); if (aos_stream[i]) cudaStreamDestroy(aos_stream[i]); } if (aos_start) cudaEventDestroy(aos_start);
@@ -954,6 +964,60 @@ template <typename real> struct Batch : BatchBase {
       if (iterations) iterations[e] = (int)r[1];
       if (vel_residual) vel_residual[e] = (double)r[2];
     }
+    return true;
+  }
+  bool set_ik(const char *const *names, const int *kinds, const int *frames, const double *weights, int count) override {
+    const std::string verb = "cassie_batch_set_ik";
+    if (count < 0 || count > IK_MAX || (count > 0 && (!names || !kinds || !weights))) { set_err(verb + ": between 0 and " + std::to_string(IK_MAX) + " targets, with names, kinds and weights"); return false; }
+    if (legacy) { set_err(verb + ": the batch belongs to a cassie_sim_t, whose host mirrors would overwrite the solved state"); return false; }
+    std::vector<int> body(count), frame(count); std::vector<double> pos(3 * count), quat(4 * count), w;
+    if (count > 0) w.assign(weights, weights + 6 * count);
+    for (int t = 0; t < count; t++) {
+      double row[FT_W]; std::string err;
+      if (frame_table_row(hm, names[t], kinds[t], row, err) < 0) { set_err(verb + ": " + err); return false; }
+      body[t] = (int)row[FT_BODY]; frame[t] = frames ? frames[t] : IK_WORLD;
+      if (frame[t] != IK_WORLD && frame[t] != IK_ROOT) { set_err(verb + ": target " + std::to_string(t) + ": frame must be CASSIE_IK_WORLD or CASSIE_IK_ROOT"); return false; }
+      for (int c = 0; c < 3; c++) pos[3 * t + c] = row[FT_POS + c];
+      for (int c = 0; c < 4; c++) quat[4 * t + c] = row[FT_QUAT + c];
+      bool any = false;
+      for (int c = 0; c < 6; c++) { const double x = w[6 * t + c]; if (!(x >= 0) || !std::isfinite(x)) { set_err(verb + ": target " + std::to_string(t) + ": weights must be finite and >= 0"); return false; } any |= x > 0; }
+      if (!any) { set_err(verb + ": target " + std::to_string(t) + ": every weight is zero"); return false; }
+    }
+    IkTable<real> I; std::string err;
+    if (count > 0 && !ik_table<real>(hm, count, body.data(), frame.data(), pos.data(), quat.data(), w.data(), I, err)) { set_err(verb + ": " + err); return false; }
+    CUDA_OK(cudaSetDevice(device)); CUDA_OK(cudaStreamSynchronize(stream));
+    CUDA_OK(cudaFree(d_ikt)); CUDA_OK(cudaFree(d_ik)); d_ikt = d_ik = nullptr; ik_n = 0;
+    if (count > 0) {
+      CUDA_OK(cudaMalloc(&d_ikt, sizeof(real) * n * IK_MAX * IK_TW)); CUDA_OK(cudaMemset(d_ikt, 0, sizeof(real) * n * IK_MAX * IK_TW));
+      CUDA_OK(cudaMalloc(&d_ik, sizeof(real) * n * IK_SLOT)); CUDA_OK(cudaMemset(d_ik, 0, sizeof(real) * n * IK_SLOT));
+      ik_n = count; ik_body = body; ik_frame = frame; ik_pos = pos; ik_quat = quat; ik_w = w;
+    }
+    return true;
+  }
+  bool solve_ik(const void *d_mask, int max_iter, double tol, int velocities) override {
+    const std::string verb = "cassie_batch_solve_ik";
+    if (legacy) { set_err(verb + ": the batch belongs to a cassie_sim_t, whose host mirrors would overwrite the solved state"); return false; }
+    if (!ik_n) { set_err(verb + ": no target list (cassie_batch_set_ik)"); return false; }
+    if (d_mask && !device_rows(d_mask, verb.c_str(), "the mask")) return false;
+    if (max_iter < 1 || max_iter > IK_MAX_ITER) { set_err(verb + ": max_iter must be between 1 and " + std::to_string(IK_MAX_ITER)); return false; }
+    if (!(tol > 0) || !std::isfinite(tol)) { set_err(verb + ": tol must be finite and > 0"); return false; }
+    if (velocities != 0 && velocities != 1) { set_err(verb + ": velocities must be 0 or 1"); return false; }
+    IkArgs<real> K; std::string err;
+    if (!ik_table<real>(hm, ik_n, ik_body.data(), ik_frame.data(), ik_pos.data(), ik_quat.data(), ik_w.data(), K.I, err)) { set_err(verb + ": " + err); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    K.model = d_model; K.qpos = A.qpos; K.qpos_w = QW; K.qvel = A.qvel; K.qvel_w = VW; K.bpos = A.bpos; K.targets = d_ikt; K.status = d_ik;
+    K.mask = (const unsigned char *)d_mask; K.n = n; K.max_iter = max_iter; K.velocities = velocities; K.tol = (real)tol;
+    K.loop_tol = (real)std::min(tol, sizeof(real) == sizeof(float) ? IK_LOOP_TOL_F : IK_LOOP_TOL_D);
+    CUDA_OK(launch_ik<real>(K, device, stream));
+    launches++;
+    return true;
+  }
+  bool get_ik_status(double *status) override {
+    if (!d_ik) { set_err("cassie_batch_get_ik_status: no target list (cassie_batch_set_ik)"); return false; }
+    CUDA_OK(cudaSetDevice(device));
+    h_tmp.resize((size_t)n * IK_SLOT);
+    CUDA_OK(cudaMemcpyAsync(h_tmp.data(), d_ik, sizeof(real) * n * IK_SLOT, cudaMemcpyDeviceToHost, stream)); CUDA_OK(cudaStreamSynchronize(stream));
+    for (size_t i = 0; i < (size_t)n * IK_SLOT; i++) status[i] = (double)h_tmp[i];
     return true;
   }
   bool rebuild_model() override {
@@ -2059,7 +2123,7 @@ template <typename real> struct Batch : BatchBase {
     if (!strcmp(f, "xfrc")) return A.xfrc; if (!strcmp(f, "cst")) return A.cst; if (!strcmp(f, "qacc_ws")) return A.qacc_ws; if (!strcmp(f, "aux")) return A.aux; if (!strcmp(f, "task")) return A.task;
     if (!strcmp(f, "frames")) return A.frames; if (!strcmp(f, "frame_jac")) return A.jac; if (!strcmp(f, "dyn")) return A.dyn; if (!strcmp(f, "acc")) return A.acc;
     if (!strcmp(f, "rays")) return d_rays; if (!strcmp(f, "depth")) return d_depth; if (!strcmp(f, "camera_env")) return d_camenv; if (!strcmp(f, "camera_geom")) return d_camgeom; if (!strcmp(f, "terrain")) return d_terrain; if (!strcmp(f, "actuators")) return row(R_ACT); if (!strcmp(f, "mechanics")) return row(R_MECH); if (!strcmp(f, "contact")) return row(R_CT);
-    if (!strcmp(f, "applied")) return row(R_APP); if (!strcmp(f, "loops")) return d_loops;
+    if (!strcmp(f, "applied")) return row(R_APP); if (!strcmp(f, "loops")) return d_loops; if (!strcmp(f, "ik_targets")) return d_ikt; if (!strcmp(f, "ik")) return d_ik;
     if (!strcmp(f, "inv_qacc") || !strcmp(f, "inv")) { if (!alloc_inverse()) return nullptr; return !strcmp(f, "inv") ? A.inv : d_iq; }
     if (!strcmp(f, "trace")) return A.trace.rows;
     if (!strcmp(f, "contacts")) return A.cl.rows;
@@ -2095,6 +2159,10 @@ static_assert(CASSIE_FRAME_JAC_WIDTH == FRAME_JAC_W && CASSIE_FRAME_JAC_COLS == 
 static_assert(CASSIE_DYN_WIDTH == DYN_W && CASSIE_DYN_COLS == DY_COLS && CASSIE_DYN_M == DY_M && CASSIE_DYN_BIAS == DY_BIAS && CASSIE_DYN_JEQ == DY_JEQ && CASSIE_DYN_EQPOS == DY_EQPOS && CASSIE_DYN_RCM == DY_RCM, "dynamics row layout");
 static_assert(CASSIE_INV_WIDTH == INV_W && CASSIE_INV_COLS == IV_COLS && CASSIE_INV_QFRC == IV_QFRC && CASSIE_INV_QFRCC == IV_QFRCC && CASSIE_INV_NEFC == IV_NEFC && CASSIE_INV_NCON == IV_NCON && CASSIE_INV_DROPPED == IV_DROPPED, "inverse row layout");
 static_assert(CASSIE_ACC_QACC == AC_QACC && CASSIE_ACC_QCOLS == AC_QCOLS && CASSIE_ACC_CACC == AC_CACC && CASSIE_ACC_SLOT == AC_SLOT && CASSIE_ACC_WIDTH(3) == acc_width(3), "acceleration row layout");
+static_assert(CASSIE_IK_MAX == IK_MAX && CASSIE_IK_TARGET_WIDTH == IK_TW && CASSIE_IK_SLOT == IK_SLOT && CASSIE_IK_MAX_ITER == IK_MAX_ITER && CASSIE_IK_WORLD == IK_WORLD && CASSIE_IK_ROOT == IK_ROOT &&
+              CASSIE_IK_POS == IT_POS && CASSIE_IK_QUAT == IT_QUAT && CASSIE_IK_VEL == IT_VEL && CASSIE_IK_ANGVEL == IT_ANGVEL && CASSIE_IK_POS_RESIDUAL == IS_POS && CASSIE_IK_ORI_RESIDUAL == IS_ORI &&
+              CASSIE_IK_LOOP_RESIDUAL == IS_LOOP && CASSIE_IK_ITERATIONS == IS_ITER && CASSIE_IK_OUTCOME == IS_OUTCOME && CASSIE_IK_JEQ_QVEL == IS_JV && CASSIE_IK_VEL_RESIDUAL == IS_VEL &&
+              CASSIE_IK_AT_BOUND == IS_BOUND, "inverse-kinematics rows");
 static_assert(CASSIE_LOOP_SLOT == LOOP_SLOT && CASSIE_LOOP_MAX_ITER == LOOP_MAX_ITER && CASSIE_LOOP_RESIDUAL == 0 && CASSIE_LOOP_ITERATIONS == 1 && CASSIE_LOOP_VEL_RESIDUAL == 2, "loop status rows");
 static_assert(CASSIE_APPLIED_WIDTH == APPLIED_W && CASSIE_APPLIED_XFRC == AP_XFRC && CASSIE_APPLIED_QFRC == AP_QFRC, "applied-force row layout");
 static_assert(CASSIE_SENSOR_WIDTH == SN_W && CASSIE_SN_ENC_OFF == SN_ENC_OFF && CASSIE_SN_ENC_STD == SN_ENC_STD && CASSIE_SN_QUAT == SN_QUAT && CASSIE_SN_ORI_STD == SN_ORI_STD && CASSIE_SN_GYRO_BIAS == SN_GYRO_BIAS && CASSIE_SN_GYRO_STD == SN_GYRO_STD && CASSIE_SN_ACC_BIAS == SN_ACC_BIAS && CASSIE_SN_ACC_STD == SN_ACC_STD, "sensor row layout");
@@ -2179,7 +2247,7 @@ int cassie_batch_row_width(const cassie_batch_t *b, const char *field) {
   if (!strcmp(field, "dyn")) return DYN_W; if (!strcmp(field, "rays")) return b->impl->nray * RAY_SLOT;
   if (!strcmp(field, "depth") || !strcmp(field, "camera_geom")) return b->impl->cam.k * b->impl->cam.width * b->impl->cam.height; if (!strcmp(field, "camera_env")) return b->impl->cam.k * CAMENV_SLOT; if (!strcmp(field, "terrain")) return 1; if (!strcmp(field, "actuators")) return ACT_W; if (!strcmp(field, "mechanics")) return MECH_W; if (!strcmp(field, "contact")) return CONTACT_W; if (!strcmp(field, "applied")) return APPLIED_W;
   if (!strcmp(field, "trace")) return b->impl->trace_width();
-  if (!strcmp(field, "contacts")) return CON_W; if (!strcmp(field, "loops")) return LOOP_SLOT;
+  if (!strcmp(field, "contacts")) return CON_W; if (!strcmp(field, "loops")) return LOOP_SLOT; if (!strcmp(field, "ik_targets")) return IK_MAX * IK_TW; if (!strcmp(field, "ik")) return IK_SLOT;
   if (!strcmp(field, "sensors")) return SN_W; if (!strcmp(field, "sensor_rng")) return SR_W;
   if (!strcmp(field, "inv_qacc")) return b->impl->hm.nv > 32 ? QVEL_W_XB : QVEL_W_MAIN; if (!strcmp(field, "inv")) return INV_W;
   if (!strcmp(field, "acc")) return acc_width((int)(b->impl->frame_list.size() / 2)); return -1;
@@ -2851,6 +2919,9 @@ int cassie_batch_reset_bank_size(const cassie_batch_t *b) { return b->impl->rese
 int cassie_batch_reset_where(cassie_batch_t *b, const void *d_mask, const void *d_entry) { return b->impl->reset_where(d_mask, d_entry) ? 0 : -1; }
 int cassie_batch_close_loops(cassie_batch_t *b, const void *d_mask, int max_iter, double tol) { return b->impl->close_loops(d_mask, max_iter, tol) ? 0 : -1; }
 int cassie_batch_get_loop_status(cassie_batch_t *b, double *residual, int *iterations, double *vel_residual) { return b->impl->get_loop_status(residual, iterations, vel_residual) ? 0 : -1; }
+int cassie_batch_set_ik(cassie_batch_t *b, const char *const *names, const int *kinds, const int *frames, const double *weights, int count) { return b->impl->set_ik(names, kinds, frames, weights, count) ? 0 : -1; }
+int cassie_batch_solve_ik(cassie_batch_t *b, const void *d_mask, int max_iter, double tol, int velocities) { return b->impl->solve_ik(d_mask, max_iter, tol, velocities) ? 0 : -1; }
+int cassie_batch_get_ik_status(cassie_batch_t *b, double *status) { return b->impl->get_ik_status(status) ? 0 : -1; }
 int cassie_batch_forward_where(cassie_batch_t *b, const void *d_mask) { return b->impl->forward_where(d_mask) ? 0 : -1; }
 #include "legacy_stubs.inc"
 }  // extern "C"

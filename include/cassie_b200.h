@@ -644,6 +644,65 @@ int cassie_batch_forward_where(cassie_batch_t *b, const void *d_mask);
 #define CASSIE_LOOP_VEL_RESIDUAL 2
 int cassie_batch_close_loops(cassie_batch_t *b, const void *d_mask, int max_iter, double tol);
 int cassie_batch_get_loop_status(cassie_batch_t *b, double *residual, int *iterations, double *vel_residual);
+/* Inverse kinematics (new): each selected environment's free coordinates posed so that up to CASSIE_IK_MAX body or site frames reach per-environment
+ * position and orientation targets, for resets onto terrain, reference motions given as foot poses and task-space targets.
+ *
+ * Rules that are ours:
+ * - Target list (per batch, shared by every environment): cassie_batch_set_ik(b, names, kinds, frames, weights, count).  kinds[i]: CASSIE_FRAME_BODY /
+ *   CASSIE_FRAME_SITE; frames[i]: CASSIE_IK_WORLD, or CASSIE_IK_ROOT for a target expressed in the root body's (the pelvis's) frame (NULL: all world);
+ *   weights[i][6] weight the position rows x, y, z (the expression frame's axes) and the orientation rows about the target frame's x, y, z; a weight of 0
+ *   drops its row (a Cassie foot: position plus pitch and yaw -- with the position fixed the leg cannot set all three angles).  The orientation error is
+ *   the rotation vector of R_target' R_frame, in the target's axes.  count 0 drops the list and its rows.  The call allocates the rows below (zero), so
+ *   a solve allocates nothing.  Refused: more than CASSIE_IK_MAX targets, an unknown name or kind, a frame other than the two, a negative or non-finite
+ *   weight, a target whose weights are all zero, a target on a body that no free coordinate moves (the pelvis, the extra free body), a connect equality
+ *   on the extra free body, the batch of a cassie_sim_t.
+ * - Free coordinates: the main-tree joints off the root body with zero jnt_stiffness -- the motors plus close_loops' free set, 22 columns for Cassie.
+ *   Everything else (the root joints, the shin and heel springs at their given deflection, the extra free body) and every unselected environment is
+ *   held bitwise.  The start point is the environment's qpos, which picks the branch (a knee forward); per-environment body offsets are honoured.
+ * - Positions: the loops are closed with close_loops' steps (motors held), then Levenberg-Marquardt steps run on the weighted task rows with the connect
+ *   rows held to first order; every limited free hinge or slide stays in its jnt_range by a projected step (a column at a bound whose step points
+ *   outward is dropped for that step); after each step the loops are re-closed, motors held, to min(tol, 1e-12 m) in fp64 / min(tol, 1e-6 m) in fp32;
+ *   a step is accepted only if the task residual sum (w e)^2 falls, else the damping grows tenfold and the step is retried.  The task residual thus
+ *   never rises above its value at the (closed) start.  The loop re-closing moves close_loops' own joints and does not hold their ranges.
+ * - Velocities (velocities = 0): the motors keep their qvel, the loops' passive joints are projected onto the loops as close_loops does.  (velocities =
+ *   1): one damped least-squares fit of the free qvel at the final pose, the connect rows held exactly, so that each target frame's linear velocity and
+ *   its angular velocity about the weighted axes match the target rows: world targets are world-frame velocities (the held pelvis motion included),
+ *   root targets velocities relative to the pelvis in its axes.
+ * - Outcome: 1 reached (position and orientation rows within tol, state written); 2 best effort (the target is out of reach or held by a range: the
+ *   steps stalled or max_iter ran out; the closest pose found is written, loops closed); -1 the start pose's loops could not be closed or a NaN appeared
+ *   (state kept).  The launch writes qpos, qvel and the status rows only: follow it with cassie_batch_forward_where(mask).
+ * - Snapshots, cassie_sim_copy, reset_where and the per-environment row blocks do not carry the target or status rows: they are a work area.
+ *
+ * cassie_batch_device_ptr(b, "ik_targets"): [n][CASSIE_IK_MAX][CASSIE_IK_TARGET_WIDTH] in the batch precision, written by the caller: position (3),
+ * quaternion (4, normalised on read), linear velocity (3), angular velocity (3, the expression frame's axes), pad.  "ik": the status rows
+ * [n][CASSIE_IK_SLOT]: position residual (m), orientation residual (rad) -- the largest error over the weighted rows --, loop residual (m),
+ * iterations, outcome, max |J_eq qvel| after the launch, velocity residual (the largest error over the weighted velocity rows; 0 for velocities = 0),
+ * the number of free joints at a bound.
+ * cassie_batch_solve_ik: d_mask is device uint8[n] (a torch.bool tensor as it is), NULL for every environment.  One launch on the batch's stream: no
+ * host synchronisation, copy or allocation, so it can be captured in a CUDA graph.  -1, with nothing enqueued, for no target list, a mask that is not
+ * device or managed memory of the batch's device, max_iter outside 1..CASSIE_IK_MAX_ITER, a tol (metres and radians) that is not finite and > 0,
+ * velocities other than 0 / 1, or the batch of a cassie_sim_t.  cassie_batch_get_ik_status: the status rows' synchronous host copy [n][CASSIE_IK_SLOT]. */
+#define CASSIE_IK_MAX 4
+#define CASSIE_IK_TARGET_WIDTH 16
+#define CASSIE_IK_SLOT 8
+#define CASSIE_IK_MAX_ITER 500
+#define CASSIE_IK_WORLD 0
+#define CASSIE_IK_ROOT 1
+#define CASSIE_IK_POS 0
+#define CASSIE_IK_QUAT 3
+#define CASSIE_IK_VEL 7
+#define CASSIE_IK_ANGVEL 10
+#define CASSIE_IK_POS_RESIDUAL 0
+#define CASSIE_IK_ORI_RESIDUAL 1
+#define CASSIE_IK_LOOP_RESIDUAL 2
+#define CASSIE_IK_ITERATIONS 3
+#define CASSIE_IK_OUTCOME 4
+#define CASSIE_IK_JEQ_QVEL 5
+#define CASSIE_IK_VEL_RESIDUAL 6
+#define CASSIE_IK_AT_BOUND 7
+int cassie_batch_set_ik(cassie_batch_t *b, const char *const *names, const int *kinds, const int *frames, const double *weights, int count);
+int cassie_batch_solve_ik(cassie_batch_t *b, const void *d_mask, int max_iter, double tol, int velocities);
+int cassie_batch_get_ik_status(cassie_batch_t *b, double *status);
 /* batched cassie_sim_apply_force / cassie_sim_clear_forces: xfrc [n][6]; one (wrench, body) slot per env, added to the applied-force rows
  * (cassie_batch_set_applied_forces) when the batch has them; clear_forces empties the slot and zeroes the rows' xfrc_applied, keeping qfrc_applied */
 int cassie_batch_apply_force(cassie_batch_t *b, const double *xfrc, const char *body_name);
